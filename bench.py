@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — the driver's benchmark contract for tensoir_b200.
+"""bench.py — the benchmark of tensoir_b200: prints one JSON result line.
 
 Step = one training step of the relight phase on one 4096-ray batch of the synthetic lego-shaped scene
 (BASELINE.json configs[1]: single light, 800x800 x 100 train views, full VM grid + BRDF MLPs):
@@ -24,6 +24,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import torch                      # noqa: E402
 import torch.distributed as dist  # noqa: E402
 
+H100_HBM_GBS = 3350.0      # HBM3 bandwidth of the H100 SXM data sheet; MEASURED_PEAKS.json overrides it
 METRIC = "primary+secondary rays/sec (800x800 lego-shaped synthetic, relight training step)"
 UNIT = "rays/s"
 
@@ -50,8 +51,9 @@ def parse():
     ap.add_argument("--envmap_w", type=int, default=None)
     ap.add_argument("--no-strong", dest="no_strong", action="store_true",
                     help="N > 1: skip the additional strong-scaling measurement")
-    ap.add_argument("--no-torch-reference", dest="no_torch_reference", action="store_true",
-                    help="skip the PyTorch-on-GPU denominator (unmodified reference from baseline/_ref)")
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed (the renderer's maps, the loss "
+                         "and a fixed sample of every updated parameter) as DIR/<name>.npy, float32")
     ap.add_argument("--scaling", choices=["weak", "strong"], default="weak",
                     help="weak: every rank renders its own --batch rays (global batch = batch x N); strong: the --batch "
                          "rays of a step are split over the ranks (SURVEY.md 8e: same draw on all ranks, contiguous slices)")
@@ -82,7 +84,7 @@ def loss_of(ret, target, model, it=0, l1_in_optimizer=False):
 
 
 class ClockSampler:
-    """nvidia-smi sampled DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampled DURING the timed region: SM clock, power and throttle reasons of the timed steps."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -348,6 +350,8 @@ def measure(a, model, n_lights, rank, world, local, dev, scaling, with_e2e, cloc
         graphed.calibrate(host_batches[:8])
         graphed.capture(warmup=3)
 
+    last = {}
+
     def step(rays, li):
         if graphed is not None:
             return graphed.run(rays, li)
@@ -355,6 +359,7 @@ def measure(a, model, n_lights, rank, world, local, dev, scaling, with_e2e, cloc
                                      is_relight=True, sample_method='stratified_sampling', chunk_size=160000,
                                      device=dev, args=Args)
         loss = loss_of(ret, target, model, l1_in_optimizer=fused_opt)
+        last["ret"], last["loss"] = ret, loss
         opt.zero_grad(set_to_none=False)
         loss.backward()
         if bucket is not None:
@@ -411,6 +416,10 @@ def measure(a, model, n_lights, rank, world, local, dev, scaling, with_e2e, cloc
     out = {"scaling": scaling, "ms": ms, "cnt": cnt, "launches": launches, "per_rank": per_rank,
            "value": cnt["rays"] / (ms * 1e-3),   # TIR_CNT_RAYS counts every marched ray: primary + secondary
            "last_batch": dev_batches[-1], "n_s": n_s}
+    if a.dump_outputs and rank == 0:
+        # taken before the end-to-end arm trains on: the maps of the last timed step and the parameters it updated
+        src = graphed.__dict__ if graphed is not None else last
+        out["dump"] = output_snapshot(src["ret"], src["loss"], model)
     if with_e2e:
         # ---- end-to-end arm: pinned HOST buffers through the public boundary, loss read back every step.
         # Default: the host sends (view, pixel, light) ids - 12 B/ray - and the rays are generated on the device
@@ -464,32 +473,34 @@ def measure(a, model, n_lights, rank, world, local, dev, scaling, with_e2e, cloc
     return out
 
 
-def torch_gpu_reference(a, model, n_lights):
-    """The unmodified reference (baseline/_ref) on the same GPU / field / batches, in a subprocess (its `models` and
-    `renderer` modules must not meet tensoir_b200's).  None when the reference copy did not travel to this box."""
-    ref = os.path.join(ROOT, "baseline", "_ref")
-    if not os.path.isdir(ref) or a.config not in (2, 3) or (a.envmap_h, a.envmap_w) != (16, 32):
-        return None          # (the reference's checkpoint kwargs carry no envmap size: only its 16x32 default is comparable)
-    import tempfile
-    tmp = tempfile.mkdtemp(prefix="tir_ref_")
-    ckpt = os.path.join(tmp, "field.th")
-    model.save(ckpt)
-    env = dict(os.environ, PYTHONPATH=os.pathsep.join([os.path.join(ROOT, "tools", "ref_stubs"), ref, ROOT]))
-    for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK", "MASTER_ADDR", "MASTER_PORT"):
-        env.pop(k, None)
-    try:
-        p = subprocess.run([sys.executable, "-P", os.path.join(ROOT, "tools", "ref_torch_gpu.py"), "--ckpt", ckpt,
-                            "--grid", str(a.grid), "--batch", str(a.batch), "--n_lights", str(n_lights)], cwd=ref, env=env,
-                           capture_output=True, text=True, timeout=600)
-        lines = [l for l in p.stdout.splitlines() if l.startswith("{")]
-        if p.returncode != 0 or not lines:
-            return {"unavailable": (p.stderr or p.stdout)[-300:]}
-        return json.loads(lines[-1])
-    except Exception as e:      # the denominator is optional context, never a reason to lose the bench line
-        return {"unavailable": repr(e)[:300]}
-    finally:
-        import shutil
-        shutil.rmtree(tmp, ignore_errors=True)
+DUMP_SAMPLE = 1 << 16       # elements kept per parameter by --dump-outputs (a fixed, seeded sample of larger ones)
+DUMP_LIMIT = 64 << 20       # bytes
+
+
+def output_snapshot(ret, loss, model):
+    """Host copies (float32) of what one training step hands its caller: every map of the renderer's return dict, the
+    loss, and each parameter after the optimiser step (all of it, or DUMP_SAMPLE entries at seeded positions)."""
+    import numpy as np
+    snap = {"loss": loss.detach().float().reshape(1)}
+    for k, v in ret.items():
+        if isinstance(v, torch.Tensor):
+            snap["ret_" + k] = v.detach().float()
+    for k, p in model.named_parameters():
+        flat = p.detach().reshape(-1)
+        if flat.numel() > DUMP_SAMPLE:
+            g = torch.Generator().manual_seed(20211202)
+            flat = flat[torch.randint(0, flat.numel(), (DUMP_SAMPLE,), generator=g).to(flat.device)]
+        snap["param_" + k] = flat.float()
+    snap = {k: np.ascontiguousarray(v.cpu().numpy(), dtype=np.float32) for k, v in snap.items()}
+    assert sum(v.nbytes for v in snap.values()) <= DUMP_LIMIT
+    return snap
+
+
+def write_outputs(directory, snap):
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    for k, v in snap.items():
+        np.save(os.path.join(directory, k + ".npy"), v)
 
 
 def main():
@@ -503,21 +514,15 @@ def main():
     dev = torch.device("cuda", local)
     if world > 1:
         dist.init_process_group("nccl", device_id=dev)
-    import __graft_entry__ as g
-    if rank == 0:
-        g.build()
-    if world > 1:
-        dist.barrier()
     from tensoir_b200 import _lib
     from tensoir_b200.dp import broadcast_parameters
-    _lib.load()
+    _lib.load()                   # the library build() made; nothing is compiled or written here
     if a.config == 5:
         run_relight_pass(a, rank, world, local, dev)
         return
 
     model, n_lights = build_model(a, dev)
     broadcast_parameters(model.parameters())
-    ref_gpu = torch_gpu_reference(a, model, n_lights) if (rank == 0 and world == 1 and not a.no_torch_reference) else None
     clocks = ClockSampler(local) if rank == 0 else None
     m = measure(a, model, n_lights, rank, world, local, dev, a.scaling, with_e2e=True, clocks=clocks)
     strong = None
@@ -565,14 +570,12 @@ def main():
                                           f"(contiguous slices, same draw everywhere), one gradient all-reduce per step",
                                   "value": strong["value"], "unit": UNIT, "ms_per_step": strong["ms"] / a.steps,
                                   "global_batch_rays": a.batch, "rays_per_rank": strong["per_rank"]}
-    if ref_gpu is not None:
-        if "ms_per_step" in ref_gpu:
-            ref_gpu["speedup_ms_per_step"] = ref_gpu["ms_per_step"] / (ms / a.steps)
-        line["torch_gpu_reference"] = ref_gpu
     if not a.no_cpu_baseline and world == 1:
         cb = cpu_baseline(a, steps=2, warmup=1)
         line["cpu_baseline"] = {"value": cb["value"], "unit": UNIT, "cores": cb["cores"], "kind": "port",
                                 "sample": cb["sample"]}
+    if "dump" in m:
+        write_outputs(a.dump_outputs, m["dump"])
     print(json.dumps(line))
     finish()
 
@@ -636,7 +639,7 @@ def run_relight_pass(a, rank, world, local, dev):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for c in batches:
-            step(c, read_back)
+            img = step(c, read_back)
         e1.record()
         torch.cuda.synchronize()
         if world > 1:
@@ -646,7 +649,7 @@ def run_relight_pass(a, rank, world, local, dev):
         if world > 1:
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
             dist.all_reduce(c, op=dist.ReduceOp.SUM)
-        return float(t.item()), ops.counters_dict(c)
+        return float(t.item()), ops.counters_dict(c), img
 
     dev_chunks = [c.to(dev) for c in chunks[:total]]
     clocks = ClockSampler(local) if rank == 0 else None
@@ -656,10 +659,11 @@ def run_relight_pass(a, rank, world, local, dev):
         step(c, False)
     if clocks is not None:
         clocks.mark()
-    ms, cnt = timed(dev_chunks[a.warmup:], False)
+    ms, cnt, img = timed(dev_chunks[a.warmup:], False)
+    snap = {"relit_rgb": img.detach().float().cpu().numpy()} if a.dump_outputs else None
     for c in pinned[:a.warmup]:
         step(c, True)
-    ms_e2e, cnt_e2e = timed(pinned[a.warmup:total], True)
+    ms_e2e, cnt_e2e, _ = timed(pinned[a.warmup:total], True)
     clk = clocks.stop() if clocks is not None else None
     if rank != 0:
         if world > 1:
@@ -667,7 +671,7 @@ def run_relight_pass(a, rank, world, local, dev):
         return
     # roofline of the dominant kernel: the visibility march (density only) over the chunk's (hit, light sample) rays
     peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    peak = json.load(open(peaks_path))["hbm_gbs"] if os.path.exists(peaks_path) else 6650.0
+    peak = json.load(open(peaks_path))["hbm_gbs"] if os.path.exists(peaks_path) else H100_HBM_GBS
     bytes_alg = 32 * cnt["mask"] + 1152 * cnt["density"] + 16 * (cnt["rays"] - a.batch * a.steps * world)
     line = {"metric": METRIC.replace("relight training step", "relight_importance pass"), "value": cnt["rays"] / (ms * 1e-3),
             "unit": UNIT, "n_gpus": world, "steps": a.steps, "warmup": a.warmup, "ms_per_step": ms / a.steps,
@@ -683,6 +687,8 @@ def run_relight_pass(a, rank, world, local, dev):
                          "note": "step-level: algorithmic bytes of all marches of the step / step time (the visibility "
                                  "march is ~all of it)", "achieved": bytes_alg / a.steps / (ms / a.steps * 1e-3) / 1e9,
                          "peak": peak, "unit": "GB/s", "frac": bytes_alg / (ms * 1e-3) / 1e9 / peak, "traffic": None}}
+    if snap is not None:
+        write_outputs(a.dump_outputs, snap)
     print(json.dumps(line))
     if world > 1:
         torch.cuda.synchronize(); dist.barrier(); os._exit(0)
@@ -701,7 +707,7 @@ def roofline(model, batch, n_s, dev, a):
     if os.path.exists(peaks_path):
         peak, src = json.load(open(peaks_path))["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
     else:
-        peak, src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, src = H100_HBM_GBS, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
     rays, li = batch
     with torch.no_grad():
         out = model(rays, li, is_train=False, is_relight=True, N_samples=n_s)
@@ -733,27 +739,15 @@ def roofline(model, batch, n_s, dev, a):
     ms_mlp = t(st.mlp)
     b_run = 32 * c_run["mask"] + 1152 * c_run["density"] + 16 * c_run["rays"]
     b_full = 32 * c["mask"] + 1152 * c["density"] + 16 * c["rays"]
-    traffic, traffic_src = None, None
-    summary = os.path.join(ROOT, "profiles", "r2_ncu_march_raw_summary.csv")
-    if os.path.exists(summary):          # dram bytes of the same kernel / workload / build, one `ncu --set full` capture
-        vals = {}
-        for ln in open(summary):
-            k, unit, v = (ln.strip().split(",") + ["", ""])[:3]
-            if k.startswith("dram__bytes"):
-                vals[k] = float(v) * {"Mbyte": 1e6, "Kbyte": 1e3, "Gbyte": 1e9, "byte": 1.0}.get(unit, 1.0)
-        if len(vals) == 2:
-            traffic = sum(vals.values())
-            traffic_src = "profiles/r2_ncu_march_raw_summary.csv (ncu --set full of tools/profile_target.py, this build)"
     b_mlp = 3456 * c["app"]
     flops_mlp = 79712 * c["app"]
     return {"bound": "hbm", "kernel": "march_kernel<16,TABLE,app,dense> (secondary density march + compaction)",
             # the launch that is timed inside the step skips the tail of rays whose transmittance is exactly 0: only the
             # units it really processed are credited (conservative); the count-parity launch is reported next to it
             "achieved": b_run / (ms_march * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
-            "frac": b_run / (ms_march * 1e-3) / 1e9 / peak, "peak_source": src, "traffic": traffic,
-            "traffic_source": traffic_src,
-            "note": "the VM factors and the alpha mask are L2-resident (126 MB L2), so measured DRAM traffic is ~400x "
-                    "below the algorithmic bytes; frac is algorithmic bytes / time / measured HBM copy bandwidth",
+            "frac": b_run / (ms_march * 1e-3) / 1e9 / peak, "peak_source": src,
+            "note": "frac is algorithmic bytes / time / HBM bandwidth; much of the VM factors and the alpha mask stays "
+                    "in the 50 MB L2, so the DRAM traffic is below the algorithmic bytes",
             "ms_per_launch": ms_march, "algorithmic_bytes_per_launch": b_run,
             "units_per_launch": {"mask_queries": c_run["mask"], "density_samples": c_run["density"], "rays": c_run["rays"]},
             "count_parity_launch": {"ms_per_launch": ms_full, "algorithmic_bytes_per_launch": b_full,
@@ -761,8 +755,8 @@ def roofline(model, batch, n_s, dev, a):
                                     "frac": b_full / (ms_full * 1e-3) / 1e9 / peak,
                                     "units_per_launch": {"mask_queries": c["mask"], "density_samples": c["density"],
                                                          "rays": c["rays"]}},
-            "second_kernel": {"kernel": "app_mlp_tc5_kernel (appearance gather -> basis_mat -> 150-128-128-3 MLP on "
-                                        "tcgen05.mma, accumulator + split-BF16 activations in TMEM, fp32 accumulate)",
+            "second_kernel": {"kernel": "app_mlp_wgmma_kernel (appearance gather -> basis_mat -> 150-128-128-3 MLP on "
+                                        "wgmma.mma_async, split-BF16 A operand + accumulator in registers, fp32 accumulate)",
                               "bound": "L2 gather bandwidth / latency (3456 B per sample from the L2-resident factors)",
                               "ms_per_launch": ms_mlp, "app_samples": c["app"],
                               "achieved_GBps": b_mlp / (ms_mlp * 1e-3) / 1e9,

@@ -1,4 +1,4 @@
-/* tensoir_b200 — C ABI of the B200-native TensoIR volume-rendering hot path.
+/* tensoir_b200 — C ABI of the H100-native (sm_90a) TensoIR volume-rendering hot path.
  *
  * The reference (Haian-Jin/TensoIR) is 100 % Python/PyTorch and has no FFI of its own
  * (SURVEY.md §8b); this ABI is what the Python shim in tensoir_b200/ binds with ctypes, and
@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define TIR_ABI_VERSION 2
+#define TIR_ABI_VERSION 3
 
 typedef enum TirStatus {
   TIR_OK = 0,
@@ -193,23 +193,21 @@ int tir_app_mlp(const TirField* field, const TirMlp* mlp, const TirAppSample* sa
                 const uint32_t* sample_count, int64_t max_samples, const float* ray_dirs, int32_t n_dirs,
                 const int32_t* light_idx, float* rgb_out, void* stream);
 
-/* The two implementations behind tir_app_mlp (which dispatches to _tc5 unless the environment has TIR_MLP_LEGACY=1):
- *   _tc5     sm_100a-native: tcgen05.mma with the accumulator and the A operand in tensor memory (TMEM), weights
- *            resident in shared memory, two warpgroups ping-ponging through one issuer thread (csrc/tir_mlp_tc5.cu)
+/* The two implementations behind tir_app_mlp (which dispatches to _wgmma unless the environment has TIR_MLP_LEGACY=1):
+ *   _wgmma   sm_90a-native: wgmma.mma_async with the A operand and the accumulator in registers, weights resident
+ *            in shared memory, two warpgroups per CTA on different 64-sample tiles (csrc/tir_mlp_wgmma.cu)
  *   _legacy  round 1: mma.sync.m16n8k16 on 64-sample tiles (csrc/tir_mlp.cu)
  * Same arguments and results (both use the error-compensated split-BF16 product with fp32 accumulation). */
-int tir_app_mlp_tc5(const TirField* field, const TirMlp* mlp, const TirAppSample* samples,
-                    const uint32_t* sample_count, int64_t max_samples, const float* ray_dirs, int32_t n_dirs,
-                    const int32_t* light_idx, float* rgb_out, void* stream);
+int tir_app_mlp_wgmma(const TirField* field, const TirMlp* mlp, const TirAppSample* samples,
+                      const uint32_t* sample_count, int64_t max_samples, const float* ray_dirs, int32_t n_dirs,
+                      const int32_t* light_idx, float* rgb_out, void* stream);
 int tir_app_mlp_legacy(const TirField* field, const TirMlp* mlp, const TirAppSample* samples,
                        const uint32_t* sample_count, int64_t max_samples, const float* ray_dirs, int32_t n_dirs,
                        const int32_t* light_idx, float* rgb_out, void* stream);
-int tir_app_mlp_points_tc5(const TirField* field, const TirMlp* mlp, const float* xn, const float* x_in,
-                           const int32_t* light_idx, int64_t n, int32_t act, float* out, void* stream);
+int tir_app_mlp_points_wgmma(const TirField* field, const TirMlp* mlp, const float* xn, const float* x_in,
+                             const int32_t* light_idx, int64_t n, int32_t act, float* out, void* stream);
 int tir_app_mlp_points_legacy(const TirField* field, const TirMlp* mlp, const float* xn, const float* x_in,
                               const int32_t* light_idx, int64_t n, int32_t act, float* out, void* stream);
-/* 0 while no bounded mbarrier wait of the tcgen05 kernel has timed out (host read; synchronises the device). */
-int tir_mlp_tc5_error(void);
 
 /* Same gather+MLP on explicit points (no compositing): xn [n,3] normalised coords, x_in [n,3] the 3-vector fed
  * to the MLP next to the features (view dir for MLPRender_Fea, position for MLPBRDF_PEandFeature),

@@ -6,11 +6,11 @@ module; only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_ba
 
 This is a *restatement* (not a copy) of the reference's PyTorch algorithm as plain
 functions over an :class:`OracleField` record.  Every function cites the reference
-``file:line`` (relative to ``/root/reference``) that it follows, and keeps the reference's
+``file:line`` (relative to the reference's root) that it follows, and keeps the reference's
 operation order so that on CPU it reproduces the reference bit-for-bit.
 
 Parity pinning: ``tests/golden/make_golden.py`` imports the real reference from
-``/root/reference`` in the build container, runs it on small seeded inputs and stores
+a checkout of it, runs it on small seeded inputs and stores
 inputs + outputs under ``tests/golden/*.pt``; ``tests/test_oracle_golden.py`` replays the
 oracle against those fixtures (bit-exact on CPU).  The reference ships no golden vectors of
 its own (SURVEY.md §4), so those generated fixtures are the pin.

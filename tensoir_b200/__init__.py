@@ -1,4 +1,4 @@
-"""tensoir_b200 — B200-native (sm_100a) implementation of TensoIR's volume-rendering hot path.
+"""tensoir_b200 — H100-native (sm_90a) implementation of TensoIR's volume-rendering hot path.
 
 Python/PyTorch host code owns tensors and autograd and mirrors the reference's public surface
 (TensorVMSplit, relight_utils, Renderer_TensoIR_train); per-sample work runs in hand-written CUDA kernels

@@ -14,7 +14,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("TIR_LIB") or os.path.join(_HERE, "lib", "libtensoir_b200.so")   # TIR_LIB: A/B builds
 
-ABI_VERSION = 2
+ABI_VERSION = 3
 CNT_MASK, CNT_DENSITY, CNT_APP, CNT_RAYS, CNT_OVERFLOW, CNT_SLOTS = 0, 1, 2, 3, 4, 8
 SAMPLE_STEP, SAMPLE_TABLE = 0, 1
 
@@ -125,15 +125,14 @@ EXPORTS = {
                                       C.c_void_p]),
     "tir_app_mlp": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), C.c_void_p, C.c_void_p, C.c_int64, f32p,
                               C.c_int32, C.c_void_p, f32p, C.c_void_p]),
-    "tir_app_mlp_tc5": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), C.c_void_p, C.c_void_p, C.c_int64, f32p,
+    "tir_app_mlp_wgmma": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), C.c_void_p, C.c_void_p, C.c_int64, f32p,
                                   C.c_int32, C.c_void_p, f32p, C.c_void_p]),
     "tir_app_mlp_legacy": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), C.c_void_p, C.c_void_p, C.c_int64, f32p,
                                      C.c_int32, C.c_void_p, f32p, C.c_void_p]),
-    "tir_app_mlp_points_tc5": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), f32p, f32p, C.c_void_p, C.c_int64,
+    "tir_app_mlp_points_wgmma": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), f32p, f32p, C.c_void_p, C.c_int64,
                                          C.c_int32, f32p, C.c_void_p]),
     "tir_app_mlp_points_legacy": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), f32p, f32p, C.c_void_p, C.c_int64,
                                             C.c_int32, f32p, C.c_void_p]),
-    "tir_mlp_tc5_error": (C.c_int, []),
     "tir_app_mlp_points": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), f32p, f32p, C.c_void_p, C.c_int64,
                                      C.c_int32, f32p, C.c_void_p]),
     "tir_app_mlp_points_save": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), f32p, f32p, C.c_void_p, C.c_int64,
@@ -193,7 +192,7 @@ EXPORTS = {
 # kernels launched per entry point (for bench.py's gpu_launches claim)
 KERNELS_PER_CALL = {"tir_pack_channels_last": 1, "tir_unpack_channels_last_add": 1, "tir_pack_alpha_mask": 2,
                     "tir_density_points": 1, "tir_alpha_mask_points": 1, "tir_march_density": 1,
-                    "tir_march_radiance": 2, "tir_secondary_march": 1, "tir_secondary_radiance": 2, "tir_app_mlp": 1, "tir_app_mlp_tc5": 1, "tir_app_mlp_legacy": 1, "tir_app_mlp_points_tc5": 1,
+                    "tir_march_radiance": 2, "tir_secondary_march": 1, "tir_secondary_radiance": 2, "tir_app_mlp": 1, "tir_app_mlp_wgmma": 1, "tir_app_mlp_legacy": 1, "tir_app_mlp_points_wgmma": 1,
                     "tir_app_mlp_points_legacy": 1,
                     "tir_shade_fwd": 1, "tir_shade_bwd": 1, "tir_app_mlp_points": 1, "tir_app_mlp_points_save": 1, "tir_vm_app_products": 1, "tir_vm_app_products_bwd": 1,
                     "tir_vm_density_bwd": 1, "tir_vm_density_grad": 1, "tir_vm_density_grad_bwd": 1,

@@ -41,17 +41,30 @@ __device__ __forceinline__ FloorI floor_fi(float x) {
   return r;
 }
 
+// Streaming multiprocessors of the current device (132 on an H100 SXM), queried once per device: persistent kernels
+// launch one wave of CTAs and grid-stride kernels cap their grids at a few CTAs per SM.
+inline int num_sms() {
+  static int cached[16] = {};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 16) dev = 0;
+  if (cached[dev] == 0) {
+    int n = 0;
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    cached[dev] = n > 0 ? n : 132;
+  }
+  return cached[dev];
+}
+
 __device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 
-// 256-bit read-only load (sm_100a LDG.E.256): one whole 32-byte sector per lane and request.  Channel-last rows are
-// multiples of 64 B, so a bilinear tap of 16 channels is two of these instead of four 128-bit loads that touch every
-// sector twice (half the L1 tag lookups / wavefronts of the gather-bound kernels).  `p` must be 32-byte aligned.
+// One whole 32-byte sector of a channel-last row through the read-only path: sm_90 has no 256-bit load, so this is two
+// adjacent 128-bit loads issued back to back (the second one hits the sector the first one brought into L1).
+// `p` must be 32-byte aligned.
 struct Float8 { float4 a, b; };
 __device__ __forceinline__ Float8 ldg8(const float* p) {
   Float8 r;
-  asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=f"(r.a.x), "=f"(r.a.y), "=f"(r.a.z), "=f"(r.a.w), "=f"(r.b.x), "=f"(r.b.y), "=f"(r.b.z), "=f"(r.b.w)
-               : "l"(p));
+  r.a = __ldg(reinterpret_cast<const float4*>(p));
+  r.b = __ldg(reinterpret_cast<const float4*>(p) + 1);
   return r;
 }
 

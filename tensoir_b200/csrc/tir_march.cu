@@ -320,7 +320,7 @@ int launch_march(const MarchParams& p, cudaStream_t stream) {
   if (p.f.dC != 16) return TIR_ERR_SHAPE;
   if (p.cfg.n_samples <= 0) return TIR_ERR_CONFIG;
   int64_t blocks = (p.n_rays + kWarpsPerBlock - 1) / kWarpsPerBlock;
-  const int64_t max_blocks = 148 * kBlocksPerSM;   // persistent: every resident CTA slot of the 148 SMs, grid-stride over rays
+  const int64_t max_blocks = (int64_t)num_sms() * kBlocksPerSM;   // persistent: every resident CTA slot, grid-stride over rays
   if (blocks > max_blocks) blocks = max_blocks;
   if (p.cfg.sampling == TIR_SAMPLE_STEP) {
     march_kernel<16, TIR_SAMPLE_STEP, WITH_APP, DENSE><<<(int)blocks, kWarpsPerBlock * 32, 0, stream>>>(p);

@@ -394,7 +394,7 @@ int launch(const MlpParams& p, int64_t max_items, cudaStream_t stream) {
   }
   int64_t tiles = (max_items + M - 1) / M;
   const int nj = POINTS ? (p.n_jobs > 0 ? p.n_jobs : 1) : 1;
-  int per_job = 148 / nj;                              // CTAs per job: one wave, one CTA per SM
+  int per_job = num_sms() / nj;                            // CTAs per job: one wave, one CTA per SM
   if (tiles < per_job) per_job = (int)(tiles > 0 ? tiles : 1);
   app_mlp_kernel<POINTS><<<per_job * nj, NT, smem, stream>>>(p);
   return (int)cudaGetLastError();
@@ -402,14 +402,14 @@ int launch(const MlpParams& p, int64_t max_items, cudaStream_t stream) {
 
 }  // namespace
 
-extern "C" int tir_app_mlp_tc5(const TirField* field, const TirMlp* mlp, const TirAppSample* samples,
-                               const uint32_t* sample_count, int64_t max_samples, const float* ray_dirs,
-                               int32_t n_dirs, const int32_t* light_idx, float* rgb_out, void* stream);
-extern "C" int tir_app_mlp_points_tc5(const TirField* field, const TirMlp* mlp, const float* xn, const float* x_in,
-                                      const int32_t* light_idx, int64_t n, int32_t act, float* out, void* stream);
+extern "C" int tir_app_mlp_wgmma(const TirField* field, const TirMlp* mlp, const TirAppSample* samples,
+                                 const uint32_t* sample_count, int64_t max_samples, const float* ray_dirs,
+                                 int32_t n_dirs, const int32_t* light_idx, float* rgb_out, void* stream);
+extern "C" int tir_app_mlp_points_wgmma(const TirField* field, const TirMlp* mlp, const float* xn, const float* x_in,
+                                        const int32_t* light_idx, int64_t n, int32_t act, float* out, void* stream);
 
 // TIR_MLP_LEGACY=1 selects the round-1 mma.sync kernel for the inference entry points (A/B comparison); the default is
-// the tcgen05 / TMEM kernel of tir_mlp_tc5.cu.  The training forward with activation dumps always uses this file.
+// the wgmma kernel of tir_mlp_wgmma.cu.  The training forward with activation dumps always uses this file.
 static bool legacy_mlp() {
   static const bool v = [] { const char* e = getenv("TIR_MLP_LEGACY"); return e && e[0] == '1'; }();
   return v;
@@ -423,7 +423,7 @@ extern "C" int tir_app_mlp(const TirField* field, const TirMlp* mlp, const TirAp
                            const uint32_t* sample_count, int64_t max_samples, const float* ray_dirs, int32_t n_dirs,
                            const int32_t* light_idx, float* rgb_out, void* stream) {
   if (!legacy_mlp())
-    return tir_app_mlp_tc5(field, mlp, samples, sample_count, max_samples, ray_dirs, n_dirs, light_idx, rgb_out, stream);
+    return tir_app_mlp_wgmma(field, mlp, samples, sample_count, max_samples, ray_dirs, n_dirs, light_idx, rgb_out, stream);
   return tir_app_mlp_legacy(field, mlp, samples, sample_count, max_samples, ray_dirs, n_dirs, light_idx, rgb_out, stream);
 }
 
@@ -469,7 +469,7 @@ extern "C" int tir_app_mlp_points_legacy(const TirField* field, const TirMlp* ml
 
 extern "C" int tir_app_mlp_points(const TirField* field, const TirMlp* mlp, const float* xn, const float* x_in,
                                   const int32_t* light_idx, int64_t n, int32_t act, float* out, void* stream) {
-  if (!legacy_mlp()) return tir_app_mlp_points_tc5(field, mlp, xn, x_in, light_idx, n, act, out, stream);
+  if (!legacy_mlp()) return tir_app_mlp_points_wgmma(field, mlp, xn, x_in, light_idx, n, act, out, stream);
   return tir_app_mlp_points_legacy(field, mlp, xn, x_in, light_idx, n, act, out, stream);
 }
 

@@ -611,7 +611,7 @@ int launch_heads_backward(const TirField& f, const HeadBwdJob* jobs, int n_jobs,
   wp.sh = sh; wp.n_jobs = n_jobs; wp.n = n; wp.n_dev = n_dev;
   for (int j = 0; j < n_jobs; ++j) { dp.jobs[j] = jobs[j]; wp.jobs[j] = jobs[j]; }
   const int64_t tiles = (n + M - 1) / M;
-  int per_job = 148 / n_jobs;
+  int per_job = num_sms() / n_jobs;
   if (tiles < per_job) per_job = (int)tiles;
   heads_dgrad_kernel<<<per_job * n_jobs, NT, sizeof(DgradSmem), stream>>>(dp);
   cudaError_t e = cudaGetLastError();

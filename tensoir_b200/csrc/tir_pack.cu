@@ -97,7 +97,8 @@ extern "C" int tir_density_points(const TirField* field, const float* xn, int64_
                                   void* stream) {
   if (n <= 0) return TIR_OK;   // empty input: nothing to do (pointers of empty tensors are NULL)
   if (!field || !xn) return TIR_ERR_NULL;
-  int blocks = (int)((n + 127) / 128 < 148 * 16 ? (n + 127) / 128 : 148 * 16);
+  const int64_t cap = (int64_t)num_sms() * 16;
+  int blocks = (int)((n + 127) / 128 < cap ? (n + 127) / 128 : cap);
   if (field->dC == 16)
     density_points_kernel<16><<<blocks, 128, 0, (cudaStream_t)stream>>>(*field, xn, n, feature, sigma);
   else if (field->dC == 8)
@@ -115,7 +116,8 @@ __global__ void alpha_points_kernel(TirField f, const float* __restrict__ xyz, i
 extern "C" int tir_alpha_mask_points(const TirField* field, const float* xyz, int64_t n, uint8_t* mask, void* stream) {
   if (n <= 0) return TIR_OK;   // empty input: nothing to do (pointers of empty tensors are NULL)
   if (!field || !xyz || !mask || !field->amask || !field->acell) return TIR_ERR_NULL;
-  int blocks = (int)((n + 255) / 256 < 148 * 8 ? (n + 255) / 256 : 148 * 8);
+  const int64_t cap = (int64_t)num_sms() * 8;
+  int blocks = (int)((n + 255) / 256 < cap ? (n + 255) / 256 : cap);
   alpha_points_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(*field, xyz, n, mask);
   return (int)cudaGetLastError();
 }

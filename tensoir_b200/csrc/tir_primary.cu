@@ -313,7 +313,8 @@ __global__ void primary_tail_bwd_kernel(TailPtrs p, TailGradPtrs q, int64_t cap,
 
 inline int blocks_for(int64_t n, int threads) {
   int64_t b = (n + threads - 1) / threads;
-  return (int)(b < 148 * 8 ? (b > 0 ? b : 1) : 148 * 8);
+  const int64_t cap = (int64_t)num_sms() * 8;
+  return (int)(b < cap ? (b > 0 ? b : 1) : cap);
 }
 
 int find_job(const TirHeadJob* jobs, int n_jobs, int role) {

@@ -305,7 +305,7 @@ extern "C" int tir_shade_bwd(const float* normal, const float* albedo, const flo
     if (e != cudaSuccess) return (int)e;
   }
   int64_t blocks = (bs + kWarps - 1) / kWarps;
-  if (blocks > 148 * 2) blocks = 148 * 2;
+  if (blocks > 2 * num_sms()) blocks = 2 * num_sms();
   shade_bwd_kernel<<<(unsigned)blocks, kWarps * 32, smem, (cudaStream_t)stream>>>(p);
   return (int)cudaGetLastError();
 }
@@ -375,7 +375,7 @@ extern "C" int tir_shade_hits_bwd(const float* rays, const uint8_t* mask, const 
     if (e != cudaSuccess) return (int)e;
   }
   int64_t blocks = (n + kWarps - 1) / kWarps;
-  if (blocks > 148 * 2) blocks = 148 * 2;
+  if (blocks > 2 * num_sms()) blocks = 2 * num_sms();
   shade_bwd_kernel<<<(unsigned)blocks, kWarps * 32, smem, (cudaStream_t)stream>>>(p);
   return (int)cudaGetLastError();
 }

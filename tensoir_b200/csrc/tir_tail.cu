@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 
 #include "../../include/tensoir_b200.h"
+#include "tir_device.cuh"
 #include "tir_epilogue_body.h"
 #include "tir_tail_body.h"
 
@@ -143,7 +144,8 @@ __global__ void epilogue_bwd_kernel(int64_t n, const float* packed, const float*
 
 inline int blocks_for(int64_t n, int threads) {
   int64_t b = (n + threads - 1) / threads;
-  return (int)(b < 148 * 8 ? (b > 0 ? b : 1) : 148 * 8);
+  const int64_t cap = (int64_t)tir::num_sms() * 8;
+  return (int)(b < cap ? (b > 0 ? b : 1) : cap);
 }
 
 }  // namespace

@@ -11,6 +11,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "../../include/tensoir_b200.h"
+#include "tir_device.cuh"
 
 namespace {
 
@@ -159,7 +160,7 @@ int make_jobs(const TirTvPlane* planes, int n, bool need_grad, TvJobs* jobs, int
 
 int grid_x(int64_t units) {
   int64_t b = (units + kThreads - 1) / kThreads;
-  const int64_t cap = 148 * 8;
+  const int64_t cap = (int64_t)tir::num_sms() * 8;
   return (int)(b < 1 ? 1 : (b > cap ? cap : b));
 }
 

@@ -379,7 +379,8 @@ __global__ void composite_bwd_kernel(const float* __restrict__ sigma, const floa
   }
 }
 
-inline int blocks_for(int64_t n, int threads, int cap = 148 * 16) {
+inline int blocks_for(int64_t n, int threads, int cap = 0) {
+  if (cap <= 0) cap = num_sms() * 16;
   int64_t b = (n + threads - 1) / threads;
   return (int)(b < 1 ? 1 : (b > cap ? cap : b));
 }

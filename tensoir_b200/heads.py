@@ -19,7 +19,7 @@ from .vm_autograd import _grad_shadows, _ptr_array, _to_param_layout
 
 def _wgrad(g, a, splits=32):
     """g^T @ a for tall-skinny operands ([n, <=128]^T @ [n, <=150], n ~ 2e4).  cuBLAS tiles only the tiny output
-    (6 CTAs on 148 SMs); splitting the reduction over n into `splits` batched GEMMs fills the machine."""
+    (6 CTAs on 132 SMs); splitting the reduction over n into `splits` batched GEMMs fills the machine."""
     n = g.shape[0]
     per = n // splits
     if per < 64:

@@ -120,6 +120,7 @@ class StaticTrainStep:
                                      white_bg=True, is_train=True, is_relight=True, sample_method=self.sample_method,
                                      chunk_size=160000, device=self.dev, args=self.args)
         loss = self.loss_fn(ret, self.model)
+        self.ret = ret                    # the captured forward's outputs: after a replay they hold that step's values
         loss.backward()
         flag = torch.maximum((st["overflow_step"] > 0).to(torch.float32), self.force_skip)
         if self.bucket is not None:

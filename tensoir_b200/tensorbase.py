@@ -186,7 +186,7 @@ class TensorBase(torch.nn.Module):
         """tensorBase_rotated_lights.py:405-434.  Only the shipped configuration (MLP_Fea,
         configs/**: shadingMode = MLP_Fea) has kernels; other modes are out of scope (SURVEY.md §2)."""
         if shadingMode != 'MLP_Fea':
-            raise NotImplementedError(f"shadingMode {shadingMode!r}: only 'MLP_Fea' is on the B200 hot path")
+            raise NotImplementedError(f"shadingMode {shadingMode!r}: only 'MLP_Fea' is on the CUDA hot path")
         self.renderModule = MLPRender_Fea(self.app_dim, view_pe, fea_pe, featureC).to(device)
         if self.normals_kind not in ("purely_predicted", "derived_plus_predicted", "purely_derived"):
             raise NotImplementedError(f"normals_kind {self.normals_kind!r}")

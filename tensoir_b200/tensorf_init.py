@@ -27,7 +27,7 @@ class TensorVMSplit(_RelightVMSplit):
         self.shadingMode, self.pos_pe, self.view_pe, self.fea_pe, self.featureC = \
             shadingMode, pos_pe, view_pe, fea_pe, featureC
         if shadingMode != 'MLP_Fea':
-            raise NotImplementedError(f"shadingMode {shadingMode!r}: only 'MLP_Fea' is on the B200 hot path")
+            raise NotImplementedError(f"shadingMode {shadingMode!r}: only 'MLP_Fea' is on the CUDA hot path")
         self.renderModule = MLPRender_Fea(self.app_dim, view_pe, fea_pe, featureC).to(device)
 
     def init_svd_volume(self, res, device):

@@ -1,8 +1,7 @@
-"""Generate golden fixtures by running the REAL reference (imported from /root/reference).
+"""Generate golden fixtures by running the REAL reference (imported from a checkout of TensoIR).
 
-Run in the build container only (the GPU box has no /root/reference):
-
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py <path to the TensoIR checkout>            # every fixture
+    python tests/golden/make_golden.py <path to the TensoIR checkout> dropin     # dropin_reference.pt only
 
 Writes tests/golden/*.pt: small seeded inputs, the reference model's state_dict / alpha mask,
 and the reference's outputs for every hot-path function (SURVEY.md §8a).  The oracle
@@ -18,12 +17,12 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(os.path.dirname(HERE))
-REF = "/root/reference"
+REF = os.path.abspath(sys.argv[1]) if len(sys.argv) > 1 else None     # the reference checkout
 sys.path.insert(0, REPO)
 
 
 def import_reference():
-    """Put /root/reference on sys.path with the stubs SURVEY.md §8c lists."""
+    """Put the reference checkout on sys.path with the stubs SURVEY.md §8c lists."""
     kornia = types.ModuleType("kornia")
 
     def create_meshgrid(h, w, normalized_coordinates=True, device=None, dtype=torch.float32):
@@ -268,7 +267,10 @@ def main():
                           density_plane1=m2.density_plane[1].detach().clone(),
                           app_line0=m2.app_line[0].detach().clone())
     out["rotated"] = fx
-    torch.save(fx, os.path.join(HERE, "rotated_g24.pt"))
+    parts = {"state_dict": "rotated_g24_state.pt", "renderer_train_grads": "rotated_g24_grads.pt"}
+    for key, part in parts.items():                  # stored apart: every fixture file stays below 1 MB
+        torch.save(fx.pop(key), os.path.join(HERE, part))
+    torch.save(dict(fx, _parts=parts), os.path.join(HERE, "rotated_g24.pt"))
 
     # ---------------- general multi-light model (boundary smoke) -------------------------
     from tensoir_b200.synthetic import install_lego_density
@@ -316,5 +318,38 @@ def main():
         print(n, os.path.getsize(os.path.join(HERE, n)) // 1024, "KiB")
 
 
+def dropin_fixture():
+    """dropin_reference.pt: what tests/test_dropin_cpu.py checks the drop-in tree against.
+    imports: every `from models.* / renderer import ...` in the reference's scripts and data loaders (the modules that
+    must import unchanged when dropin/ shadows models/ and renderer.py); grid_sample: the reference's
+    relight_utils.grid_sample on coordinates up to 1.5x outside [-1, 1] (its border-clamping extrapolation)."""
+    import ast
+    imports = []
+    for d, _, files in sorted(os.walk(REF)):
+        rel = os.path.relpath(d, REF)
+        if rel.split(os.sep)[0] in ("models", "__pycache__") or "__pycache__" in rel:
+            continue
+        for f in sorted(files):
+            if not f.endswith(".py") or (rel == "." and f == "renderer.py"):
+                continue
+            for node in ast.walk(ast.parse(open(os.path.join(d, f)).read())):
+                if isinstance(node, ast.ImportFrom) and node.module and node.module.split(".")[0] in ("models", "renderer"):
+                    imports.append((os.path.normpath(os.path.join(rel, f)), node.module, [a.name for a in node.names]))
+    ru, _, _, _ = import_reference()
+    g = torch.Generator().manual_seed(0)
+    img = torch.randn(2, 5, 7, 9, generator=g)
+    wide = torch.rand(2, 6, 4, 2, generator=g) * 3 - 1.5
+    out = ru.grid_sample(img, wide)
+    torch.save({"imports": imports, "grid_sample": {"img": img, "wide": wide, "out": out.detach().clone()}},
+               os.path.join(HERE, "dropin_reference.pt"))
+    print("dropin_reference.pt", os.path.getsize(os.path.join(HERE, "dropin_reference.pt")), "bytes,", len(imports), "imports")
+
+
 if __name__ == "__main__":
-    main()
+    if REF is None or not os.path.isdir(REF):
+        raise SystemExit(__doc__)
+    if sys.argv[2:] == ["dropin"]:
+        dropin_fixture()
+    else:
+        main()
+        dropin_fixture()

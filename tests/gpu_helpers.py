@@ -8,7 +8,11 @@ GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 def load_fixture(name):
-    return torch.load(os.path.join(GOLDEN, name), weights_only=False)
+    """A golden fixture; entries listed under "_parts" are stored in files of their own (every file stays < 1 MB)."""
+    fx = torch.load(os.path.join(GOLDEN, name), weights_only=False)
+    for key, part in fx.pop("_parts", {}).items():
+        fx[key] = torch.load(os.path.join(GOLDEN, part), weights_only=False)
+    return fx
 
 
 def renderer_args(n=96, near=0.05, far=1.5):

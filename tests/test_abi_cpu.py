@@ -26,7 +26,7 @@ def test_header_symbols_exported(lib):
     for n in names:
         assert hasattr(lib, n), f"{n} declared in the header but not exported"
         assert n in _lib.EXPORTS, f"{n} has no ctypes binding"
-    assert lib.tir_abi_version() == 2
+    assert lib.tir_abi_version() == 3
 
 
 def test_struct_sizes_match_header(lib):

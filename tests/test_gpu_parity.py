@@ -731,10 +731,10 @@ def test_fused_primary_matches_modular_path(golden_rotated, kind):
     assert not bad, bad
 
 
-def test_tcgen05_mlp_matches_mma_sync_kernel(rot):
-    """The sm_100a-native appearance MLP (tcgen05.mma, accumulator + activations in TMEM, csrc/tir_mlp_tc5.cu) against
-    the round-1 mma.sync kernel: explicit points for the three heads (ragged sizes incl. a partial tile and an odd
-    number of tiles), and the secondary appearance list; no bounded wait may have timed out."""
+def test_wgmma_mlp_matches_mma_sync_kernel(rot):
+    """The sm_90a-native appearance MLP (wgmma.mma_async, A operand + accumulator in registers, csrc/tir_mlp_wgmma.cu)
+    against the round-1 mma.sync kernel: explicit points for the three heads (ragged sizes incl. a partial tile and an
+    odd number of tiles), and the secondary appearance list."""
     import ctypes as C
     from tensoir_b200 import _lib, ops
     from tensoir_b200.device_field import mlp_struct
@@ -751,14 +751,13 @@ def test_tcgen05_mlp_matches_mma_sync_kernel(rot):
             keep = []
             mlp = mlp_struct(m, head, keep, light=light)
             outs = []
-            for fn in (lib.tir_app_mlp_points_legacy, lib.tir_app_mlp_points_tc5):
+            for fn in (lib.tir_app_mlp_points_legacy, lib.tir_app_mlp_points_wgmma):
                 out = torch.full((n, mlp.out_dim), -7.0, device=DEV)
                 _lib.check(fn(C.byref(f), C.byref(mlp), _lib.dptr(xn), _lib.dptr(xi),
                               _lib.dptr(li, torch.int32) if light == "index" else None, n, act, _lib.dptr(out),
                               _lib.stream_ptr()), "mlp points")
                 outs.append(out)
             torch.cuda.synchronize()
-            assert lib.tir_mlp_tc5_error() == 0
             close(outs[1], outs[0], 2e-5, f"{head} n={n}")
     # sample-list form on a real secondary march
     with torch.no_grad():
@@ -770,14 +769,13 @@ def test_tcgen05_mlp_matches_mma_sync_kernel(rot):
     st = ops.SecondaryStages(m, surf, out[2][mask], fx["light_idx"].to(DEV)[mask], dirs, n_sample=24)
     st.march()
     res = []
-    for fn in (lib.tir_app_mlp_legacy, lib.tir_app_mlp_tc5):
+    for fn in (lib.tir_app_mlp_legacy, lib.tir_app_mlp_wgmma):
         st.ind.zero_()
         _lib.check(fn(C.byref(st.f), C.byref(st.mlp_s), _lib.dptr(st.sc.buf, torch.uint8),
                       _lib.dptr(st.sc.count, torch.int32), st.sc.capacity, _lib.dptr(st.dr), st.n_dirs,
                       _lib.dptr(st.li, torch.int32), _lib.dptr(st.ind), _lib.stream_ptr()), "mlp list")
         res.append(st.ind.clone())
     torch.cuda.synchronize()
-    assert lib.tir_mlp_tc5_error() == 0
     assert int(st.sc.count.item()) > 100
     close(res[1], res[0], 2e-5, "indirect light")
 

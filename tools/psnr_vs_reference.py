@@ -1,4 +1,4 @@
-"""PSNR of our image against the reference algorithm's image (BASELINE metric, second half) on the GPU box.
+"""PSNR of our image against the reference algorithm's image (BASELINE metric, second half) on the GPU.
 
 Renders a centred W x W crop of one 800x800 test view of the synthetic lego scene twice — through the library
 (`Renderer_TensoIR_train`, CUDA kernels) and through the oracle's restatement of the reference run as eager PyTorch on the

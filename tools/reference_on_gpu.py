@@ -41,6 +41,6 @@ for it in range(warm + steps):
     if it >= warm:
         ts.append(time.perf_counter() - t0)
         rays_n.append(batch + f.counters.get("secondary_rays", 0))
-print(json.dumps({"what": "reference algorithm (oracle port, eager PyTorch) on one B200, same workload as bench.py",
+print(json.dumps({"what": "reference algorithm (oracle port, eager PyTorch) on one GPU, same workload as bench.py",
                   "grid": grid, "batch": batch, "steps": steps, "ms_per_step": 1e3 * sum(ts) / len(ts),
                   "rays_per_s": sum(rays_n) / sum(ts), "peak_mem_GB": torch.cuda.max_memory_allocated() / 1e9}))
