@@ -1,10 +1,7 @@
-"""Shadow of the reference's renderer.py for unchanged train scripts: the hot-path boundary comes from tensoir_b200;
-the evaluation loops (I/O + metrics, out of scope) are taken from the reference's own renderer.py when it is
-importable further down sys.path."""
-import importlib.util
-import os
+"""Shadow of the reference's renderer.py for unchanged train scripts: the hot-path boundary, compute_rescale_ratio and
+the three evaluation loops all come from tensoir_b200 (same signatures, return values and written files)."""
+import os  # noqa: F401
 import random  # noqa: F401  (the train scripts take np / random / os / tqdm / torch from `from renderer import *`)
-import sys
 
 import numpy as np  # noqa: F401
 import torch  # noqa: F401
@@ -22,26 +19,6 @@ except ImportError:
 
 from tensoir_b200.renderer import Renderer_TensoIR_train, OctreeRender_trilinear_fast  # noqa: F401
 from tensoir_b200.relight_utils import render_with_BRDF  # noqa: F401
+from tensoir_b200.evaluation import (compute_rescale_ratio, evaluation_iter_TensoIR,  # noqa: F401
+                                     evaluation_iter_TensoIR_simple, evaluation_iter_TensoIR_general_multi_lights)
 
-
-def _load_reference_renderer():
-    here = os.path.dirname(os.path.abspath(__file__))
-    for p in sys.path:
-        cand = os.path.join(p, "renderer.py")
-        if os.path.abspath(p) != here and os.path.exists(cand):
-            spec = importlib.util.spec_from_file_location("_reference_renderer", cand)
-            mod = importlib.util.module_from_spec(spec)
-            try:
-                spec.loader.exec_module(mod)
-            except Exception:      # optional eval-only dependencies (imageio, lpips, ...) missing
-                return None
-            return mod
-    return None
-
-
-_ref = _load_reference_renderer()
-if _ref is not None:
-    for _name in ("compute_rescale_ratio", "evaluation_iter_TensoIR", "evaluation_iter_TensoIR_simple",
-                  "evaluation_iter_TensoIR_general_multi_lights"):
-        if hasattr(_ref, _name):
-            globals()[_name] = getattr(_ref, _name)

@@ -461,6 +461,38 @@ int tir_tv_loss_bwd(const TirTvPlane* planes, int32_t n_planes, const float* gou
 int tir_generate_rays(const float* c2w, const int32_t* view_idx, const int32_t* pix_idx, int64_t n, int32_t H, int32_t W,
                       float focal, float* rays, void* stream);
 
+/* Test-view metrics of one rendered view (renderer.py:211-501, utils.py:93-139) from the device maps the renderer
+ * returns, [H*W,3] in row-major pixel order.  out[TIR_EVAL_N_OUT] (fp64, device, overwritten):
+ *   0 sum (clamp01(rgb) - gt_rgb)^2              1 sum (clamp01(rgb_brdf) - gt_rgb)^2          (over H*W*3)
+ *   2 sum (gt_albedo^g - single_aligned^g)^2      3 sum (gt_albedo^g - three_aligned^g)^2       (g = 1/2.2)
+ *   4 sum over all pixels of the normal angular error in degrees
+ *   5..8 SSIM of rgb/gt_rgb, rgb_brdf/gt_rgb, single_aligned/gt_albedo, three_aligned/gt_albedo (mean over the
+ *        (H-10)*(W-10)*3 valid windows; needs H, W >= 11 and ssim != 0, else 0; 7 and 8 need the albedo terms)
+ * Terms whose inputs are NULL are skipped and left 0.  The aligned albedo maps (clamp(ratio * albedo, 0, 1) inside
+ * gt_mask, 1 outside; ratio[0] for the single-channel and ratio[1..3] for the three-channel variant, in device memory)
+ * are written to aligned_single / aligned_three.  Every reduction is fixed-order (per-block fp64 partials in `work`,
+ * then one ordered pass): two calls on the same inputs return bit-identical outputs.  work holds
+ * tir_eval_work_size(H, W) doubles. */
+#define TIR_EVAL_N_OUT 9
+typedef struct TirEvalView {
+  int32_t H, W;
+  int32_t ssim;                           /* != 0: compute the four SSIMs */
+  int32_t reserved;
+  const float* rgb;                       /* required */
+  const float* rgb_brdf;                  /* required */
+  const float* gt_rgb;                    /* required */
+  const float* albedo;                    /* albedo terms: albedo, gt_albedo, gt_mask, ratio, aligned_* all set, */
+  const float* gt_albedo;                 /*   or albedo and gt_albedo both NULL                                   */
+  const uint8_t* gt_mask;                 /* [H*W] bool */
+  const float* ratio;                     /* [4]: single-channel ratio, three-channel ratio */
+  float* aligned_single;                  /* [H*W,3] out */
+  float* aligned_three;                   /* [H*W,3] out */
+  const float* normal;                    /* normal term: both set, or both NULL */
+  const float* gt_normal;
+} TirEvalView;
+int tir_eval_work_size(int32_t H, int32_t W, int64_t* n_doubles);
+int tir_eval_view(const TirEvalView* view, double* work, int64_t work_cap, double* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -8,5 +8,7 @@ from .tensorf import TensorVMSplit, AlphaGridMask, raw2alpha            # noqa: 
 from .tensorf_init import TensorVMSplit as TensorVMSplitInit            # noqa: F401
 from .renderer import Renderer_TensoIR_train, OctreeRender_trilinear_fast  # noqa: F401
 from . import relight_utils                                              # noqa: F401
+from .evaluation import (compute_rescale_ratio, evaluation_iter_TensoIR, evaluation_iter_TensoIR_simple,  # noqa: F401
+                         evaluation_iter_TensoIR_general_multi_lights)
 
 __version__ = "0.1.0"

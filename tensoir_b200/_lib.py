@@ -104,6 +104,14 @@ class TirPrimaryGrads(C.Structure):
                 + [(k, C.c_void_p * MAX_HEADS) for k in ("w0", "b0", "w1", "b1", "w2", "b2")])
 
 
+# ---- test-view metrics (csrc/tir_eval.cu) ------------------------------------------------------------------------------
+class TirEvalView(C.Structure):
+    _fields_ = ([("H", C.c_int32), ("W", C.c_int32), ("ssim", C.c_int32), ("reserved", C.c_int32)]
+                + [(k, C.c_void_p) for k in ("rgb", "rgb_brdf", "gt_rgb", "albedo", "gt_albedo", "gt_mask", "ratio",
+                                             "aligned_single", "aligned_three", "normal", "gt_normal")])
+
+
+EVAL_N_OUT = 9         # TIR_EVAL_N_OUT
 
 EXPORTS = {
     "tir_abi_version": (C.c_int, []),
@@ -187,6 +195,8 @@ EXPORTS = {
                                    C.c_void_p, f32p, C.c_void_p]),
     "tir_epilogue_bwd": (C.c_int, [C.c_int64, f32p, f32p, f32p, f32p, C.c_float, C.c_int32, C.POINTER(TirRayMaps),
                                    f32p, f32p, f32p, f32p, f32p, C.c_void_p]),
+    "tir_eval_work_size": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(C.c_int64)]),
+    "tir_eval_view": (C.c_int, [C.POINTER(TirEvalView), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
 }
 
 # kernels launched per entry point (for bench.py's gpu_launches claim)
@@ -201,7 +211,7 @@ KERNELS_PER_CALL = {"tir_pack_channels_last": 1, "tir_unpack_channels_last_add":
                     "tir_primary_march": 6, "tir_primary_app_list": 1, "tir_primary_heads": 5,
                     "tir_primary_backward": 9,
                     "tir_composite_bwd": 1, "tir_tail_fwd": 1, "tir_tail_bwd": 1, "tir_epilogue_fwd": 1,
-                    "tir_epilogue_bwd": 1}
+                    "tir_epilogue_bwd": 1, "tir_eval_view": 3}
 launch_count = 0
 
 _lib = None

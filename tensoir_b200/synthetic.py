@@ -185,3 +185,97 @@ def make_lego_model(grid: int, device, *, lights=("000",), general=False, mask_r
 def n_samples_for(grid: int, step_ratio: float = 0.5, cap: int = 1000000) -> int:
     """min(args.nSamples, cal_n_samples(reso, step_ratio)) (train_tensoIR.py:161, utils.py:63-64)."""
     return min(cap, int(np.linalg.norm([grid] * 3) / step_ratio))
+
+
+# per-box albedo of the synthetic test views (base plate, studs, arch, wall, block), linear RGB
+_BOX_ALBEDO = ((0.70, 0.12, 0.10), (0.85, 0.75, 0.20), (0.15, 0.35, 0.75), (0.30, 0.65, 0.30), (0.55, 0.55, 0.60))
+
+
+def _box_albedo(b: int) -> Tuple[float, float, float]:
+    if b == 0:
+        return _BOX_ALBEDO[0]
+    if b <= 12:
+        return _BOX_ALBEDO[1]
+    if b <= 15:
+        return _BOX_ALBEDO[2]
+    return _BOX_ALBEDO[3] if b == 16 else _BOX_ALBEDO[4]
+
+
+def trace_boxes(rays: torch.Tensor):
+    """Nearest hit of each ray [n,6] with the lego boxes (slab test, fp64): (hit [n] bool, box id [n] long,
+    face normal [n,3] float32, pointing against the ray)."""
+    o, d = rays[:, :3].double(), rays[:, 3:6].double()
+    n = rays.shape[0]
+    best = torch.full((n,), float("inf"), dtype=torch.float64)
+    box = torch.full((n,), -1, dtype=torch.long)
+    axis = torch.zeros(n, dtype=torch.long)
+    inv = 1.0 / torch.where(d == 0, torch.full_like(d, 1e-30), d)
+    for b, (lo, hi, _) in enumerate(_lego_boxes()):
+        t0 = (torch.tensor(lo, dtype=torch.float64) - o) * inv
+        t1 = (torch.tensor(hi, dtype=torch.float64) - o) * inv
+        tn = torch.minimum(t0, t1)
+        t_in, ax = tn.max(dim=1)
+        t_out = torch.maximum(t0, t1).min(dim=1).values
+        hit = (t_in <= t_out) & (t_in > 0) & (t_in < best)
+        best = torch.where(hit, t_in, best)
+        box = torch.where(hit, torch.full_like(box, b), box)
+        axis = torch.where(hit, ax, axis)
+    found = box >= 0
+    normal = torch.zeros(n, 3)
+    sgn = -torch.sign(d.gather(1, axis[:, None])).float()
+    normal.scatter_(1, axis[:, None], sgn)
+    normal[~found] = 0.0
+    return found, box, normal
+
+
+class SyntheticViews:
+    """Test views of the lego box scene with analytic ground truth, following the item contract of the reference's test
+    dataset (dataLoader/tensoIR_rotation_setting.py:180-245).  Item i, for camera ``poses[i]``:
+        rays [H*W,6], rgbs [L,H*W,3], light_idx [L,H*W,1] int32, rgbs_mask [H*W,1] bool, albedo [H*W,3],
+        normals [H*W,3] (background (0,0,1)), img_wh, c2w, w2c.
+    The mask, albedo and face normals come from ray-box intersection; rgb is albedo times a Lambert shading
+    0.25 + 0.75 max(n.l, 0) under light l (a sun direction rotated by 360 l / L degrees about z), over white."""
+
+    def __init__(self, poses: torch.Tensor, H: int, W: int, n_lights: int = 1, cam_angle_x: float = 0.6911,
+                 near_far=(2.0, 6.0)):
+        self.poses = poses.float()
+        self.img_wh = (int(W), int(H))
+        self.near_far = list(near_far)
+        self.white_bg = True
+        self.lights_probes = None
+        self.n_lights = int(n_lights)
+        self.cam_angle_x = cam_angle_x
+        self.focal = 0.5 * W / math.tan(0.5 * cam_angle_x)
+
+    def __len__(self):
+        return int(self.poses.shape[0])
+
+    def __getitem__(self, i):
+        W, H = self.img_wh
+        c2w = self.poses[i]
+        focal = self.focal
+        pix = torch.arange(H * W)
+        u = (pix % W).float() + 0.5
+        v = (pix // W).float() + 0.5
+        d = torch.stack([(u - W / 2) / focal, (v - H / 2) / focal, torch.ones_like(u)], -1)
+        d = d / torch.norm(d, dim=-1, keepdim=True)
+        rays = torch.cat([c2w[:3, 3].expand(H * W, 3), d @ c2w[:3, :3].T], 1)
+        hit, box, normal = trace_boxes(rays)
+        alb_tab = torch.tensor([_box_albedo(b) for b in range(len(_lego_boxes()))])
+        albedo = torch.ones(H * W, 3)
+        albedo[hit] = alb_tab[box[hit]]
+        normals = torch.tensor([0.0, 0.0, 1.0]).expand(H * W, 3).clone()
+        normals[hit] = normal[hit]
+        rgbs = []
+        for l in range(self.n_lights):
+            a = 2 * math.pi * l / self.n_lights
+            sun = torch.tensor([0.5 * math.cos(a), 0.5 * math.sin(a), 0.8])
+            sun = sun / sun.norm()
+            shade = 0.25 + 0.75 * (normal @ sun).clamp(min=0.0)
+            rgb = torch.ones(H * W, 3)
+            rgb[hit] = albedo[hit] * shade[hit, None]
+            rgbs.append(rgb)
+        light_idx = torch.arange(self.n_lights, dtype=torch.int32).view(-1, 1, 1).expand(-1, H * W, 1).contiguous()
+        return {'img_wh': self.img_wh, 'light_idx': light_idx, 'rgbs': torch.stack(rgbs, 0),
+                'rgbs_mask': hit.view(-1, 1), 'albedo': albedo, 'rays': rays, 'normals': normals,
+                'c2w': c2w, 'w2c': torch.linalg.inv(c2w)}
