@@ -493,6 +493,51 @@ typedef struct TirEvalView {
 int tir_eval_work_size(int32_t H, int32_t W, int64_t* n_doubles);
 int tir_eval_view(const TirEvalView* view, double* work, int64_t work_cap, double* out, void* stream);
 
+/* Metrics of P image pairs (relight_importance.py:216-219): a, b [P,H,W,3] fp32, out[P,2] (fp64, device, overwritten)
+ * = per pair the squared-error sum over H*W*3 ((a-b)^2 in fp32, summed in fp64) and the mean SSIM of utils.rgb_ssim
+ * (the same pass and the same fixed-order partials as tir_eval_view, so a pair gives the same bits through either
+ * entry point).  Needs H, W >= 11.  work holds tir_eval_pairs_work_size(P, H, W) doubles. */
+int tir_eval_pairs_work_size(int32_t P, int32_t H, int32_t W, int64_t* n_doubles);
+int tir_eval_pairs(const float* a, const float* b, int32_t P, int32_t H, int32_t W, double* work, int64_t work_cap,
+                   double* out, void* stream);
+
+/* ---- relighting under environment maps (scripts/relight_importance.py:99-181, Environment_Light of
+ * models/relight_utils.py:110-205) ------------------------------------------------------------------------------------
+ * One chunk of n primary rays, L environment maps, S importance samples per surface hit, in two calls around the
+ * existing density march (tir_march_density with the 96-sample equal-z table over [0.05, 1.5]):
+ *   tir_relight_sample  per (map, ray, sample) of a hit ray (acc > acc_mask_threshold): bin = upper bound of u in the
+ *                       map's CDF, clamped to H*W-1 (torch.searchsorted(cdf, u, right=True).clamp(max=H*W-1)); the
+ *                       sample is appended to the visibility list (origin o + depth*d, direction hdr_dir[bin]) when
+ *                       cosine = dir . normal (raw normal) > 1e-6.  bin[L,n,S] and pos[L,n,S] (list row, or -1) are
+ *                       written for every slot (bin 0 / pos -1 on non-hit rays).  The list length is accumulated in
+ *                       *count (device, caller zeroes); rows past `capacity` are not written (pos -1) but counted.
+ *   tir_relight_shade   one warp per (map, ray): mean over S of (albedo*rescale/pi + GGX) * vis * rgb[bin] * cosine /
+ *                       pdf_return[bin] with vis = vis_list[pos] (vis_kind 0, nerv: the march's t_last) or
+ *                       1 - vis_list[pos] (vis_kind 1, nerfactor: the march's acc), 0 where pos < 0; clamp, sRGB.
+ *                       Non-hit rays are white.  The background of every ray is the bilinear (align_corners, zero
+ *                       padding) lookup of get_light, clamped and sRGB; with_bg = acc_t*without_bg + (1-acc_t)*bg with
+ *                       acc_t = acc > 0.9 ? acc : 0.  Rows are written at [l, row0 + i] of [L, out_rows, 3] maps.
+ * Every reduction is in a fixed order (no float atomics): repeated calls give identical bits. */
+#define TIR_RELIGHT_MAX_LIGHTS 16
+typedef struct TirEnvMap {
+  int32_t H, W;
+  const float* rgb;         /* [H*W,3] hdr_rgbs */
+  const float* dir;         /* [H*W,3] hdr_dir */
+  const float* pdf_return;  /* [H*W]   hdr_pdf_return */
+  const double* cdf;        /* [H*W]   normalised cumulative sum of hdr_pdf_sample (last entry 1) */
+} TirEnvMap;
+int tir_relight_sample(const TirEnvMap* envs /* host array [n_lights] */, int32_t n_lights, const float* rays,
+                       const float* depth, const float* normal, const float* acc, int64_t n, int32_t n_samples,
+                       float acc_mask_threshold, const double* u /* [L,n,S] */, int32_t* bin, int32_t* pos,
+                       float* list_o, float* list_d /* [capacity,3] */, int64_t capacity, int64_t* count,
+                       void* stream);
+int tir_relight_shade(const TirEnvMap* envs, int32_t n_lights, const float* rays, const float* normal,
+                      const float* albedo, const float* rough, int32_t rough_stride /* 1: [n,1], 3: [n,3] */,
+                      const float* fresnel, const float* acc, int64_t n, int32_t n_samples, float acc_mask_threshold,
+                      const float* rescale /* [3] */, const int32_t* bin, const int32_t* pos, const float* vis_list,
+                      int32_t vis_kind, float* with_bg, float* without_bg, int64_t out_rows, int64_t row0,
+                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif

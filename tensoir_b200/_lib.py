@@ -113,6 +113,14 @@ class TirEvalView(C.Structure):
 
 EVAL_N_OUT = 9         # TIR_EVAL_N_OUT
 
+
+# ---- relighting (csrc/tir_relight.cu) ----------------------------------------------------------------------------------
+class TirEnvMap(C.Structure):
+    _fields_ = [("H", C.c_int32), ("W", C.c_int32)] + [(k, C.c_void_p) for k in ("rgb", "dir", "pdf_return", "cdf")]
+
+
+RELIGHT_MAX_LIGHTS = 16   # TIR_RELIGHT_MAX_LIGHTS
+
 EXPORTS = {
     "tir_abi_version": (C.c_int, []),
     "tir_pack_channels_last": (C.c_int, [f32p, f32p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
@@ -197,6 +205,15 @@ EXPORTS = {
                                    f32p, f32p, f32p, f32p, f32p, C.c_void_p]),
     "tir_eval_work_size": (C.c_int, [C.c_int32, C.c_int32, C.POINTER(C.c_int64)]),
     "tir_eval_view": (C.c_int, [C.POINTER(TirEvalView), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "tir_eval_pairs_work_size": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int64)]),
+    "tir_eval_pairs": (C.c_int, [f32p, f32p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p,
+                                 C.c_void_p]),
+    "tir_relight_sample": (C.c_int, [C.POINTER(TirEnvMap), C.c_int32, f32p, f32p, f32p, f32p, C.c_int64, C.c_int32,
+                                     C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, f32p, f32p, C.c_int64, C.c_void_p,
+                                     C.c_void_p]),
+    "tir_relight_shade": (C.c_int, [C.POINTER(TirEnvMap), C.c_int32, f32p, f32p, f32p, f32p, C.c_int32, f32p, f32p,
+                                    C.c_int64, C.c_int32, C.c_float, f32p, C.c_void_p, C.c_void_p, f32p, C.c_int32,
+                                    f32p, f32p, C.c_int64, C.c_int64, C.c_void_p]),
 }
 
 # kernels launched per entry point (for bench.py's gpu_launches claim)
@@ -211,7 +228,7 @@ KERNELS_PER_CALL = {"tir_pack_channels_last": 1, "tir_unpack_channels_last_add":
                     "tir_primary_march": 6, "tir_primary_app_list": 1, "tir_primary_heads": 5,
                     "tir_primary_backward": 9,
                     "tir_composite_bwd": 1, "tir_tail_fwd": 1, "tir_tail_bwd": 1, "tir_epilogue_fwd": 1,
-                    "tir_epilogue_bwd": 1, "tir_eval_view": 3}
+                    "tir_epilogue_bwd": 1, "tir_eval_view": 3, "tir_relight_sample": 1, "tir_relight_shade": 1}
 launch_count = 0
 
 _lib = None

@@ -73,22 +73,32 @@ __global__ void __launch_bounds__(kThreads) eval_pixel_kernel(TirEvalView v, boo
   }
 }
 
-// blockIdx.z: pair 0 rgb/gt_rgb, 1 rgb_brdf/gt_rgb, 2 aligned_single/gt_albedo, 3 aligned_three/gt_albedo
-__global__ void __launch_bounds__(kThreads) eval_ssim_kernel(TirEvalView v, int64_t n_tiles,
+// A batch of SSIM pairs for one launch (blockIdx.z indexes it): image a (clamped to [0,1] first when clamp_a), image b,
+// both [H*W,3]; their partials go to part[(first + z) * n_tiles + tile].
+constexpr int kPairsPerLaunch = 8;
+struct SsimPairs {
+  const float* a[kPairsPerLaunch];
+  const float* b[kPairsPerLaunch];
+  int clamp_a[kPairsPerLaunch];
+  int first;
+};
+
+__global__ void __launch_bounds__(kThreads) eval_ssim_kernel(int32_t H, int32_t W, SsimPairs pairs, int64_t n_tiles,
                                                              double* __restrict__ part) {
   __shared__ float sx[kIn][kIn + 1], sy[kIn][kIn + 1];
   __shared__ double sv[5][EVAL_TILE][kIn];
   __shared__ double taps[EVAL_WIN];
   __shared__ double red[kThreads];
-  const int pair = blockIdx.z;
-  const float* a = pair == 0 ? v.rgb : pair == 1 ? v.rgb_brdf : pair == 2 ? v.aligned_single : v.aligned_three;
-  const float* b = pair < 2 ? v.gt_rgb : v.gt_albedo;
-  const bool clamp_a = pair < 2;                              // the renderer maps are clamped before the metrics
+  const int z = blockIdx.z;
+  const int pair = pairs.first + z;
+  const float* a = pairs.a[z];
+  const float* b = pairs.b[z];
+  const bool clamp_a = pairs.clamp_a[z] != 0;
   const int x0 = blockIdx.x * EVAL_TILE, y0 = blockIdx.y * EVAL_TILE;
   const int t = threadIdx.x;
   if (t < EVAL_WIN) taps[t] = eval_tap(t);
   const int ty = t / EVAL_TILE, tx = t % EVAL_TILE;
-  const bool out_ok = (y0 + ty) < v.H - EVAL_HALO && (x0 + tx) < v.W - EVAL_HALO;
+  const bool out_ok = (y0 + ty) < H - EVAL_HALO && (x0 + tx) < W - EVAL_HALO;
   double acc = 0.0;
   for (int c = 0; c < 3; ++c) {
     __syncthreads();
@@ -96,8 +106,8 @@ __global__ void __launch_bounds__(kThreads) eval_ssim_kernel(TirEvalView v, int6
       const int r = k / kIn, col = k % kIn;
       const int gy = y0 + r, gx = x0 + col;
       float xa = 0.f, xb = 0.f;
-      if (gy < v.H && gx < v.W) {
-        const int64_t pix = (int64_t)gy * v.W + gx;
+      if (gy < H && gx < W) {
+        const int64_t pix = (int64_t)gy * W + gx;
         xa = a[pix * 3 + c];
         xb = b[pix * 3 + c];
         if (clamp_a) xa = ev_clamp01(xa);
@@ -159,7 +169,71 @@ __global__ void __launch_bounds__(kThreads) eval_finalize_kernel(const double* _
   }
 }
 
+// squared-error partials of pair blockIdx.y: (a - b)^2 in fp32, fp64 sums in a fixed order
+__global__ void __launch_bounds__(kThreads) eval_pair_sse_kernel(const float* __restrict__ a,
+                                                                 const float* __restrict__ b, int64_t n,
+                                                                 double* __restrict__ part) {
+  __shared__ double red[kThreads];
+  const int64_t off = (int64_t)blockIdx.y * n;
+  double acc = 0.0;
+  for (int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x; i < n; i += (int64_t)gridDim.x * kThreads) {
+    const float d = ev_sub(a[off + i], b[off + i]);
+    acc += (double)ev_mul(d, d);
+  }
+  const double s = block_sum_det(acc, red);
+  if (threadIdx.x == 0) part[(int64_t)blockIdx.y * EVAL_PAIR_SSE_BLOCKS + blockIdx.x] = s;
+}
+
+// one block per pair: out[p] = {sse, mean ssim}
+__global__ void __launch_bounds__(kThreads) eval_pairs_finalize_kernel(const double* __restrict__ work,
+                                                                       int64_t n_tiles, double n_windows,
+                                                                       double* __restrict__ out) {
+  __shared__ double red[kThreads];
+  const int p = blockIdx.x;
+  double v = 0.0;
+  for (int k = threadIdx.x; k < EVAL_PAIR_SSE_BLOCKS; k += kThreads) v += work[(int64_t)p * EVAL_PAIR_SSE_BLOCKS + k];
+  const double sse = block_sum_det(v, red);
+  const double* part = work + (int64_t)gridDim.x * EVAL_PAIR_SSE_BLOCKS;
+  v = 0.0;
+  for (int64_t k = threadIdx.x; k < n_tiles; k += kThreads) v += part[p * n_tiles + k];
+  const double ss = block_sum_det(v, red);
+  if (threadIdx.x == 0) { out[2 * p] = sse; out[2 * p + 1] = ss / n_windows; }
+}
+
 }  // namespace
+
+extern "C" int tir_eval_pairs_work_size(int32_t P, int32_t H, int32_t W, int64_t* n_doubles) {
+  if (!n_doubles) return TIR_ERR_NULL;
+  if (P < 0 || H < 0 || W < 0) return TIR_ERR_SHAPE;
+  *n_doubles = eval_pairs_work_doubles(P, H, W);
+  return TIR_OK;
+}
+
+extern "C" int tir_eval_pairs(const float* a, const float* b, int32_t P, int32_t H, int32_t W, double* work,
+                              int64_t work_cap, double* out, void* stream) {
+  const int rc = eval_pairs_validate(a, b, P, H, W, work, work_cap, out);
+  if (rc <= 0) return rc;
+  cudaStream_t s = (cudaStream_t)stream;
+  const int64_t n = (int64_t)H * W * 3;
+  const int64_t n_tiles = eval_ssim_tiles(H, W);
+  eval_pair_sse_kernel<<<dim3(EVAL_PAIR_SSE_BLOCKS, P), kThreads, 0, s>>>(a, b, n, work);
+  double* part = work + (int64_t)P * EVAL_PAIR_SSE_BLOCKS;
+  for (int first = 0; first < P; first += kPairsPerLaunch) {
+    SsimPairs pairs{};
+    const int m = P - first < kPairsPerLaunch ? P - first : kPairsPerLaunch;
+    for (int z = 0; z < m; ++z) {
+      pairs.a[z] = a + (int64_t)(first + z) * n;
+      pairs.b[z] = b + (int64_t)(first + z) * n;
+      pairs.clamp_a[z] = 0;
+    }
+    pairs.first = first;
+    const dim3 grid((W - EVAL_HALO + EVAL_TILE - 1) / EVAL_TILE, (H - EVAL_HALO + EVAL_TILE - 1) / EVAL_TILE, m);
+    eval_ssim_kernel<<<grid, kThreads, 0, s>>>(H, W, pairs, n_tiles, part);
+  }
+  const double n_windows = (double)(H - EVAL_HALO) * (double)(W - EVAL_HALO) * 3.0;
+  eval_pairs_finalize_kernel<<<P, kThreads, 0, s>>>(work, n_tiles, n_windows, out);
+  return (int)cudaGetLastError();
+}
 
 extern "C" int tir_eval_work_size(int32_t H, int32_t W, int64_t* n_doubles) {
   if (!n_doubles) return TIR_ERR_NULL;
@@ -181,7 +255,11 @@ extern "C" int tir_eval_view(const TirEvalView* view, double* work, int64_t work
   eval_pixel_kernel<<<EVAL_PIX_BLOCKS, kThreads, 0, s>>>(v, has_albedo, has_normal, work);
   if (n_ssim) {
     const dim3 grid((v.W - EVAL_HALO + EVAL_TILE - 1) / EVAL_TILE, (v.H - EVAL_HALO + EVAL_TILE - 1) / EVAL_TILE, n_ssim);
-    eval_ssim_kernel<<<grid, kThreads, 0, s>>>(v, n_tiles, work + EVAL_N_PIX * EVAL_PIX_BLOCKS);
+    // pair 0 rgb/gt_rgb, 1 rgb_brdf/gt_rgb (the renderer maps are clamped before the metrics),
+    // 2 aligned_single/gt_albedo, 3 aligned_three/gt_albedo
+    SsimPairs pairs{{v.rgb, v.rgb_brdf, v.aligned_single, v.aligned_three},
+                    {v.gt_rgb, v.gt_rgb, v.gt_albedo, v.gt_albedo}, {1, 1, 0, 0}, 0};
+    eval_ssim_kernel<<<grid, kThreads, 0, s>>>(v.H, v.W, pairs, n_tiles, work + EVAL_N_PIX * EVAL_PIX_BLOCKS);
   }
   const double n_windows = (double)(v.H - EVAL_HALO) * (double)(v.W - EVAL_HALO) * 3.0;
   eval_finalize_kernel<<<1, kThreads, 0, s>>>(work, n_tiles, n_ssim, n_windows, out);

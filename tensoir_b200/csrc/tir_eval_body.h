@@ -150,6 +150,24 @@ inline int eval_validate(const TirEvalView* v, bool* has_albedo, bool* has_norma
   return 1;
 }
 
+// ---- tir_eval_pairs: [P * EVAL_PAIR_SSE_BLOCKS] squared-error partials, then [P * tiles] SSIM partials -------------
+#define EVAL_PAIR_SSE_BLOCKS 64
+
+inline int64_t eval_pairs_work_doubles(int32_t P, int32_t H, int32_t W) {
+  return (int64_t)P * (EVAL_PAIR_SSE_BLOCKS + eval_ssim_tiles(H, W));
+}
+
+// 1: run, 0: nothing to do (no pairs), < 0: TirStatus
+inline int eval_pairs_validate(const float* a, const float* b, int32_t P, int32_t H, int32_t W, const double* work,
+                               int64_t work_cap, const double* out) {
+  if (P < 0 || H < 0 || W < 0) return TIR_ERR_SHAPE;
+  if (P == 0) return 0;
+  if (H < EVAL_WIN || W < EVAL_WIN) return TIR_ERR_SHAPE;
+  if (!a || !b || !work || !out) return TIR_ERR_NULL;
+  if (work_cap < eval_pairs_work_doubles(P, H, W)) return TIR_ERR_CAPACITY;
+  return 1;
+}
+
 // SSIM of one window from the blurred moments E[x], E[y], E[x^2], E[y^2], E[xy] (utils.py:118-137, max_val = 1)
 EVAL_HD double eval_ssim_point(double mu0, double mu1, double e00, double e11, double e01) {
   const double mu00 = mu0 * mu0, mu11 = mu1 * mu1, mu01 = mu0 * mu1;

@@ -4,12 +4,12 @@
 // each: one warp per surface point, lanes stride over the directions.  Replaces ~60 forward + ~120 backward
 // element-wise / reduction launches on [bs, n_dirs, 3] tensors.
 #include "tir_device.cuh"
+#include "tir_ggx.h"
 
 using namespace tir;
 
 namespace {
 
-constexpr float kPi = 3.14159265358979323846f;
 constexpr int kWarps = 8;
 
 struct ShadeParams {
@@ -43,78 +43,27 @@ struct ShadeParams {
   float* lin;             // [bs,3] linear value before clamp / sRGB (saved by the forward, read by the backward)
 };
 
-// linear2srgb_torch after the [0,1] clip (relight_utils.py:489-515) and its derivative
-__device__ __forceinline__ float tone(float x, int srgb) {
-  const float t = fminf(fmaxf(x, 0.f), 1.f);
-  if (!srgb) return t;
-  return t <= 0.0031308f ? t * 12.92f : 1.055f * powf(t + 1e-6f, 1.f / 2.4f) - 0.055f;
-}
 __device__ __forceinline__ float tone_grad(float x, int srgb) {
   if (!(x >= 0.f && x <= 1.f)) return 0.f;          // torch.clamp passes the gradient on [min, max]
   if (!srgb) return 1.f;
   return x <= 0.0031308f ? 12.92f : 1.055f / 2.4f * powf(x + 1e-6f, 1.f / 2.4f - 1.f);
 }
 
-__device__ __forceinline__ float clamp01e6(float x) { return fminf(fmaxf(x, 1e-6f), 1.f); }
-__device__ __forceinline__ bool in_clamp(float x) { return (x >= 1e-6f) & (x <= 1.f); }
-
-struct PointCtx {
-  float n[3], Np[3], V[3], inv_nn, sgn, NoV, NoV_raw;
-  float a[3], F0[3], r[3], alpha2[3], k[3], nom1[3];
-};
-
+// PointCtx / DirCtx and their arithmetic live in tir_ggx.h (shared with the relighting kernel); these load the inputs
 __device__ __forceinline__ void load_point(const ShadeParams& p, int64_t i, PointCtx& c) {
-  float nn = 0.f, vn = 0.f;
 #pragma unroll
   for (int d = 0; d < 3; ++d) {
     c.n[d] = p.normal[i * 3 + d]; c.V[d] = p.rays ? -p.rays[i * 6 + 3 + d] : p.view[i * 3 + d];
     c.a[d] = p.albedo[i * 3 + d]; c.F0[d] = p.fresnel[i * 3 + d];
     c.r[d] = p.rough_stride == 1 ? p.rough[i] : p.rough[i * 3 + d];
-    nn += c.n[d] * c.n[d]; vn += c.V[d] * c.V[d];
   }
-  c.inv_nn = 1.f / fmaxf(sqrtf(nn), 1e-12f);
-  const float inv_vn = 1.f / fmaxf(sqrtf(vn), 1e-12f);
-  float nov = 0.f;
-#pragma unroll
-  for (int d = 0; d < 3; ++d) { c.V[d] *= inv_vn; nov += c.V[d] * c.n[d] * c.inv_nn; }
-  c.sgn = (nov > 0.f) ? 1.f : ((nov < 0.f) ? -1.f : 0.f);
-  float nov2 = 0.f;
-#pragma unroll
-  for (int d = 0; d < 3; ++d) { c.Np[d] = c.n[d] * c.inv_nn * c.sgn; nov2 += c.Np[d] * c.V[d]; }
-  c.NoV_raw = nov2;
-  c.NoV = clamp01e6(nov2);
-#pragma unroll
-  for (int ch = 0; ch < 3; ++ch) {
-    const float al = c.r[ch] * c.r[ch];
-    c.alpha2[ch] = al * al;
-    c.k[ch] = (al + 2.f * c.r[ch] + 1.f) / 8.f;
-    c.nom1[ch] = c.NoV * (1.f - c.k[ch]) + c.k[ch];
-  }
+  ggx_point(c);
 }
 
-struct DirCtx {
-  float L[3], H[3], cosr, cosv, NoL_raw, NoH_raw, VoH_raw, NoL, NoH, VoH, p2;
-};
-
 __device__ __forceinline__ void load_dir(const ShadeParams& p, const PointCtx& c, int l, DirCtx& d) {
-  float ln = 0.f;
 #pragma unroll
-  for (int e = 0; e < 3; ++e) { d.L[e] = __ldg(p.dirs + l * 3 + e); ln += d.L[e] * d.L[e]; }
-  d.cosr = d.L[0] * c.n[0] + d.L[1] * c.n[1] + d.L[2] * c.n[2];    // cosine uses the un-normalised direction
-  d.cosv = fmaxf(d.cosr, 0.f);
-  const float inv_ln = 1.f / fmaxf(sqrtf(ln), 1e-12f);
-  float hn = 0.f;
-#pragma unroll
-  for (int e = 0; e < 3; ++e) { d.L[e] *= inv_ln; d.H[e] = (d.L[e] + c.V[e]) * 0.5f; hn += d.H[e] * d.H[e]; }
-  const float inv_hn = 1.f / fmaxf(sqrtf(hn), 1e-12f);
-  d.NoL_raw = d.NoH_raw = d.VoH_raw = 0.f;
-#pragma unroll
-  for (int e = 0; e < 3; ++e) {
-    d.H[e] *= inv_hn;
-    d.NoL_raw += c.Np[e] * d.L[e]; d.NoH_raw += c.Np[e] * d.H[e]; d.VoH_raw += c.V[e] * d.H[e];
-  }
-  d.NoL = clamp01e6(d.NoL_raw); d.NoH = clamp01e6(d.NoH_raw); d.VoH = clamp01e6(d.VoH_raw);
-  d.p2 = exp2f((-5.55473f * d.VoH - 6.98316f) * d.VoH);
+  for (int e = 0; e < 3; ++e) d.L[e] = __ldg(p.dirs + l * 3 + e);
+  ggx_dir(c, d);
 }
 
 __global__ void __launch_bounds__(kWarps * 32) shade_fwd_kernel(const ShadeParams p) {
@@ -136,10 +85,8 @@ __global__ void __launch_bounds__(kWarps * 32) shade_fwd_kernel(const ShadeParam
     const float cw = d.cosv * __ldg(p.weight + l);
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) {
-      const float frac = (c.F0[ch] + (1.f - c.F0[ch]) * d.p2) * c.alpha2[ch];
-      const float nom0 = d.NoH * d.NoH * (c.alpha2[ch] - 1.f) + 1.f;
-      const float nom2 = d.NoL * (1.f - c.k[ch]) + c.k[ch];
-      const float nom = fminf(fmaxf(4.f * kPi * nom0 * nom0 * c.nom1[ch] * nom2, 1e-6f), 4.f * kPi);
+      float frac, nom;
+      ggx_terms(c, d, ch, frac, nom);
       const float brdf = c.a[ch] / kPi + frac / nom;
       const float light = v * __ldg(D + l * 3 + ch) + p.ind[(i * p.nl + l) * 3 + ch];
       acc[ch] += brdf * light * cw;

@@ -234,10 +234,18 @@ class SyntheticViews:
         rays [H*W,6], rgbs [L,H*W,3], light_idx [L,H*W,1] int32, rgbs_mask [H*W,1] bool, albedo [H*W,3],
         normals [H*W,3] (background (0,0,1)), img_wh, c2w, w2c.
     The mask, albedo and face normals come from ray-box intersection; rgb is albedo times a Lambert shading
-    0.25 + 0.75 max(n.l, 0) under light l (a sun direction rotated by 360 l / L degrees about z), over white."""
+    0.25 + 0.75 max(n.l, 0) under light l (a sun direction rotated by 360 l / L degrees about z), over white.
+
+    With ``light_names`` the views follow the reference's relighting test set instead
+    (dataLoader/tensoIR_relighting_test.py:217-228): ``split`` is 'test', ``light_names`` is the list, rgbs holds one
+    ground-truth image per name, light_idx is 0 everywhere and the item gains normals_white (background (1,1,1))."""
 
     def __init__(self, poses: torch.Tensor, H: int, W: int, n_lights: int = 1, cam_angle_x: float = 0.6911,
-                 near_far=(2.0, 6.0)):
+                 near_far=(2.0, 6.0), light_names=None):
+        if light_names is not None:
+            self.split = 'test'
+            self.light_names = list(light_names)
+            n_lights = len(self.light_names)
         self.poses = poses.float()
         self.img_wh = (int(W), int(H))
         self.near_far = list(near_far)
@@ -276,6 +284,12 @@ class SyntheticViews:
             rgb[hit] = albedo[hit] * shade[hit, None]
             rgbs.append(rgb)
         light_idx = torch.arange(self.n_lights, dtype=torch.int32).view(-1, 1, 1).expand(-1, H * W, 1).contiguous()
-        return {'img_wh': self.img_wh, 'light_idx': light_idx, 'rgbs': torch.stack(rgbs, 0),
+        item = {'img_wh': self.img_wh, 'light_idx': light_idx, 'rgbs': torch.stack(rgbs, 0),
                 'rgbs_mask': hit.view(-1, 1), 'albedo': albedo, 'rays': rays, 'normals': normals,
                 'c2w': c2w, 'w2c': torch.linalg.inv(c2w)}
+        if hasattr(self, 'light_names'):
+            item['light_idx'] = torch.zeros_like(light_idx)
+            normals_white = torch.ones(H * W, 3)
+            normals_white[hit] = normal[hit]
+            item['normals_white'] = normals_white
+        return item
