@@ -105,19 +105,22 @@ class OracleField:
             ps += list(self.lgt_sgs)
         return ps
 
-    def to(self, device):
+    def to(self, device=None, dtype=None):
+        """Move every tensor to ``device`` and/or cast it to ``dtype``.  The functions below create their
+        intermediates in the default dtype, so a float64 field is evaluated under
+        ``torch.set_default_dtype(torch.float64)``."""
         def mv(t):
-            return None if t is None else t.to(device)
+            return None if t is None else t.to(device=device, dtype=dtype)
         for name in ("aabb", "basis_w", "light_line_w", "alpha_volume", "alpha_aabb"):
             setattr(self, name, mv(getattr(self, name)))
         for name in ("density_plane", "density_line", "app_plane", "app_line"):
-            setattr(self, name, [t.to(device) for t in getattr(self, name)])
+            setattr(self, name, [mv(t) for t in getattr(self, name)])
         for name in ("mlp_rgb", "mlp_brdf", "mlp_normal"):
             m = getattr(self, name)
             if m is not None:
-                setattr(self, name, Mlp(*[t.to(device) for t in m.params()]))
+                setattr(self, name, Mlp(*[mv(t) for t in m.params()]))
         if self.lgt_sgs is not None:
-            self.lgt_sgs = [t.to(device) for t in self.lgt_sgs]
+            self.lgt_sgs = [mv(t) for t in self.lgt_sgs]
         return self
 
 

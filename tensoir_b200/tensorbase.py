@@ -300,9 +300,13 @@ class TensorBase(torch.nn.Module):
         self.invaabbSize = 2.0 / self.aabbSize
         self.gridSize = torch.LongTensor(gridSize).to(self.device)
         self.units = self.aabbSize / (self.gridSize - 1)
-        self.stepSize = torch.mean(self.units) * self.step_ratio
-        self.aabbDiag = torch.sqrt(torch.sum(torch.square(self.aabbSize)))
-        self.nSamples = int((self.aabbDiag / self.stepSize).item()) + 1
+        # the step and the diagonal are reduced on the host: on a non-cubic grid the three units differ, and a CUDA mean
+        # may round differently from the CPU one, which would move every sample position by an ulp of the step
+        size_h = self.aabbSize.detach().cpu()
+        step_h = torch.mean(size_h / (torch.LongTensor(gridSize) - 1)) * self.step_ratio
+        self.stepSize = step_h.to(self.device)
+        self.aabbDiag = torch.sqrt(torch.sum(torch.square(size_h))).to(self.device)
+        self.nSamples = int((torch.sqrt(torch.sum(torch.square(size_h))) / step_h).item()) + 1
         # host copies of the (device-resident) geometry so that kernel launches never sync on .tolist()/.item();
         # every path that changes aabb / gridSize (constructor, shrink, upsample) ends in update_stepSize
         self._host_geom = {"grid": [int(g) for g in self.gridSize.tolist()], "lo": self.aabb[0].tolist(),

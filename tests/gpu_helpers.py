@@ -15,6 +15,19 @@ def load_fixture(name):
     return fx
 
 
+def load_shrunk_state(state):
+    """State "A" or "B" of shrunk_g30.pt (tests/golden/make_shrunk_golden.py) as one flat fixture dict, in the layout
+    of rotated_g24.pt: the state's records plus the shared parameters, rays and light indices."""
+    fx = load_fixture("shrunk_g30.pt")
+    for key in ("state_dict", f"renderer_train_grads_{state}"):
+        fx[key] = {**fx.pop(f"{key}:factors"), **fx.pop(f"{key}:rest")}
+    out = {k: v for k, v in fx.items() if k != "states" and not k.startswith("renderer_train_grads_")}
+    out.update(fx["states"][state])
+    out["renderer_train_grads"] = fx[f"renderer_train_grads_{state}"]
+    out["state"] = state
+    return out
+
+
 def renderer_args(n=96, near=0.05, far=1.5):
     a = types.SimpleNamespace()
     a.second_nSample, a.second_near, a.second_far = n, near, far

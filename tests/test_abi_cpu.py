@@ -133,6 +133,26 @@ def test_regularisers_and_grid_maintenance_match_reference(golden_rotated):
     assert torch.equal(m.density_plane[1], up["density_plane1"]) and torch.equal(m.app_line[0], up["app_line0"])
 
 
+def test_shrink_and_upsample_reproduce_the_whole_reference_state(golden_rotated):
+    """shrink to an asymmetric box + upsample_volume_grid([30,31,29]) reproduce the reference's whole state_dict
+    (every factor, bit-exact), aabb, gridSize, nSamples and stepSize (shrunk_g30.pt, state A), and the host geometry
+    the kernels read follows all three axes."""
+    from gpu_helpers import load_shrunk_state, model_from_fixture
+    want = load_shrunk_state("A")
+    m = model_from_fixture(golden_rotated, "cpu")
+    m.shrink(want["shrink_box"].clone())
+    m.upsample_volume_grid(want["upsample"])
+    assert torch.equal(m.aabb, want["aabb"]) and m.gridSize.tolist() == want["grid_size"]
+    assert m.nSamples == want["nSamples"] and float(m.stepSize) == want["stepSize"]
+    sd = m.state_dict()
+    assert set(sd) == set(want["state_dict"])
+    for k, v in want["state_dict"].items():
+        assert sd[k].shape == v.shape and torch.equal(sd[k], v), k
+    hg = m._host_geom
+    assert hg["grid"] == [30, 31, 29] and hg["lo"] == want["aabb"][0].tolist()
+    assert hg["inv"] == (2.0 / (want["aabb"][1] - want["aabb"][0])).tolist()
+
+
 def test_importance_sampled_light_dirs_match_reference(golden_rotated):
     from gpu_helpers import model_from_fixture
     fx = golden_rotated
