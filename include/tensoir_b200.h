@@ -551,6 +551,24 @@ int tir_relight_shade(const TirEnvMap* envs, int32_t n_lights, const float* rays
                       int32_t vis_kind, float* with_bg, float* without_bg, int64_t out_rows, int64_t row0,
                       void* stream);
 
+/* ---- mesh export: marching cubes over a dense volume (utils.py:165-225, skimage.measure.marching_cubes on
+ * TensorBase.getDenseAlpha(), tensorBase_rotated_lights.py:737-753) ---------------------------------------------------
+ * volume [X,Y,Z] fp32 C-contiguous, X, Y, Z >= 2 and X*Y*Z <= INT32_MAX (TIR_ERR_SHAPE otherwise).  A point is inside
+ * iff v > level; the topology, vertex placement and winding are documented in csrc/tir_mc_body.h.
+ *   tir_marching_cubes_work_size  bytes of the caller's scratch `work` for an X x Y x Z volume;
+ *   tir_marching_cubes_count      totals[2] (device, int64, overwritten) = vertex and triangle counts; fills `work`;
+ *   tir_marching_cubes_emit       with the same volume, level and work: verts [n_verts,3] fp32 = (axis0, axis1, axis2)
+ *                                 coordinates scaled by (sx, sy, sz), faces [n_faces,3] int32.  n_verts / n_faces are
+ *                                 the counts read back from totals; a count above INT32_MAX is TIR_ERR_SHAPE.
+ * Vertices are ordered by (grid-point linear index, axis), faces by (cell linear index, loop order): reruns are
+ * bit-identical. */
+int tir_marching_cubes_work_size(int32_t X, int32_t Y, int32_t Z, int64_t* bytes);
+int tir_marching_cubes_count(const float* volume, int32_t X, int32_t Y, int32_t Z, float level, void* work,
+                             int64_t work_bytes, int64_t* totals, void* stream);
+int tir_marching_cubes_emit(const float* volume, int32_t X, int32_t Y, int32_t Z, float level, double sx, double sy,
+                            double sz, const void* work, int64_t work_bytes, int64_t n_verts, int64_t n_faces,
+                            float* verts, int32_t* faces, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -10,5 +10,6 @@ from .renderer import Renderer_TensoIR_train, OctreeRender_trilinear_fast  # noq
 from . import relight_utils                                              # noqa: F401
 from .evaluation import (compute_rescale_ratio, evaluation_iter_TensoIR, evaluation_iter_TensoIR_simple,  # noqa: F401
                          evaluation_iter_TensoIR_general_multi_lights)
+from .mesh import convert_sdf_samples_to_ply, export_mesh, marching_cubes                   # noqa: F401
 
 __version__ = "0.1.0"

@@ -216,6 +216,12 @@ EXPORTS = {
     "tir_relight_shade": (C.c_int, [C.POINTER(TirEnvMap), C.c_int32, f32p, f32p, f32p, f32p, C.c_int32, f32p, f32p,
                                     C.c_int64, C.c_int32, C.c_float, f32p, C.c_void_p, C.c_void_p, f32p, C.c_int32,
                                     f32p, f32p, C.c_int64, C.c_int64, C.c_void_p]),
+    "tir_marching_cubes_work_size": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int64)]),
+    "tir_marching_cubes_count": (C.c_int, [f32p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_int64,
+                                           C.c_void_p, C.c_void_p]),
+    "tir_marching_cubes_emit": (C.c_int, [f32p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_double, C.c_double,
+                                          C.c_double, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, f32p, C.c_void_p,
+                                          C.c_void_p]),
 }
 
 # kernels launched per entry point (for bench.py's gpu_launches claim)
@@ -230,7 +236,8 @@ KERNELS_PER_CALL = {"tir_pack_channels_last": 1, "tir_unpack_channels_last_add":
                     "tir_primary_march": 6, "tir_primary_app_list": 1, "tir_primary_heads": 5,
                     "tir_primary_backward": 9,
                     "tir_composite_bwd": 1, "tir_tail_fwd": 1, "tir_tail_bwd": 1, "tir_epilogue_fwd": 1,
-                    "tir_epilogue_bwd": 1, "tir_eval_view": 3, "tir_relight_sample": 1, "tir_relight_shade": 1}
+                    "tir_epilogue_bwd": 1, "tir_eval_view": 3, "tir_relight_sample": 1, "tir_relight_shade": 1,
+                    "tir_marching_cubes_count": 7, "tir_marching_cubes_emit": 2}
 launch_count = 0
 
 _lib = None
