@@ -433,6 +433,26 @@ int tir_primary_backward(const TirField* field, const TirHeadJob* jobs, int32_t 
                          const float* g_acc_map /* [n_rays] or NULL */, const float* g_loss_albedo,
                          const float* g_loss_rough, const TirPrimaryGrads* grads, void* stream);
 
+/* TensorBase.forward with is_relight=False (tensorBase_rotated_lights.py:868-986, the radiance-only warm-up phase of
+ * training) on the same march, appearance list and scratch: after tir_primary_march + tir_primary_app_list,
+ *   tir_primary_radiance           ONE head (role TIR_HEAD_RGB, point_set 0, x_in 0: renderModule on the view
+ *                                  direction) into work->out[0], then per ray rgb_map = sum w * rgb and, when
+ *                                  white_bg != 0, rgb_map += 1 - acc, depth_map = depth + (1 - acc) * rays[..., 5].
+ *                                  No clamp, no sRGB (the reference's radiance branch has neither).  rgb_map [n_rays,3],
+ *                                  depth_map [n_rays]; acc stays in work->acc.  work->noise, a_xj, packed, dn_* unused.
+ *   tir_primary_radiance_backward  epilogue -> per-sample tail -> head dgrad / wgrad (job slot 0 of bwork and grads) ->
+ *                                  appearance scatter -> compositing -> density scatter.  g_rgb_map [n_rays,3],
+ *                                  g_depth_map, g_acc_map [n_rays] may each be NULL (zero).  grads ACCUMULATED.
+ * Saving the activations for the backward needs work->x0[0], inp[0], h1[0], h2[0]; x0[1] is never read. */
+int tir_primary_radiance(const TirField* field, const TirHeadJob* job, const float* rays, const int32_t* light_idx,
+                         int64_t n_rays, const TirPrimaryWork* work, int32_t white_bg, float* rgb_map,
+                         float* depth_map, void* stream);
+int tir_primary_radiance_backward(const TirField* field, const TirHeadJob* job, const float* rays,
+                                  const int32_t* light_idx, int64_t n_rays, const TirPrimaryWork* work,
+                                  const TirPrimaryBwdWork* bwork, int32_t white_bg, const float* g_rgb_map,
+                                  const float* g_depth_map, const float* g_acc_map, const TirPrimaryGrads* grads,
+                                  void* stream);
+
 /* ---- optimiser pass (SURVEY.md 8 f3): torch.optim.Adam's update for a list of dense fp32 tensors in ONE launch, with
  * the L1 regulariser's gradient (l1 * sign(param), density_L1 of tensoRF_rotated_lights.py:74-78) folded in, the
  * gradient cleared for the next accumulation, and a device-side skip flag (found_inf != 0: parameters, moments and the

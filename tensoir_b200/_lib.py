@@ -198,6 +198,12 @@ EXPORTS = {
                                        C.c_void_p, C.c_int64, C.POINTER(TirPrimaryWork), C.POINTER(TirPrimaryBwdWork),
                                        C.c_float, C.c_int32, C.POINTER(TirRayMaps), C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.POINTER(TirPrimaryGrads), C.c_void_p]),
+    "tir_primary_radiance": (C.c_int, [C.POINTER(TirField), C.POINTER(TirHeadJob), C.c_void_p, C.c_void_p, C.c_int64,
+                                       C.POINTER(TirPrimaryWork), C.c_int32, f32p, f32p, C.c_void_p]),
+    "tir_primary_radiance_backward": (C.c_int, [C.POINTER(TirField), C.POINTER(TirHeadJob), C.c_void_p, C.c_void_p,
+                                                C.c_int64, C.POINTER(TirPrimaryWork), C.POINTER(TirPrimaryBwdWork),
+                                                C.c_int32, f32p, f32p, f32p, C.POINTER(TirPrimaryGrads),
+                                                C.c_void_p]),
     "tir_tail_fwd": (C.c_int, [C.c_int64, f32p, C.c_void_p, f32p, f32p, f32p, f32p, f32p, f32p, f32p, C.c_void_p]),
     "tir_tail_bwd": (C.c_int, [C.c_int64, f32p, C.c_void_p, f32p, f32p, f32p, f32p, f32p, f32p, f32p, f32p, f32p, f32p,
                                f32p, f32p, f32p, C.c_void_p]),
@@ -234,7 +240,7 @@ KERNELS_PER_CALL = {"tir_pack_channels_last": 1, "tir_unpack_channels_last_add":
                     "tir_valid_samples_count": 1, "tir_valid_samples_fill": 1, "tir_composite_fwd": 1,
                     "tir_adam_step": 2, "tir_tv_loss": 1, "tir_tv_loss_bwd": 1, "tir_generate_rays": 1, "tir_hits_prepare": 1, "tir_shade_hits_fwd": 1, "tir_shade_hits_bwd": 1,
                     "tir_primary_march": 6, "tir_primary_app_list": 1, "tir_primary_heads": 5,
-                    "tir_primary_backward": 9,
+                    "tir_primary_backward": 9, "tir_primary_radiance": 2, "tir_primary_radiance_backward": 6,
                     "tir_composite_bwd": 1, "tir_tail_fwd": 1, "tir_tail_bwd": 1, "tir_epilogue_fwd": 1,
                     "tir_epilogue_bwd": 1, "tir_eval_view": 3, "tir_relight_sample": 1, "tir_relight_shade": 1,
                     "tir_marching_cubes_count": 7, "tir_marching_cubes_emit": 2}

@@ -8,6 +8,11 @@
 //   backward  epilogue -> tail (+ derived-normal backward, weight scatter) -> heads dgrad -> heads wgrad -> 2 appearance
 //             scatters -> derived-normal scatter -> compositing (+ softplus') -> density scatter        = 9 launches
 // (round 1: ~25 own + ~500 torch launches for the same work.)
+// The radiance-only forward of training's warm-up phase (is_relight=False) shares the march and the appearance list and
+// replaces the last two calls by tir_primary_radiance / tir_primary_radiance_backward:
+//   forward   ... appearance list -> 1 head -> per-ray weighted sum + radiance epilogue                   =  9 launches
+//   backward  per-ray epilogue + tail -> head dgrad -> head wgrad -> 1 appearance scatter -> compositing ->
+//             density scatter                                                                            =  6 launches
 #include "tir_device.cuh"
 #include "tir_internal.h"
 #include "tir_tail_body.h"
@@ -311,6 +316,67 @@ __global__ void primary_tail_bwd_kernel(TailPtrs p, TailGradPtrs q, int64_t cap,
   }
 }
 
+// ---- radiance-only tail (is_relight=False, tensorBase:930-986) -------------------------------------------------------
+// One thread per ray.  The appearance list is ray-sorted, so rows a_offsets[ray] .. a_offsets[ray+1] are exactly the
+// ray's samples: the weighted sum walks them in list order (no atomics, no memset, same bits on every run) and the
+// radiance epilogue rgb + (1 - acc), depth + (1 - acc) * rays[..., -1] follows in the same thread.  No clamp, no sRGB.
+__global__ void radiance_ray_fwd_kernel(const float* __restrict__ out, const float* __restrict__ a_w,
+                                        const int64_t* __restrict__ a_offsets, int64_t n_rays, int64_t cap,
+                                        const float* __restrict__ acc, const float* __restrict__ depth,
+                                        const float* __restrict__ rays, int32_t bg, float* __restrict__ rgb_map,
+                                        float* __restrict__ depth_map) {
+  const int64_t ray = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (ray >= n_rays) return;
+  const int64_t b = a_offsets[ray] < cap ? a_offsets[ray] : cap;
+  const int64_t e = a_offsets[ray + 1] < cap ? a_offsets[ray + 1] : cap;
+  float s[3] = {0.f, 0.f, 0.f};
+  for (int64_t i = b; i < e; ++i) {
+    const float w = a_w[i];
+    const float4 c = *reinterpret_cast<const float4*>(out + i * 4);
+    s[0] = __fadd_rn(s[0], __fmul_rn(w, c.x));
+    s[1] = __fadd_rn(s[1], __fmul_rn(w, c.y));
+    s[2] = __fadd_rn(s[2], __fmul_rn(w, c.z));
+  }
+  float d = depth[ray];
+  if (bg) {
+    const float t = __fsub_rn(1.f, acc[ray]);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) s[c] = __fadd_rn(s[c], t);
+    d = __fadd_rn(d, __fmul_rn(t, __ldg(rays + ray * 6 + 5)));
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) rgb_map[ray * 3 + c] = s[c];
+  depth_map[ray] = d;
+}
+
+// backward of the above: d acc / d depth of the compositing, d out of the head (row stride 4) and d weight scattered to
+// the valid list (rows that are not appearance samples keep the caller's zero)
+__global__ void radiance_ray_bwd_kernel(const float* __restrict__ out, const float* __restrict__ a_w,
+                                        const int64_t* __restrict__ a_offsets, const int64_t* __restrict__ a_src,
+                                        int64_t n_rays, int64_t cap, const float* __restrict__ rays, int32_t bg,
+                                        const float* __restrict__ g_rgb_map, const float* __restrict__ g_depth_map,
+                                        float* __restrict__ g_out, float* __restrict__ g_weight,
+                                        float* __restrict__ g_acc, float* __restrict__ g_depth) {
+  const int64_t ray = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (ray >= n_rays) return;
+  float g[3] = {0.f, 0.f, 0.f};
+  if (g_rgb_map) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) g[c] = g_rgb_map[ray * 3 + c];
+  }
+  const float gd = g_depth_map ? g_depth_map[ray] : 0.f;
+  g_acc[ray] = bg ? -(g[0] + g[1] + g[2]) - gd * __ldg(rays + ray * 6 + 5) : 0.f;
+  g_depth[ray] = gd;
+  const int64_t b = a_offsets[ray] < cap ? a_offsets[ray] : cap;
+  const int64_t e = a_offsets[ray + 1] < cap ? a_offsets[ray + 1] : cap;
+  for (int64_t i = b; i < e; ++i) {
+    const float w = a_w[i];
+    const float4 c = *reinterpret_cast<const float4*>(out + i * 4);
+    *reinterpret_cast<float4*>(g_out + i * 4) = make_float4(w * g[0], w * g[1], w * g[2], 0.f);
+    g_weight[a_src[i]] = c.x * g[0] + c.y * g[1] + c.z * g[2];
+  }
+}
+
 inline int blocks_for(int64_t n, int threads) {
   int64_t b = (n + threads - 1) / threads;
   const int64_t cap = (int64_t)num_sms() * 8;
@@ -533,6 +599,109 @@ extern "C" int tir_primary_backward(const TirField* field, const TirHeadJob* job
       *field, w->v_feat, w->v_sigma, w->v_dist, w->v_z, w->offsets, n_rays, field->distance_scale, w->cap_valid,
       w->v_weight, w->v_trans, b->g_weight, b->g_acc, g_acc_map, b->g_depth, b->g_feat);
   // 7. density scatter
+  rc = launch_density_bwd(*field, w->v_xn, w->cap_valid, n_valid, b->g_feat, gd, stream);
+  if (rc) return rc;
+  return (int)cudaGetLastError();
+}
+
+// ---- radiance-only primary: TensorBase.forward with is_relight=False -------------------------------------------------
+namespace {
+
+int check_radiance_job(const TirHeadJob* job) {
+  if (!job) return TIR_ERR_NULL;
+  if (job->role != TIR_HEAD_RGB || job->point_set != 0 || job->x_in != 0) return TIR_ERR_CONFIG;
+  if (job->light_mode < 0 || job->light_mode > 2) return TIR_ERR_CONFIG;
+  return TIR_OK;
+}
+
+int radiance_light_mode(const TirHeadJob* job) { return job->mlp.light_line ? job->light_mode : 0; }
+
+}  // namespace
+
+extern "C" int tir_primary_radiance(const TirField* field, const TirHeadJob* job, const float* rays,
+                                    const int32_t* light_idx, int64_t n_rays, const TirPrimaryWork* w, int32_t white_bg,
+                                    float* rgb_map, float* depth_map, void* stream_) {
+  if (n_rays <= 0) return TIR_OK;
+  if (!field || !rays || !w || !rgb_map || !depth_map) return TIR_ERR_NULL;
+  int rc = check_radiance_job(job);
+  if (rc) return rc;
+  if (!w->a_offsets || !w->a_ray || !w->a_w || !w->a_xn || !w->acc || !w->depth || !w->out[0]) return TIR_ERR_NULL;
+  const int mode = radiance_light_mode(job);
+  if (mode == 1 && !light_idx) return TIR_ERR_NULL;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const int64_t cap = w->cap_app;
+  const int64_t* n_app = w->a_offsets + n_rays;
+  HeadJobDev d{};
+  d.mlp = job->mlp;
+  d.xn = w->a_xn;
+  d.x_in = rays + 3; d.x_in_stride = 6; d.x_index = w->a_ray;
+  d.light_mode = mode;
+  d.light_idx = mode == 1 ? light_idx : nullptr;
+  d.act = job->act;
+  d.out = w->out[0]; d.out_stride = 4;
+  d.save_x0 = w->x0[0]; d.save_in = w->inp[0]; d.save_h1 = w->h1[0]; d.save_h2 = w->h2[0];
+  rc = launch_heads_forward(*field, &d, 1, cap, n_app, stream);
+  if (rc) return rc;
+  radiance_ray_fwd_kernel<<<(unsigned)((n_rays + 127) / 128), 128, 0, stream>>>(
+      w->out[0], w->a_w, w->a_offsets, n_rays, cap, w->acc, w->depth, rays, white_bg, rgb_map, depth_map);
+  return (int)cudaGetLastError();
+}
+
+extern "C" int tir_primary_radiance_backward(const TirField* field, const TirHeadJob* job, const float* rays,
+                                             const int32_t* light_idx, int64_t n_rays, const TirPrimaryWork* w,
+                                             const TirPrimaryBwdWork* b, int32_t white_bg, const float* g_rgb_map,
+                                             const float* g_depth_map, const float* g_acc_map,
+                                             const TirPrimaryGrads* gr, void* stream_) {
+  if (n_rays <= 0) return TIR_OK;
+  if (!field || !rays || !w || !b || !gr) return TIR_ERR_NULL;
+  int rc = check_radiance_job(job);
+  if (rc) return rc;
+  if (!b->g_acc || !b->g_depth || !b->g_weight || !b->g_feat || !b->g_out[0] || !b->gz1[0] || !b->gz2[0] ||
+      !b->gfeat[0] || !b->gx0[0])
+    return TIR_ERR_NULL;
+  if (!w->x0[0] || !w->inp[0] || !w->h1[0] || !w->h2[0] || !w->out[0] || !w->a_src || !w->a_w || !w->a_xn)
+    return TIR_ERR_NULL;
+  const int mode = radiance_light_mode(job);
+  if (mode == 1 && !light_idx) return TIR_ERR_NULL;
+  GradPtrs ga{}, gd{};
+  for (int k = 0; k < 3; ++k) {
+    ga.plane[k] = gr->aplane[k]; ga.line[k] = gr->aline[k];
+    gd.plane[k] = gr->dplane[k]; gd.line[k] = gr->dline[k];
+    if (!ga.plane[k] || !ga.line[k] || !gd.plane[k] || !gd.line[k]) return TIR_ERR_NULL;
+  }
+  cudaStream_t stream = (cudaStream_t)stream_;
+  const int64_t cap = w->cap_app;
+  const int64_t* n_app = w->a_offsets + n_rays;
+  const int64_t* n_valid = w->offsets + n_rays;
+
+  // 1. epilogue + per-sample tail: d out of the head, d weight onto the valid list, d acc / d depth per ray
+  cudaError_t e = cudaMemsetAsync(b->g_weight, 0, (size_t)w->cap_valid * sizeof(float), stream);
+  if (e != cudaSuccess) return (int)e;
+  radiance_ray_bwd_kernel<<<(unsigned)((n_rays + 127) / 128), 128, 0, stream>>>(
+      w->out[0], w->a_w, w->a_offsets, w->a_src, n_rays, cap, rays, white_bg, g_rgb_map, g_depth_map, b->g_out[0],
+      b->g_weight, b->g_acc, b->g_depth);
+  // 2. head: data gradient + weight gradients
+  HeadBwdJob h{};
+  h.mlp = job->mlp;
+  h.light_mode = mode;
+  h.x_index = mode == 1 ? w->a_ray : nullptr;
+  h.light_idx = mode == 1 ? light_idx : nullptr;
+  h.act = job->act; h.point_set = 0;
+  h.out = w->out[0]; h.out_stride = 4; h.g_out = b->g_out[0];
+  h.inp = w->inp[0]; h.h1 = w->h1[0]; h.h2 = w->h2[0];
+  h.gz1 = b->gz1[0]; h.gz2 = b->gz2[0]; h.gfeat = b->gfeat[0]; h.gx0 = b->gx0[0];
+  h.g_w0 = gr->w0[0]; h.g_b0 = gr->b0[0]; h.g_w1 = gr->w1[0]; h.g_b1 = gr->b1[0]; h.g_w2 = gr->w2[0]; h.g_b2 = gr->b2[0];
+  HeadsBwdShared sh{};
+  sh.x0[0] = w->x0[0]; sh.x0[1] = nullptr; sh.g_basis = gr->basis; sh.g_light = gr->light_line;
+  rc = launch_heads_backward(*field, &h, 1, sh, cap, n_app, stream);
+  if (rc) return rc;
+  // 3. appearance scatter (point set 0 only)
+  rc = launch_app_products_bwd(*field, w->a_xn, cap, n_app, b->gx0[0], nullptr, nullptr, ga, stream);
+  if (rc) return rc;
+  // 4. compositing (+ feature2density) with the acc / depth gradients, 5. density scatter
+  primary_composite_bwd_kernel<<<(unsigned)((n_rays * 32 + 255) / 256), 256, 0, stream>>>(
+      *field, w->v_feat, w->v_sigma, w->v_dist, w->v_z, w->offsets, n_rays, field->distance_scale, w->cap_valid,
+      w->v_weight, w->v_trans, b->g_weight, b->g_acc, g_acc_map, b->g_depth, b->g_feat);
   rc = launch_density_bwd(*field, w->v_xn, w->cap_valid, n_valid, b->g_feat, gd, stream);
   if (rc) return rc;
   return (int)cudaGetLastError();

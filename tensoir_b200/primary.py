@@ -87,12 +87,14 @@ def march(model, rays, is_train, n_samples, counters=None):
 
 
 def forward_relight(model, rays_chunk, light_idx, white_bg=True, is_train=False, is_relight=True, N_samples=-1):
-    if is_relight:
-        from . import primary_fused
-        if primary_fused.supported(model):
-            # the whole primary march as one autograd node over the fused C entry points (csrc/tir_primary.cu);
-            # the modular path below (model.__dict__['_tir_modular'] = True) is kept as its cross-check
+    from . import primary_fused
+    if primary_fused.supported(model):
+        # the whole primary march as one autograd node over the fused C entry points (csrc/tir_primary.cu), with all
+        # the heads (is_relight=True) or the radiance head only (is_relight=False, training's warm-up phase); the
+        # modular path below (model.__dict__['_tir_modular'] = True) is kept as its cross-check
+        if is_relight:
             return primary_fused.forward_relight(model, rays_chunk, light_idx, white_bg, is_train, N_samples)
+        return primary_fused.forward_radiance(model, rays_chunk, light_idx, white_bg, is_train, N_samples)
     dev = rays_chunk.device
     rays = rays_chunk.float()
     n_rays = rays.shape[0]

@@ -30,8 +30,9 @@ class Workspace:
     """Scratch of one primary march: per-ray arrays, the valid list, the appearance list and (training) the
     activation dumps + backward scratch.  Re-used across calls; grown, never shrunk."""
 
-    def __init__(self, device):
+    def __init__(self, device, point_sets=2):
         self.dev = device
+        self.point_sets = point_sets      # 1: no jittered point set (radiance-only forward), so no second x0 dump
         self.n_rays = self.cap_valid = self.cap_app = 0
         self.n_jobs = 0
         self.grad = False
@@ -63,7 +64,9 @@ class Workspace:
         for j in range(n_jobs):
             a(f"out{j}", (cap_app, 4))
         if grad:
-            a("x0_0", (cap_app, 144)); a("x0_1", (cap_app, 144))
+            a("x0_0", (cap_app, 144))
+            if self.point_sets > 1:
+                a("x0_1", (cap_app, 144))
             a("g_packed", (n_rays, 14)); a("g_acc", n_rays); a("g_depth", n_rays)
             a("g_weight", cap_valid); a("g_feat", cap_valid)
             a("g_dn_feat", cap_app); a("g_dn_dfdx", (cap_app, 3))
@@ -88,7 +91,8 @@ class Workspace:
             if grad:
                 w.inp[j], w.h1[j], w.h2[j] = t[f"inp{j}"].data_ptr(), t[f"h1_{j}"].data_ptr(), t[f"h2_{j}"].data_ptr()
         if grad:
-            w.x0[0], w.x0[1] = t["x0_0"].data_ptr(), t["x0_1"].data_ptr()
+            w.x0[0] = t["x0_0"].data_ptr()
+            w.x0[1] = t["x0_1"].data_ptr() if "x0_1" in t else None
         return w
 
     def bwd_struct(self, n_jobs):
@@ -125,6 +129,92 @@ def _cl_zeros(p):
     return buf, buf.permute(2, 0, 1).unsqueeze(0)
 
 
+def _workspace(model, key, dev, need, point_sets=2):
+    """The cached workspace of ``model.__dict__[key]``, marked busy until the backward when ``need``."""
+    ws = model.__dict__.get(key)
+    if ws is None or ws.dev != dev:
+        ws = Workspace(dev, point_sets)
+        model.__dict__[key] = ws
+    if ws.busy and model.__dict__.get("_tir_static") is None:
+        # a previous training forward still waits for its backward (several chunks per step): its dumps live in the
+        # cached workspace, so this call gets a private one
+        ws = Workspace(dev, point_sets)
+    ws.busy = need
+    return ws
+
+
+def _march(lib, f, rays, cfg, ws, n_jobs, need, counters, st):
+    """tir_primary_march + tir_primary_app_list -> (work struct, appearance rows; None in shape-static mode)."""
+    n_rays = rays.shape[0]
+    cptr = None if counters is None else _lib.dptr(counters, torch.int64)
+    if st is not None:
+        ws.ensure(n_rays, st["cap_valid"], st["cap_app"], n_jobs, need)
+    else:
+        ws.ensure(n_rays, max(ws.cap_valid, 96 * n_rays + 1024), max(ws.cap_app, 8 * n_rays + 1024), n_jobs, need)
+    stream = _lib.stream_ptr()
+    snap = counters.clone() if (counters is not None and st is None) else None
+    n_app = None
+    while True:
+        w = ws.work_struct(None, n_jobs, need)
+        _lib.check(lib.tir_primary_march(C.byref(f), _lib.dptr(rays), n_rays, C.byref(cfg), C.byref(w), cptr, stream),
+                   "tir_primary_march")
+        if st is not None:
+            # shape-static mode: the kernels already left the real list lengths and the overflow flag on the device
+            st["stats"][0:2].copy_(ws.t["status"][0:2])
+            st["overflow_step"].add_(ws.t["status"][2])
+            break
+        n_valid, n_app, _, _ = ws.t["status"].tolist()          # the one host read of the eager forward
+        if n_valid <= ws.cap_valid and n_app <= ws.cap_app:
+            break
+        if counters is not None:      # the march runs again: do not count its rays twice
+            counters.copy_(snap)
+        ws.ensure(n_rays, int(1.25 * n_valid) + 1024, int(1.25 * n_app) + 1024, n_jobs, need)
+    if counters is not None:
+        counters[_lib.CNT_APP] += ws.t["status"][1]
+    _lib.check(lib.tir_primary_app_list(C.byref(f), n_rays, C.byref(w), stream), "tir_primary_app_list")
+    return w, n_app
+
+
+def _vm_grad_buffers(model):
+    """Gradient buffers of the VM factors (17-31 M floats), in the order density planes, density lines, app planes, app
+    lines -> (buffers the kernels accumulate into, what autograd gets for each factor).  When a parameter already HAS
+    a dense channel-last .grad (kept zeroed in place by tensoir_b200.optim.FusedAdam, or the views of a dp.GradBucket)
+    the kernels accumulate straight into it and autograd gets None for that input: no 70 MB allocation + memset +
+    AccumulateGrad pass per step.  Otherwise a zeroed buffer in the kernels' layout is returned the usual way."""
+    vm = list(model.density_plane) + list(model.density_line) + list(model.app_plane) + list(model.app_line)
+    bufs, views = [], []
+    for p in vm:
+        g = p.grad
+        if (g is not None and g.dtype == torch.float32 and g.shape == p.shape and p.shape[0] == 1
+                and all(a == b for a, b, n in zip(g.stride(), p.stride(), p.shape) if n > 1)
+                and p.is_contiguous(memory_format=torch.channels_last)
+                and model.__dict__.get("_tir_grad_inplace", True)):
+            bufs.append(g)
+            views.append(None)
+        else:
+            b_, v_ = _cl_zeros(p)
+            bufs.append(b_)
+            views.append(v_)
+    return bufs, views
+
+
+def _set_vm_grads(gr, bufs):
+    for k in range(3):
+        gr.dplane[k], gr.dline[k] = bufs[k].data_ptr(), bufs[3 + k].data_ptr()
+        gr.aplane[k], gr.aline[k] = bufs[6 + k].data_ptr(), bufs[9 + k].data_ptr()
+
+
+def _grad_target(p, inplace):
+    """(buffer the kernels accumulate into, what autograd gets): the parameter's own .grad when it is a plain fp32
+    tensor of the same layout (then autograd gets None: no zero-fill, no AccumulateGrad add), else zeros."""
+    g = p.grad
+    if inplace and g is not None and g.dtype == torch.float32 and g.shape == p.shape and g.is_contiguous() \
+            and p.is_contiguous():
+        return g, None
+    z = torch.zeros_like(p)
+    return z, z
+
+
 class _PrimaryRelight(torch.autograd.Function):
     @staticmethod
     def forward(ctx, model, rays, light_idx, white_bg, is_train, n_samples, bg_flag, jitter, *params):
@@ -141,40 +231,10 @@ class _PrimaryRelight(torch.autograd.Function):
         cfg = ops.march_cfg(model, n_samples=n_samples, jitter=jitter, keep=keep)
         counters = model.__dict__.get("_tir_counters")
         cptr = None if counters is None else _lib.dptr(counters, torch.int64)
-        ws = model.__dict__.get("_tir_primary_ws")
-        if ws is None or ws.dev != dev:
-            ws = Workspace(dev)
-            model.__dict__["_tir_primary_ws"] = ws
-        if ws.busy and st is None:
-            # a previous training forward still waits for its backward (several chunks per step): its dumps live in the
-            # cached workspace, so this call gets a private one
-            ws = Workspace(dev)
-        ws.busy = need
-        if st is not None:
-            ws.ensure(n_rays, st["cap_valid"], st["cap_app"], n_jobs, need)
-        else:
-            ws.ensure(n_rays, max(ws.cap_valid, 96 * n_rays + 1024), max(ws.cap_app, 8 * n_rays + 1024), n_jobs, need)
+        ws = _workspace(model, "_tir_primary_ws", dev, need)
         li = light_idx.reshape(-1).to(torch.int32).contiguous()
         stream = _lib.stream_ptr()
-        snap = counters.clone() if (counters is not None and st is None) else None
-        while True:
-            w = ws.work_struct(None, n_jobs, need)
-            _lib.check(cd.tir_primary_march(C.byref(f), _lib.dptr(rays), n_rays, C.byref(cfg), C.byref(w), cptr, stream),
-                       "tir_primary_march")
-            if st is not None:
-                # shape-static mode: the kernels already left the real list lengths and the overflow flag on the device
-                st["stats"][0:2].copy_(ws.t["status"][0:2])
-                st["overflow_step"].add_(ws.t["status"][2])
-                break
-            n_valid, n_app, _, _ = ws.t["status"].tolist()          # the one host read of the eager forward
-            if n_valid <= ws.cap_valid and n_app <= ws.cap_app:
-                break
-            if counters is not None:      # the march runs again: do not count its rays twice
-                counters.copy_(snap)
-            ws.ensure(n_rays, int(1.25 * n_valid) + 1024, int(1.25 * n_app) + 1024, n_jobs, need)
-        if counters is not None:
-            counters[_lib.CNT_APP] += ws.t["status"][1]
-        _lib.check(cd.tir_primary_app_list(C.byref(f), n_rays, C.byref(w), stream), "tir_primary_app_list")
+        w, n_app = _march(cd, f, rays, cfg, ws, n_jobs, need, counters, st)
         # xyz noise of the smoothness term: randn_like(xyz_sampled[app_mask]) (tensorBase:937), drawn on the device in
         # list order; the eager path draws exactly n_app rows like the reference
         draw = model.__dict__.get("_tir_randn_like")       # test hook: replay the oracle's stream / deterministic noise
@@ -228,38 +288,12 @@ class _PrimaryRelight(torch.autograd.Function):
         w = ws.work_struct(noise, n_jobs, True)
         b = ws.bwd_struct(n_jobs)
         gr = TirPrimaryGrads()
-        vm = list(model.density_plane) + list(model.density_line) + list(model.app_plane) + list(model.app_line)
-        # Gradient buffers of the VM factors (17-31 M floats).  When a parameter already HAS a dense channel-last .grad
-        # (kept zeroed in place by tensoir_b200.optim.FusedAdam, or the views of a dp.GradBucket) the kernels accumulate
-        # straight into it and autograd gets None for that input: no 70 MB allocation + memset + AccumulateGrad pass per
-        # step.  Otherwise a zeroed buffer in the kernels' layout is returned the usual way.
-        bufs, views = [], []
-        for p in vm:
-            g = p.grad
-            if (g is not None and g.dtype == torch.float32 and g.shape == p.shape and p.shape[0] == 1
-                    and all(a == b for a, b, n in zip(g.stride(), p.stride(), p.shape) if n > 1)
-                    and p.is_contiguous(memory_format=torch.channels_last)
-                    and model.__dict__.get("_tir_grad_inplace", True)):
-                bufs.append(g)
-                views.append(None)
-            else:
-                b_, v_ = _cl_zeros(p)
-                bufs.append(b_)
-                views.append(v_)
-        for k in range(3):
-            gr.dplane[k], gr.dline[k] = bufs[k].data_ptr(), bufs[3 + k].data_ptr()
-            gr.aplane[k], gr.aline[k] = bufs[6 + k].data_ptr(), bufs[9 + k].data_ptr()
+        bufs, views = _vm_grad_buffers(model)
+        _set_vm_grads(gr, bufs)
         inplace = model.__dict__.get("_tir_grad_inplace", True)
 
         def target(p):
-            """(buffer the kernels accumulate into, what autograd gets): the parameter's own .grad when it is a plain
-            fp32 tensor of the same layout (then autograd gets None: no zero-fill, no AccumulateGrad add), else zeros."""
-            g = p.grad
-            if inplace and g is not None and g.dtype == torch.float32 and g.shape == p.shape and g.is_contiguous() \
-                    and p.is_contiguous():
-                return g, None
-            z = torch.zeros_like(p)
-            return z, z
+            return _grad_target(p, inplace)
         g_basis, r_basis = target(model.basis_mat.weight)
         gr.basis = g_basis.data_ptr()
         ll = getattr(model, "light_line", None)
@@ -305,19 +339,120 @@ def forward_relight(model, rays_chunk, light_idx, white_bg=True, is_train=False,
         nan = torch.full((), float("nan"), device=dev)
         return (z3, z, z3.clone(), z3.clone(), z1, z3.clone(), z.clone(), z1.clone(), z1.clone(), z > 0.5, nan,
                 nan.clone())
-    # host-side draws in the reference's order: per-ray jitter on the CPU (tensorBase:714-718), then the background
-    # coin, which white_bg short-circuits (tensorBase:979 / :1004)
+    jitter, bg = _host_draws(model, n_rays, dev, white_bg, is_train)
+    params = _params(model, ("renderModule", "renderModule_brdf", "renderModule_normal"))
+    return _PrimaryRelight.apply(model, rays, light_idx, white_bg, is_train, N_samples, bg, jitter, *params)
+
+
+def _host_draws(model, n_rays, dev, white_bg, is_train):
+    """Host-side draws in the reference's order: per-ray jitter on the CPU (tensorBase:714-718), then the background
+    coin, which white_bg short-circuits (tensorBase:979 / :1004) -> (jitter or None, background flag)."""
     jitter = None
     if is_train:
         st = model.__dict__.get("_tir_static")
         jitter = st["jitter"] if st is not None else torch.rand(n_rays, 1).to(dev)
-    bg = white_bg or (is_train and bool(torch.rand((1,)) < 0.5))
+    return jitter, white_bg or (is_train and bool(torch.rand((1,)) < 0.5))
+
+
+def _params(model, heads):
+    """Autograd inputs of a primary node: VM factors, basis, [light_line], 6 tensors per head."""
     params = list(model.density_plane) + list(model.density_line) + list(model.app_plane) + list(model.app_line)
     params.append(model.basis_mat.weight)
     ll = getattr(model, "light_line", None)
     if ll is not None:
         params.append(ll.weight)
-    for head in ("renderModule", "renderModule_brdf", "renderModule_normal"):
+    for head in heads:
         m = getattr(model, head).mlp
         params += [m[0].weight, m[0].bias, m[2].weight, m[2].bias, m[4].weight, m[4].bias]
-    return _PrimaryRelight.apply(model, rays, light_idx, white_bg, is_train, N_samples, bg, jitter, *params)
+    return params
+
+
+# ---- radiance-only primary (is_relight=False): training's warm-up phase -------------------------------------------------
+def _radiance_job(model, keep):
+    """The one head of the radiance branch: renderModule on the view direction, light_line[light_idx] if the model has
+    one (tensorBase:930-946, is_relight=False)."""
+    has_light = getattr(model, "light_line", None) is not None
+    job = TirHeadJob()
+    job.mlp = mlp_struct(model, "renderModule", keep, light="index" if has_light else "none")
+    job.point_set, job.x_in, job.light_mode, job.act, job.role = 0, 0, 1 if has_light else 0, 0, HEAD_RGB
+    return job
+
+
+class _PrimaryRadiance(torch.autograd.Function):
+    """TensorBase.forward with is_relight=False around tir_primary_march / _app_list / _radiance (9 launches) and
+    tir_primary_radiance_backward (6 launches) -> (rgb_map, depth_map, acc_map)."""
+
+    @staticmethod
+    def forward(ctx, model, rays, light_idx, is_train, n_samples, bg_flag, jitter, *params):
+        lib = _lib.load()
+        dev = rays.device
+        need = any(ctx.needs_input_grad)
+        n_rays = rays.shape[0]
+        f = ops.device_field(model).refresh(model, force=bool(is_train))
+        keep = []
+        job = _radiance_job(model, keep)
+        cfg = ops.march_cfg(model, n_samples=n_samples, jitter=jitter, keep=keep)
+        ws = _workspace(model, "_tir_radiance_ws", dev, need, point_sets=1)
+        w, _ = _march(lib, f, rays, cfg, ws, 1, need, model.__dict__.get("_tir_counters"),
+                      model.__dict__.get("_tir_static"))
+        li = light_idx.reshape(-1).to(torch.int32).contiguous()
+        rgb, depth = torch.empty(n_rays, 3, device=dev), torch.empty(n_rays, device=dev)
+        _lib.check(lib.tir_primary_radiance(C.byref(f), C.byref(job), _lib.dptr(rays), _lib.dptr(li, torch.int32),
+                                            n_rays, C.byref(w), int(bool(bg_flag)), _lib.dptr(rgb), _lib.dptr(depth),
+                                            _lib.stream_ptr()), "tir_primary_radiance")
+        acc = ws.t["acc"].clone()
+        ctx.model = model
+        ctx.keep = (keep, job, li, rays, ws, jitter, int(bool(bg_flag)))
+        return rgb, depth, acc
+
+    @staticmethod
+    def backward(ctx, g_rgb, g_depth, g_acc):
+        model = ctx.model
+        keep, job, li, rays, ws, jitter, bg = ctx.keep
+        lib = _lib.load()
+        f = ops.device_field(model).refresh(model)
+
+        def c(t):
+            return None if t is None else t.contiguous().float()
+        g_rgb, g_depth, g_acc = c(g_rgb), c(g_depth), c(g_acc)
+        w = ws.work_struct(None, 1, True)
+        b = ws.bwd_struct(1)
+        gr = TirPrimaryGrads()
+        bufs, views = _vm_grad_buffers(model)
+        _set_vm_grads(gr, bufs)
+        inplace = model.__dict__.get("_tir_grad_inplace", True)
+        g_basis, r_basis = _grad_target(model.basis_mat.weight, inplace)
+        gr.basis = g_basis.data_ptr()
+        ll = getattr(model, "light_line", None)
+        g_light, r_light = _grad_target(ll.weight, inplace) if ll is not None else (None, None)
+        gr.light_line = None if g_light is None else g_light.data_ptr()
+        m = model.renderModule.mlp
+        mg = [_grad_target(t, inplace) for t in (m[0].weight, m[0].bias, m[2].weight, m[2].bias, m[4].weight,
+                                                  m[4].bias)]
+        gr.w0[0], gr.b0[0], gr.w1[0], gr.b1[0], gr.w2[0], gr.b2[0] = [t[0].data_ptr() for t in mg]
+
+        def ptr(t):
+            return None if t is None else _lib.dptr(t)
+        _lib.check(lib.tir_primary_radiance_backward(C.byref(f), C.byref(job), _lib.dptr(rays),
+                                                     _lib.dptr(li, torch.int32), rays.shape[0], C.byref(w), C.byref(b),
+                                                     bg, ptr(g_rgb), ptr(g_depth), ptr(g_acc), C.byref(gr),
+                                                     _lib.stream_ptr()), "tir_primary_radiance_backward")
+        ws.busy = False
+        # gradients in the order of `params` (see forward_radiance): VM factors, basis, [light_line], renderModule
+        out = list(views) + [r_basis] + ([r_light] if ll is not None else []) + [t[1] for t in mg]
+        return (None,) * 7 + tuple(out)
+
+
+def forward_radiance(model, rays_chunk, light_idx, white_bg=True, is_train=False, N_samples=-1):
+    """-> the 12-tuple of TensorBase.forward (is_relight=False): rgb_map, depth_map, acc_map, the rest None."""
+    rays = rays_chunk.float().contiguous()
+    n_rays = rays.shape[0]
+    dev = rays.device
+    if n_rays == 0:
+        z = torch.zeros(0, device=dev)
+        rgb, depth, acc = torch.zeros(0, 3, device=dev), z, z.clone()
+    else:
+        jitter, bg = _host_draws(model, n_rays, dev, white_bg, is_train)
+        params = _params(model, ("renderModule",))
+        rgb, depth, acc = _PrimaryRadiance.apply(model, rays, light_idx, is_train, N_samples, bg, jitter, *params)
+    return rgb, depth, None, None, None, None, acc, None, None, None, None, None

@@ -47,8 +47,12 @@ class StaticTrainStep:
     LISTS = ("cap_valid", "cap_app")      # surface hits are not a list any more (relight_utils.render_hits)
 
     def __init__(self, model, optimizer, n_rays, n_samples, args, loss_fn, *, sample_method="stratified_sampling",
-                 cap_valid=None, cap_app=None, grad_bucket=None, device=None, grow_at=0.8, headroom=1.5, lag=2):
+                 cap_valid=None, cap_app=None, grad_bucket=None, device=None, grow_at=0.8, headroom=1.5, lag=2,
+                 is_relight=True):
         self.model, self.opt, self.args, self.loss_fn = model, optimizer, args, loss_fn
+        # False: the radiance-only step of training's warm-up phase (train_tensoIR.py trains with is_relight=False until
+        # update_AlphaMask_list[0]), which draws no light directions
+        self.is_relight = bool(is_relight)
         self.n_rays, self.n_samples, self.sample_method = int(n_rays), int(n_samples), sample_method
         self.bucket = grad_bucket
         dev = device or model.device
@@ -99,9 +103,13 @@ class StaticTrainStep:
         self._set_caps(int(headroom * nv) + 4096, int(headroom * na) + 1024)
         return self.capacities()
 
+    def _clamp_caps(self, cap_valid, cap_app):
+        """No list can be longer than n_rays * n_samples valid samples, the appearance list than the valid list."""
+        cap_valid = int(min(cap_valid, self.n_rays * max(self.n_samples, 1)))
+        return cap_valid, int(min(cap_app, cap_valid))
+
     def _set_caps(self, cap_valid, cap_app, *_unused):
-        self.static["cap_valid"] = int(min(cap_valid, self.n_rays * max(self.n_samples, 1)))
-        self.static["cap_app"] = int(min(cap_app, self.static["cap_valid"]))
+        self.static["cap_valid"], self.static["cap_app"] = self._clamp_caps(cap_valid, cap_app)
 
     def capacities(self):
         return tuple(self.static[k] for k in self.LISTS)
@@ -109,15 +117,17 @@ class StaticTrainStep:
     # -- host side of one step: the reference's CPU draws, in the reference's order, into the static buffers
     def _stage_host_randoms(self, slot):
         slot["jitter"].copy_(torch.rand(self.n_rays, 1))                                    # tensorBase:714-718
-        slot["dirs"].copy_(self.model.gen_light_incident_dirs(method=self.sample_method))   # tensorBase:511-526
         self.static["jitter"].copy_(slot["jitter"], non_blocking=True)
-        self.static["dirs"].copy_(slot["dirs"], non_blocking=True)
+        if self.is_relight:
+            slot["dirs"].copy_(self.model.gen_light_incident_dirs(method=self.sample_method))   # tensorBase:511-526
+            self.static["dirs"].copy_(slot["dirs"], non_blocking=True)
 
     def _body(self):
         st = self.static
         st["overflow_step"].zero_()
         ret = Renderer_TensoIR_train(self.rays, None, self.light_idx, self.model, N_samples=self.n_samples,
-                                     white_bg=True, is_train=True, is_relight=True, sample_method=self.sample_method,
+                                     white_bg=True, is_train=True, is_relight=self.is_relight,
+                                     sample_method=self.sample_method,
                                      chunk_size=160000, device=self.dev, args=self.args)
         loss = self.loss_fn(ret, self.model)
         self.ret = ret                    # the captured forward's outputs: after a replay they hold that step's values
@@ -210,6 +220,9 @@ class StaticTrainStep:
         for i in range(2):
             if seen[i] > self.grow_at * caps[i]:
                 want[i] = int(self.headroom * seen[i]) + 64
+        # a list already at its largest possible length cannot grow (without an alpha mask nearly every in-box sample is
+        # valid, and the valid list of the warm-up phase runs close to n_rays * n_samples): no re-capture for that
+        want = list(self._clamp_caps(*want))
         slots = self.n_rays * self.static["dirs"].shape[0]
         sec_cap = max(1 << 16, self.static["sec_per_slot"] * slots)
         if n_sec > self.grow_at * sec_cap:          # secondary appearance scratch: rows per (ray, direction) slot
