@@ -197,6 +197,47 @@ int tir_secondary_march(const TirField* field, const float* surf_xyz, const floa
                         TirAppSample* samples, uint32_t* sample_count, int64_t capacity,
                         uint64_t* counters, void* stream);
 
+/* The density feature of compute_densityfeature (models/tensoRF_rotated_lights.py:95-110) sampled at the density-grid
+ * vertices of a sub-box [lo, lo+n) of the grid, stored [z][y][x] with x fastest (n[0]*n[1]*n[2] floats):
+ *   D[x,y,z] = sum_k sum_c plane_k[c](x_{m0}, x_{m1}) * line_k[c](x_v)
+ * For every orientation k, bilinear(plane) * linear(line) uses separable weights, so the feature at any point is the
+ * trilinear interpolation of D with the same taps and the same zero padding.  The secondary march reads 8 floats of D
+ * per sample instead of 6 taps x 3 orientations x C channels of the factors.  D is a function of the live density
+ * factors: rebuild it (tir_density_volume_build) before every march that reads it, never keep it across a parameter
+ * update. */
+typedef struct TirDensityVolume {
+  float* data;
+  int32_t lo[3];           /* first density-grid vertex x,y,z of the box */
+  int32_t n[3];            /* vertices along x,y,z; 0 along any axis = empty box */
+} TirDensityVolume;
+
+/* Host-only (no device access, no stream).  The box every valid sample of the secondary march reads: the density-grid
+ * vertices whose trilinear taps a point inside the occupied-cell box field->occ_lo/occ_hi can touch (computed with the
+ * kernels' own coordinate arithmetic), grown by one vertex on each side against rounding and clamped to the grid.  The
+ * whole grid when the field has no alpha mask or no box (occ_lo > occ_hi); an empty box (some n == 0) when the
+ * occupied-cell box does not meet the grid.  TIR_ERR_SHAPE when a grid size is < 1. */
+int tir_density_volume_extent(const TirField* field, int32_t lo[3], int32_t n[3]);
+
+/* Fills vol->data over the box vol->lo / vol->n from the density factors of `field` (plane and line rows are read once
+ * per tile of vertices; per vertex the channels of an orientation are summed in channel order, then the three
+ * orientations in order 0,1,2, as the factor path sums them).  TIR_ERR_CAPACITY when capacity (floats) is smaller than
+ * n[0]*n[1]*n[2]; TIR_ERR_SHAPE when the box leaves the grid or dC != 16. */
+int tir_density_volume_build(const TirField* field, TirDensityVolume* vol, int64_t capacity, void* stream);
+
+/* tir_secondary_march / tir_secondary_radiance with the density of every sample read from `vol` (built from the same
+ * field by tir_density_volume_build over the box tir_density_volume_extent gives): 8 trilinear corner reads instead of
+ * the 18-tap factor gather.  Same samples, masks, counters and outputs as the factor path up to the rounding of the
+ * density feature.  The factor-path entry points above stay the reference. */
+int tir_secondary_radiance_vol(const TirField* field, const TirMlp* mlp, const float* surf_xyz, const float* normals,
+                               const int32_t* light_idx, int64_t n_pts, const float* dirs, int32_t n_dirs,
+                               const TirMarchCfg* cfg, const TirDensityVolume* vol, float* vis, float* indirect,
+                               TirAppSample* samples, uint32_t* sample_count, int64_t capacity,
+                               uint64_t* counters, void* stream);
+int tir_secondary_march_vol(const TirField* field, const float* surf_xyz, const float* normals, int64_t n_pts,
+                            const float* dirs, int32_t n_dirs, const TirMarchCfg* cfg, const TirDensityVolume* vol,
+                            float* vis, TirAppSample* samples, uint32_t* sample_count, int64_t capacity,
+                            uint64_t* counters, void* stream);
+
 /* Appearance gather + basis_mat + MLPRender_Fea on a compacted sample list
  * (compute_appfeature tensoRF_rotated_lights.py:197-224 + MLPRender_Fea tensorBase:136-146):
  *   rgb_out[ray] += weight * sigmoid(mlp(...)) for every sample; dirs_of_ray gives the view dir.

@@ -49,6 +49,10 @@ class TirMarchCfg(C.Structure):
     ]
 
 
+class TirDensityVolume(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("lo", C.c_int32 * 3), ("n", C.c_int32 * 3)]
+
+
 MARCH_NO_BBOX = 1
 MARCH_LEAN_COUNTERS = 2
 MARCH_CELL_BRICKS = 4
@@ -141,6 +145,15 @@ EXPORTS = {
     "tir_secondary_march": (C.c_int, [C.POINTER(TirField), f32p, f32p, C.c_int64, f32p, C.c_int32,
                                       C.POINTER(TirMarchCfg), f32p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
                                       C.c_void_p]),
+    "tir_density_volume_extent": (C.c_int, [C.POINTER(TirField), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "tir_density_volume_build": (C.c_int, [C.POINTER(TirField), C.POINTER(TirDensityVolume), C.c_int64, C.c_void_p]),
+    "tir_secondary_radiance_vol": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), f32p, f32p, C.c_void_p,
+                                             C.c_int64, f32p, C.c_int32, C.POINTER(TirMarchCfg),
+                                             C.POINTER(TirDensityVolume), f32p, f32p, C.c_void_p, C.c_void_p,
+                                             C.c_int64, C.c_void_p, C.c_void_p]),
+    "tir_secondary_march_vol": (C.c_int, [C.POINTER(TirField), f32p, f32p, C.c_int64, f32p, C.c_int32,
+                                          C.POINTER(TirMarchCfg), C.POINTER(TirDensityVolume), f32p, C.c_void_p,
+                                          C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "tir_app_mlp": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), C.c_void_p, C.c_void_p, C.c_int64, f32p,
                               C.c_int32, C.c_void_p, f32p, C.c_void_p]),
     "tir_app_mlp_wgmma": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), C.c_void_p, C.c_void_p, C.c_int64, f32p,
@@ -233,7 +246,8 @@ EXPORTS = {
 # kernels launched per entry point (for bench.py's gpu_launches claim)
 KERNELS_PER_CALL = {"tir_pack_channels_last": 1, "tir_unpack_channels_last_add": 1, "tir_pack_alpha_mask": 3,
                     "tir_density_points": 1, "tir_alpha_mask_points": 1, "tir_march_density": 1,
-                    "tir_march_radiance": 2, "tir_secondary_march": 1, "tir_secondary_radiance": 2, "tir_app_mlp": 1, "tir_app_mlp_wgmma": 1, "tir_app_mlp_legacy": 1, "tir_app_mlp_points_wgmma": 1,
+                    "tir_march_radiance": 2, "tir_secondary_march": 1, "tir_secondary_radiance": 2,
+                    "tir_density_volume_build": 1, "tir_secondary_march_vol": 1, "tir_secondary_radiance_vol": 2, "tir_app_mlp": 1, "tir_app_mlp_wgmma": 1, "tir_app_mlp_legacy": 1, "tir_app_mlp_points_wgmma": 1,
                     "tir_app_mlp_points_legacy": 1,
                     "tir_shade_fwd": 1, "tir_shade_bwd": 1, "tir_app_mlp_points": 1, "tir_app_mlp_points_save": 1, "tir_vm_app_products": 1, "tir_vm_app_products_bwd": 1,
                     "tir_vm_density_bwd": 1, "tir_vm_density_grad": 1, "tir_vm_density_grad_bwd": 1,

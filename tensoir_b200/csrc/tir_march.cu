@@ -50,7 +50,34 @@ struct MarchParams {
   uint32_t* sample_count;
   int64_t capacity;
   unsigned long long* counters;
+  // density volume (VOL instances): the box [vlo, vlo+vn) of grid vertices, [z][y][x]; nullptr when the box is empty
+  const float* vol;
+  int vlo[3], vn[3];
 };
+
+// The density feature at a normalised point as the trilinear interpolation of the baked volume (TirDensityVolume).  The
+// per-axis taps and weights are linear_setup's, i.e. the same unnormalize / floor_fi / zero-weight rule the factor path
+// uses for the plane and line taps of that axis; only the association of the products differs.  Clamping into the box
+// keeps every read in bounds; a valid sample's taps lie inside the box by construction (tir_density_volume_extent).
+__device__ __forceinline__ float volume_feature(const MarchParams& p, float x, float y, float z) {
+  if (!p.vol) return 0.f;
+  const Linear1 tx = linear_setup(x, p.f.grid[0]), ty = linear_setup(y, p.f.grid[1]), tz = linear_setup(z, p.f.grid[2]);
+  const int nx = p.vn[0], ny = p.vn[1], nz = p.vn[2];
+  const int x0 = min(max(tx.o0 - p.vlo[0], 0), nx - 1), x1 = min(max(tx.o1 - p.vlo[0], 0), nx - 1);
+  const int y0 = min(max(ty.o0 - p.vlo[1], 0), ny - 1), y1 = min(max(ty.o1 - p.vlo[1], 0), ny - 1);
+  const int z0 = min(max(tz.o0 - p.vlo[2], 0), nz - 1), z1 = min(max(tz.o1 - p.vlo[2], 0), nz - 1);
+  const float* r00 = p.vol + ((size_t)z0 * ny + y0) * nx;
+  const float* r01 = p.vol + ((size_t)z0 * ny + y1) * nx;
+  const float* r10 = p.vol + ((size_t)z1 * ny + y0) * nx;
+  const float* r11 = p.vol + ((size_t)z1 * ny + y1) * nx;
+  const float a00 = fmaf(__ldg(r00 + x1), tx.w1, __fmul_rn(__ldg(r00 + x0), tx.w0));
+  const float a01 = fmaf(__ldg(r01 + x1), tx.w1, __fmul_rn(__ldg(r01 + x0), tx.w0));
+  const float a10 = fmaf(__ldg(r10 + x1), tx.w1, __fmul_rn(__ldg(r10 + x0), tx.w0));
+  const float a11 = fmaf(__ldg(r11 + x1), tx.w1, __fmul_rn(__ldg(r11 + x0), tx.w0));
+  const float b0 = fmaf(a01, ty.w1, __fmul_rn(a00, ty.w0));
+  const float b1 = fmaf(a11, ty.w1, __fmul_rn(a10, ty.w0));
+  return fmaf(b1, tz.w1, __fmul_rn(b0, tz.w0));
+}
 
 // Segmented warp scans over lanes whose segment heads are flagged (consecutive samples of one ray form a segment).
 __device__ __forceinline__ float seg_scan_mul(float v, bool head, int lane) {
@@ -80,7 +107,7 @@ __device__ __forceinline__ float seg_scan_add(float v, bool head, int lane) {
   return v;
 }
 
-template <int C, int SAMPLING, bool WITH_APP, bool DENSE>
+template <int C, int SAMPLING, bool WITH_APP, bool DENSE, bool VOL>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, kBlocksPerSM) march_kernel(const MarchParams p) {
   __shared__ QEntry queue[kWarpsPerBlock][kQueue];
   __shared__ uint32_t brick_bits[kBrickMaxWords];
@@ -114,7 +141,10 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, kBlocksPerSM) march_kerne
     const QEntry e = q[active ? lane : 0];
     const int ray_l = active ? e.ray : -2 - lane;
     float sigma = 0.f;
-    if (active) sigma = feature_to_sigma(f, density_feature<C>(f, e.x, e.y, e.z));
+    if (active) {
+      const float feat = VOL ? volume_feature(p, e.x, e.y, e.z) : density_feature<C>(f, e.x, e.y, e.z);
+      sigma = feature_to_sigma(f, feat);
+    }
     // raw2alpha: alpha = 1 - exp(-sigma * (dist*scale)); T = cumprod(1 - alpha + 1e-10)
     const float alpha = active ? __fsub_rn(1.f, expf(__fmul_rn(-sigma, __fmul_rn(e.dist, scale)))) : 0.f;
     const int prev_ray = __shfl_up_sync(0xffffffffu, ray_l, 1);
@@ -356,7 +386,7 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, kBlocksPerSM) march_kerne
   }
 }
 
-template <bool WITH_APP, bool DENSE>
+template <bool WITH_APP, bool DENSE, bool VOL = false>
 int launch_march(const MarchParams& p, cudaStream_t stream) {
   if (p.n_rays <= 0) return TIR_OK;
   if (p.f.dC != 16) return TIR_ERR_SHAPE;
@@ -366,17 +396,123 @@ int launch_march(const MarchParams& p, cudaStream_t stream) {
   const int64_t max_blocks = (int64_t)num_sms() * kBlocksPerSM;
   if (blocks > max_blocks) blocks = max_blocks;
   if (p.cfg.sampling == TIR_SAMPLE_STEP) {
-    march_kernel<16, TIR_SAMPLE_STEP, WITH_APP, DENSE><<<(int)blocks, kWarpsPerBlock * 32, 0, stream>>>(p);
+    march_kernel<16, TIR_SAMPLE_STEP, WITH_APP, DENSE, VOL><<<(int)blocks, kWarpsPerBlock * 32, 0, stream>>>(p);
   } else if (p.cfg.sampling == TIR_SAMPLE_TABLE) {
     if (!p.cfg.z_table) return TIR_ERR_NULL;
-    march_kernel<16, TIR_SAMPLE_TABLE, WITH_APP, DENSE><<<(int)blocks, kWarpsPerBlock * 32, 0, stream>>>(p);
+    march_kernel<16, TIR_SAMPLE_TABLE, WITH_APP, DENSE, VOL><<<(int)blocks, kWarpsPerBlock * 32, 0, stream>>>(p);
   } else {
     return TIR_ERR_CONFIG;
   }
   return (int)cudaGetLastError();
 }
 
+// Density volume builder: D[x,y,z] = sum_k sum_c plane_k[c] * line_k[c] at the grid vertices of the box.  A CTA is a
+// 32 (x) x 8 (y) tile of vertices and walks kVolZ consecutive z.  The three factor rows that do not depend on z
+// (plane 0 at (x,y), line 1 at y, line 2 at x) stay in registers for the whole walk; per z a warp reads line 0 at z
+// (one row for the CTA), plane 2 at (y,z) (one row per warp) and plane 1 at (x,z) (coalesced along x).
+constexpr int kVolTileX = 32, kVolTileY = 8, kVolZ = 8;
+
+__device__ __forceinline__ float dot16(const float (&a)[16], const float* b) {
+  float s = 0.f;
+#pragma unroll
+  for (int c = 0; c < 16; c += 4) {           // channel order, like density_feature
+    const float4 v = ldg4(b + c);
+    s = __fadd_rn(s, __fmul_rn(a[c + 0], v.x));
+    s = __fadd_rn(s, __fmul_rn(a[c + 1], v.y));
+    s = __fadd_rn(s, __fmul_rn(a[c + 2], v.z));
+    s = __fadd_rn(s, __fmul_rn(a[c + 3], v.w));
+  }
+  return s;
+}
+
+__device__ __forceinline__ void load16(float (&a)[16], const float* src) {
+#pragma unroll
+  for (int c = 0; c < 16; c += 4) {
+    const float4 v = ldg4(src + c);
+    a[c] = v.x; a[c + 1] = v.y; a[c + 2] = v.z; a[c + 3] = v.w;
+  }
+}
+
+__global__ void __launch_bounds__(kVolTileX * kVolTileY) density_volume_kernel(const TirField f, TirDensityVolume v) {
+  const int xi = blockIdx.x * kVolTileX + threadIdx.x, yi = blockIdx.y * kVolTileY + threadIdx.y;
+  if (xi >= v.n[0] || yi >= v.n[1]) return;
+  const int X = f.grid[0], Y = f.grid[1];
+  const int x = v.lo[0] + xi, y = v.lo[1] + yi;
+  // matMode {0,1},{0,2},{1,2}, vecMode {2,1,0}: plane k is [G[m1]][G[m0]][C], line k is [G[v]][C]
+  float p0[16], l1[16], l2[16];
+  load16(p0, f.dplane[0] + ((size_t)y * X + x) * 16);
+  load16(l1, f.dline[1] + (size_t)y * 16);
+  load16(l2, f.dline[2] + (size_t)x * 16);
+  const int z_end = min(v.n[2], (int)(blockIdx.z + 1) * kVolZ);
+  for (int zi = blockIdx.z * kVolZ; zi < z_end; ++zi) {
+    const int z = v.lo[2] + zi;
+    const float s0 = dot16(p0, f.dline[0] + (size_t)z * 16);
+    const float s1 = dot16(l1, f.dplane[1] + ((size_t)z * X + x) * 16);
+    const float s2 = dot16(l2, f.dplane[2] + ((size_t)z * Y + y) * 16);
+    v.data[((size_t)zi * v.n[1] + yi) * v.n[0] + xi] = __fadd_rn(__fadd_rn(s0, s1), s2);
+  }
+}
+
+// grid vertex index of world coordinate c along `axis`, with the march's normalize_coord / unnormalize arithmetic
+int host_floor_index(const TirField& f, int axis, float c) {
+  const float n = (c - f.aabb_lo[axis]) * f.inv_aabb[axis] - 1.f;
+  const float i = ((n + 1.f) * 0.5f) * (float)(f.grid[axis] - 1);
+  const float lim = (float)f.grid[axis] + 2.f;                 // keeps the int conversion in range
+  return (int)floorf(fminf(fmaxf(i, -lim), lim));
+}
+
+// validate a box handed in by the caller against the field's grid
+int check_box(const TirField& f, const TirDensityVolume& v, bool* empty) {
+  *empty = false;
+  for (int a = 0; a < 3; ++a) {
+    if (v.n[a] < 0 || v.lo[a] < 0 || (int64_t)v.lo[a] + v.n[a] > f.grid[a]) return TIR_ERR_SHAPE;
+    if (v.n[a] == 0) *empty = true;
+  }
+  if (!*empty && !v.data) return TIR_ERR_NULL;
+  return TIR_OK;
+}
+
 }  // namespace
+
+extern "C" int tir_density_volume_extent(const TirField* field, int32_t lo[3], int32_t n[3]) {
+  if (!field || !lo || !n) return TIR_ERR_NULL;
+  const TirField& f = *field;
+  for (int a = 0; a < 3; ++a)
+    if (f.grid[a] < 1) return TIR_ERR_SHAPE;
+  const bool box = f.amask != nullptr && f.occ_lo[0] <= f.occ_hi[0];
+  bool empty = false;
+  for (int a = 0; a < 3; ++a) {
+    if (!box) { lo[a] = 0; n[a] = f.grid[a]; continue; }
+    // taps floor(i) and floor(i)+1 of every coordinate in [occ_lo, occ_hi] (the arithmetic is monotone), plus a
+    // one-vertex guard on each side for any host / device rounding difference
+    const int i0 = host_floor_index(f, a, f.occ_lo[a]) - 1;
+    const int i1 = host_floor_index(f, a, f.occ_hi[a]) + 2;
+    const int a0 = i0 < 0 ? 0 : i0, a1 = i1 > f.grid[a] - 1 ? f.grid[a] - 1 : i1;
+    lo[a] = a0;
+    n[a] = a1 >= a0 ? a1 - a0 + 1 : 0;
+    if (n[a] == 0) empty = true;
+  }
+  if (empty)
+    for (int a = 0; a < 3; ++a) { lo[a] = 0; n[a] = 0; }
+  return TIR_OK;
+}
+
+extern "C" int tir_density_volume_build(const TirField* field, TirDensityVolume* vol, int64_t capacity, void* stream) {
+  if (!field || !vol) return TIR_ERR_NULL;
+  const TirField& f = *field;
+  if (f.dC != 16) return TIR_ERR_SHAPE;
+  bool empty = false;
+  if (int rc = check_box(f, *vol, &empty)) return rc;
+  if (empty) return TIR_OK;
+  if ((int64_t)vol->n[0] * vol->n[1] * vol->n[2] > capacity) return TIR_ERR_CAPACITY;
+  for (int k = 0; k < 3; ++k)
+    if (!f.dplane[k] || !f.dline[k]) return TIR_ERR_NULL;
+  const dim3 block(kVolTileX, kVolTileY);
+  const dim3 grid((vol->n[0] + kVolTileX - 1) / kVolTileX, (vol->n[1] + kVolTileY - 1) / kVolTileY,
+                  (vol->n[2] + kVolZ - 1) / kVolZ);
+  density_volume_kernel<<<grid, block, 0, (cudaStream_t)stream>>>(f, *vol);
+  return (int)cudaGetLastError();
+}
 
 extern "C" int tir_march_density(const TirField* field, const float* rays_o, const float* rays_d, int64_t n_rays,
                                  const TirMarchCfg* cfg, float* t_last, float* acc, float* depth,
@@ -406,10 +542,12 @@ extern "C" int tir_march_radiance(const TirField* field, const TirMlp* mlp, cons
   return tir_app_mlp(field, mlp, samples, sample_count, capacity, rays_d, 0, light_idx, rgb, stream);
 }
 
-extern "C" int tir_secondary_march(const TirField* field, const float* surf_xyz, const float* normals,
-                                  int64_t n_pts, const float* dirs, int32_t n_dirs, const TirMarchCfg* cfg,
-                                  float* vis, TirAppSample* samples, uint32_t* sample_count, int64_t capacity,
-                                  uint64_t* counters, void* stream) {
+namespace {
+// tir_secondary_march(_vol): vol == nullptr selects the factor path
+int secondary_march(const TirField* field, const float* surf_xyz, const float* normals, int64_t n_pts,
+                    const float* dirs, int32_t n_dirs, const TirMarchCfg* cfg, const TirDensityVolume* vol, float* vis,
+                    TirAppSample* samples, uint32_t* sample_count, int64_t capacity, uint64_t* counters,
+                    void* stream) {
   if (n_pts <= 0) return TIR_OK;   // empty input: nothing to do (pointers of empty tensors are NULL)
   if (!field || !cfg || !surf_xyz || !normals || !dirs || !vis || !samples || !sample_count) return TIR_ERR_NULL;
   if (n_dirs <= 0) return TIR_ERR_SHAPE;
@@ -420,7 +558,30 @@ extern "C" int tir_secondary_march(const TirField* field, const float* surf_xyz,
   p.n_rays = n_pts * (int64_t)n_dirs;
   p.t_last = vis; p.counters = (unsigned long long*)counters;
   p.samples = samples; p.sample_count = sample_count; p.capacity = capacity;
-  return launch_march<true, true>(p, (cudaStream_t)stream);
+  if (!vol) return launch_march<true, true, false>(p, (cudaStream_t)stream);
+  bool empty = false;
+  if (int rc = check_box(*field, *vol, &empty)) return rc;
+  p.vol = empty ? nullptr : vol->data;
+  for (int a = 0; a < 3; ++a) { p.vlo[a] = vol->lo[a]; p.vn[a] = vol->n[a]; }
+  return launch_march<true, true, true>(p, (cudaStream_t)stream);
+}
+}  // namespace
+
+extern "C" int tir_secondary_march(const TirField* field, const float* surf_xyz, const float* normals,
+                                  int64_t n_pts, const float* dirs, int32_t n_dirs, const TirMarchCfg* cfg,
+                                  float* vis, TirAppSample* samples, uint32_t* sample_count, int64_t capacity,
+                                  uint64_t* counters, void* stream) {
+  return secondary_march(field, surf_xyz, normals, n_pts, dirs, n_dirs, cfg, nullptr, vis, samples, sample_count,
+                         capacity, counters, stream);
+}
+
+extern "C" int tir_secondary_march_vol(const TirField* field, const float* surf_xyz, const float* normals,
+                                      int64_t n_pts, const float* dirs, int32_t n_dirs, const TirMarchCfg* cfg,
+                                      const TirDensityVolume* vol, float* vis, TirAppSample* samples,
+                                      uint32_t* sample_count, int64_t capacity, uint64_t* counters, void* stream) {
+  if (n_pts > 0 && !vol) return TIR_ERR_NULL;
+  return secondary_march(field, surf_xyz, normals, n_pts, dirs, n_dirs, cfg, vol, vis, samples, sample_count,
+                         capacity, counters, stream);
 }
 
 extern "C" int tir_secondary_radiance(const TirField* field, const TirMlp* mlp, const float* surf_xyz,
@@ -432,6 +593,20 @@ extern "C" int tir_secondary_radiance(const TirField* field, const TirMlp* mlp, 
   if (!mlp || !indirect) return TIR_ERR_NULL;
   int rc = tir_secondary_march(field, surf_xyz, normals, n_pts, dirs, n_dirs, cfg, vis, samples, sample_count,
                                capacity, counters, stream);
+  if (rc) return rc;
+  return tir_app_mlp(field, mlp, samples, sample_count, capacity, dirs, n_dirs, light_idx, indirect, stream);
+}
+
+extern "C" int tir_secondary_radiance_vol(const TirField* field, const TirMlp* mlp, const float* surf_xyz,
+                                          const float* normals, const int32_t* light_idx, int64_t n_pts,
+                                          const float* dirs, int32_t n_dirs, const TirMarchCfg* cfg,
+                                          const TirDensityVolume* vol, float* vis, float* indirect,
+                                          TirAppSample* samples, uint32_t* sample_count, int64_t capacity,
+                                          uint64_t* counters, void* stream) {
+  if (n_pts <= 0) return TIR_OK;   // empty input: nothing to do (pointers of empty tensors are NULL)
+  if (!mlp || !indirect) return TIR_ERR_NULL;
+  int rc = tir_secondary_march_vol(field, surf_xyz, normals, n_pts, dirs, n_dirs, cfg, vol, vis, samples,
+                                   sample_count, capacity, counters, stream);
   if (rc) return rc;
   return tir_app_mlp(field, mlp, samples, sample_count, capacity, dirs, n_dirs, light_idx, indirect, stream);
 }

@@ -176,6 +176,28 @@ def lean_counters(model) -> bool:
     return bool(model.__dict__.get("_tir_lean", False))
 
 
+def density_volume(model, f) -> "_lib.TirDensityVolume":
+    """The density feature baked at the grid vertices the secondary march can read (tir_density_volume_extent /
+    tir_density_volume_build), built from the factors ``f`` points at, on the current stream.  Callers build it on every
+    march: it is never reused across calls, so it can never be older than the parameters.  The storage is sized to the
+    whole grid and kept on the model, so its address is stable for CUDA-graph capture; it is replaced only when the grid
+    changes."""
+    lib = _lib.load()
+    lo, n = (C.c_int32 * 3)(), (C.c_int32 * 3)()
+    _lib.check(lib.tir_density_volume_extent(C.byref(f), lo, n), "tir_density_volume_extent")
+    size = f.grid[0] * f.grid[1] * f.grid[2]
+    dev = model.density_plane[0].device
+    buf = model.__dict__.get("_tir_density_vol")
+    if buf is None or buf.numel() != size or buf.device != dev:
+        buf = torch.empty(size, device=dev)
+        model.__dict__["_tir_density_vol"] = buf
+    vol = _lib.TirDensityVolume()
+    vol.data, vol.lo, vol.n = buf.data_ptr(), lo, n
+    _lib.check(lib.tir_density_volume_build(C.byref(f), C.byref(vol), size, _lib.stream_ptr()),
+               "tir_density_volume_build")
+    return vol
+
+
 def secondary_radiance(model, surf_xyz, normals, light_idx, dirs, *, n_sample=96, near=0.05, far=1.5,
                        counters=None, capacity=None):
     """Secondary shading of render_with_BRDF -> (vis [n_pts,n_dirs,1], indirect [n_pts,n_dirs,3], scratch)."""
@@ -197,14 +219,16 @@ def secondary_radiance(model, surf_xyz, normals, light_idx, dirs, *, n_sample=96
     st = model.__dict__.get("_tir_static")
     per_slot = 4 if st is None else int(st.get("sec_per_slot", 4))
     cap = capacity if capacity is not None else max(1 << 16, per_slot * n_pts * n_dirs)
+    vol = density_volume(model, f)
     while True:
         sc = _scratch(model, dev, cap)
-        _lib.check(lib.tir_secondary_radiance(C.byref(f), C.byref(mlp), _lib.dptr(sx), _lib.dptr(nr),
-                                              _lib.dptr(li, torch.int32), n_pts, _lib.dptr(dr), n_dirs, C.byref(cfg),
-                                              _lib.dptr(vis), _lib.dptr(ind), _lib.dptr(sc.buf, torch.uint8),
-                                              _lib.dptr(sc.count, torch.int32), sc.capacity,
-                                              None if counters is None else _lib.dptr(counters, torch.int64),
-                                              _lib.stream_ptr()), "tir_secondary_radiance")
+        _lib.check(lib.tir_secondary_radiance_vol(C.byref(f), C.byref(mlp), _lib.dptr(sx), _lib.dptr(nr),
+                                                  _lib.dptr(li, torch.int32), n_pts, _lib.dptr(dr), n_dirs,
+                                                  C.byref(cfg), C.byref(vol), _lib.dptr(vis), _lib.dptr(ind),
+                                                  _lib.dptr(sc.buf, torch.uint8), _lib.dptr(sc.count, torch.int32),
+                                                  sc.capacity,
+                                                  None if counters is None else _lib.dptr(counters, torch.int64),
+                                                  _lib.stream_ptr()), "tir_secondary_radiance_vol")
         if st is not None:
             # shape-static mode (CUDA-graph capture): no host sync; the step's overflow flag turns an overflowed step
             # into a no-op that the host redoes with a larger scratch list (static_step.py)
@@ -242,10 +266,12 @@ def app_mlp_points(model, xn, x_in, light_idx=None, *, head="renderModule", ligh
 
 
 class SecondaryStages:
-    """The two kernels of tir_secondary_radiance as separately launchable stages (bench / profiling):
-    ``march()`` = cosine test + density march + compaction, ``mlp()`` = appearance gather + MLP on the list."""
+    """The two stages of tir_secondary_radiance_vol as separately launchable stages (bench / profiling):
+    ``march()`` = density-volume build + cosine test + density march + compaction, ``mlp()`` = appearance gather + MLP
+    on the list."""
 
     def __init__(self, model, surf_xyz, normals, light_idx, dirs, n_sample=96, near=0.05, far=1.5):
+        self.model = model
         self.lib = _lib.load()
         self.f = device_field(model).refresh(model)
         self.keep = []
@@ -265,12 +291,14 @@ class SecondaryStages:
     def march(self):
         self.sc.count.zero_()
         self.counters.zero_()
-        _lib.check(self.lib.tir_secondary_march(C.byref(self.f), _lib.dptr(self.sx), _lib.dptr(self.nr), self.n_pts,
-                                                _lib.dptr(self.dr), self.n_dirs, C.byref(self.cfg),
-                                                _lib.dptr(self.vis), _lib.dptr(self.sc.buf, torch.uint8),
-                                                _lib.dptr(self.sc.count, torch.int32), self.sc.capacity,
-                                                _lib.dptr(self.counters, torch.int64), _lib.stream_ptr()),
-                   "tir_secondary_march")
+        vol = density_volume(self.model, self.f)
+        _lib.check(self.lib.tir_secondary_march_vol(C.byref(self.f), _lib.dptr(self.sx), _lib.dptr(self.nr),
+                                                    self.n_pts, _lib.dptr(self.dr), self.n_dirs, C.byref(self.cfg),
+                                                    C.byref(vol), _lib.dptr(self.vis),
+                                                    _lib.dptr(self.sc.buf, torch.uint8),
+                                                    _lib.dptr(self.sc.count, torch.int32), self.sc.capacity,
+                                                    _lib.dptr(self.counters, torch.int64), _lib.stream_ptr()),
+                   "tir_secondary_march_vol")
 
     def mlp(self):
         _lib.check(self.lib.tir_app_mlp(C.byref(self.f), C.byref(self.mlp_s), _lib.dptr(self.sc.buf, torch.uint8),

@@ -177,11 +177,12 @@ class StaticTrainStep:
         torch.cuda.synchronize()
         for slot in self._slots:
             slot["event"], slot["batch"] = None, None
-        # The captured kernels hold raw pointers into buffers owned elsewhere (the sample-list scratch, the alpha-mask
-        # and VM shadows).  Keep references so that a later eager call that re-sizes / rebuilds them cannot hand the
-        # memory back to the allocator while this graph can still be replayed.
+        # The captured kernels hold raw pointers into buffers owned elsewhere (the sample-list scratch, the density
+        # volume, the alpha-mask and VM shadows).  Keep references so that a later eager call that re-sizes / rebuilds
+        # them cannot hand the memory back to the allocator while this graph can still be replayed.
         df = self.model.__dict__.get("_tir_device_field")
-        self._keepalive = [self.model.__dict__.get("_tir_scratch"), self.model.alphaMask,
+        self._keepalive = [self.model.__dict__.get("_tir_scratch"), self.model.__dict__.get("_tir_density_vol"),
+                           self.model.alphaMask,
                            None if df is None else (df.dplane, df.dline, df.aplane, df.aline, df.amask, df.acell)]
         self._captured_for = self._model_signature()
         return self
