@@ -240,39 +240,23 @@ int tir_secondary_march_vol(const TirField* field, const float* surf_xyz, const 
 
 /* Appearance gather + basis_mat + MLPRender_Fea on a compacted sample list
  * (compute_appfeature tensoRF_rotated_lights.py:197-224 + MLPRender_Fea tensorBase:136-146):
- *   rgb_out[ray] += weight * sigmoid(mlp(...)) for every sample; dirs_of_ray gives the view dir.
- *   ray_dirs [n_rays,3] when dir_stride_rays = 1, or the [n_dirs,3] table with ray % n_dirs indexing
- *   when n_dirs > 0.  light_idx indexed by ray (n_dirs == 0) or by ray / n_dirs. */
+ *   rgb_out[ray] += weight * sigmoid(mlp(...)) for every sample; mlp->out_dim must be 3.
+ *   The view dir of a sample is ray_dirs[ray] ([n_rays,3]) when n_dirs == 0, or the [n_dirs,3] table row ray % n_dirs
+ *   when n_dirs > 0.  light_idx indexed by ray (n_dirs == 0) or by ray / n_dirs.
+ * Runs the sm_90a wgmma kernel (csrc/tir_mlp_wgmma.cu): A operand and accumulator in registers, split-BF16 weights
+ * resident in shared memory, two warpgroups per CTA on different 64-sample tiles. */
 int tir_app_mlp(const TirField* field, const TirMlp* mlp, const TirAppSample* samples,
                 const uint32_t* sample_count, int64_t max_samples, const float* ray_dirs, int32_t n_dirs,
                 const int32_t* light_idx, float* rgb_out, void* stream);
 
-/* The two implementations behind tir_app_mlp (which dispatches to _wgmma unless the environment has TIR_MLP_LEGACY=1):
- *   _wgmma   sm_90a-native: wgmma.mma_async with the A operand and the accumulator in registers, weights resident
- *            in shared memory, two warpgroups per CTA on different 64-sample tiles (csrc/tir_mlp_wgmma.cu)
- *   _legacy  round 1: mma.sync.m16n8k16 on 64-sample tiles (csrc/tir_mlp.cu)
- * Same arguments and results (both use the error-compensated split-BF16 product with fp32 accumulation). */
-int tir_app_mlp_wgmma(const TirField* field, const TirMlp* mlp, const TirAppSample* samples,
-                      const uint32_t* sample_count, int64_t max_samples, const float* ray_dirs, int32_t n_dirs,
-                      const int32_t* light_idx, float* rgb_out, void* stream);
-int tir_app_mlp_legacy(const TirField* field, const TirMlp* mlp, const TirAppSample* samples,
-                       const uint32_t* sample_count, int64_t max_samples, const float* ray_dirs, int32_t n_dirs,
-                       const int32_t* light_idx, float* rgb_out, void* stream);
-int tir_app_mlp_points_wgmma(const TirField* field, const TirMlp* mlp, const float* xn, const float* x_in,
-                             const int32_t* light_idx, int64_t n, int32_t act, float* out, void* stream);
-int tir_app_mlp_points_legacy(const TirField* field, const TirMlp* mlp, const float* xn, const float* x_in,
-                              const int32_t* light_idx, int64_t n, int32_t act, float* out, void* stream);
-
-/* Same gather+MLP on explicit points (no compositing): xn [n,3] normalised coords, x_in [n,3] the 3-vector fed
+/* The same gather + MLP on explicit points (no compositing): xn [n,3] normalised coords, x_in [n,3] the 3-vector fed
  * to the MLP next to the features (view dir for MLPRender_Fea, position for MLPBRDF_PEandFeature),
  * light_idx [n] or NULL (row 0 of mlp->light_line, e.g. the mean-light row of compute_intrinfeature),
- * act 0 = sigmoid, 1 = tanh -> out [n,out_dim].  Mirrors renderModule*(compute_*feature(...)). */
-int tir_app_mlp_points(const TirField* field, const TirMlp* mlp, const float* xn, const float* x_in,
-                       const int32_t* light_idx, int64_t n, int32_t act, float* out, void* stream);
-
-/* tir_app_mlp_points that also dumps the activations a host-side backward needs (training forward of the primary
- * MLP heads): save_xl [n, 3*aC] light-scaled products, save_in [n, in_dim] MLP input incl. positional encoding,
- * save_h1 / save_h2 [n, hidden] post-ReLU hidden layers; any of them may be NULL. */
+ * act 0 = sigmoid, 1 = tanh -> out [n,out_dim].  Mirrors renderModule*(compute_*feature(...)).
+ * Optionally dumps the activations a host-side backward needs (training forward of the primary MLP heads):
+ * save_xl [n, 3*aC] light-scaled products, save_in [n, in_dim] MLP input incl. positional encoding,
+ * save_h1 / save_h2 [n, hidden] post-ReLU hidden layers; any of them may be NULL.
+ * Runs the split-BF16 mma.sync kernel of the primary heads (csrc/tir_mlp.cu). */
 int tir_app_mlp_points_save(const TirField* field, const TirMlp* mlp, const float* xn, const float* x_in,
                             const int32_t* light_idx, int64_t n, int32_t act, float* out, float* save_xl,
                             float* save_in, float* save_h1, float* save_h2, void* stream);

@@ -156,16 +156,6 @@ EXPORTS = {
                                           C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "tir_app_mlp": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), C.c_void_p, C.c_void_p, C.c_int64, f32p,
                               C.c_int32, C.c_void_p, f32p, C.c_void_p]),
-    "tir_app_mlp_wgmma": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), C.c_void_p, C.c_void_p, C.c_int64, f32p,
-                                  C.c_int32, C.c_void_p, f32p, C.c_void_p]),
-    "tir_app_mlp_legacy": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), C.c_void_p, C.c_void_p, C.c_int64, f32p,
-                                     C.c_int32, C.c_void_p, f32p, C.c_void_p]),
-    "tir_app_mlp_points_wgmma": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), f32p, f32p, C.c_void_p, C.c_int64,
-                                         C.c_int32, f32p, C.c_void_p]),
-    "tir_app_mlp_points_legacy": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), f32p, f32p, C.c_void_p, C.c_int64,
-                                            C.c_int32, f32p, C.c_void_p]),
-    "tir_app_mlp_points": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), f32p, f32p, C.c_void_p, C.c_int64,
-                                     C.c_int32, f32p, C.c_void_p]),
     "tir_app_mlp_points_save": (C.c_int, [C.POINTER(TirField), C.POINTER(TirMlp), f32p, f32p, C.c_void_p, C.c_int64,
                                           C.c_int32, f32p, f32p, f32p, f32p, f32p, C.c_void_p]),
     "tir_shade_fwd": (C.c_int, [f32p, f32p, f32p, f32p, f32p, C.c_void_p, C.c_int64, f32p, f32p, C.c_int32, f32p,
@@ -247,9 +237,8 @@ EXPORTS = {
 KERNELS_PER_CALL = {"tir_pack_channels_last": 1, "tir_unpack_channels_last_add": 1, "tir_pack_alpha_mask": 3,
                     "tir_density_points": 1, "tir_alpha_mask_points": 1, "tir_march_density": 1,
                     "tir_march_radiance": 2, "tir_secondary_march": 1, "tir_secondary_radiance": 2,
-                    "tir_density_volume_build": 1, "tir_secondary_march_vol": 1, "tir_secondary_radiance_vol": 2, "tir_app_mlp": 1, "tir_app_mlp_wgmma": 1, "tir_app_mlp_legacy": 1, "tir_app_mlp_points_wgmma": 1,
-                    "tir_app_mlp_points_legacy": 1,
-                    "tir_shade_fwd": 1, "tir_shade_bwd": 1, "tir_app_mlp_points": 1, "tir_app_mlp_points_save": 1, "tir_vm_app_products": 1, "tir_vm_app_products_bwd": 1,
+                    "tir_density_volume_build": 1, "tir_secondary_march_vol": 1, "tir_secondary_radiance_vol": 2, "tir_app_mlp": 1,
+                    "tir_shade_fwd": 1, "tir_shade_bwd": 1, "tir_app_mlp_points_save": 1, "tir_vm_app_products": 1, "tir_vm_app_products_bwd": 1,
                     "tir_vm_density_bwd": 1, "tir_vm_density_grad": 1, "tir_vm_density_grad_bwd": 1,
                     "tir_valid_samples_count": 1, "tir_valid_samples_fill": 1, "tir_composite_fwd": 1,
                     "tir_adam_step": 2, "tir_tv_loss": 1, "tir_tv_loss_bwd": 1, "tir_generate_rays": 1, "tir_hits_prepare": 1, "tir_shade_hits_fwd": 1, "tir_shade_hits_bwd": 1,

@@ -1,7 +1,8 @@
 // Appearance gather (3 x 48-channel plane*line products) -> * light_line -> basis_mat (144 -> 27) ->
-// positional encoding -> 150 -> 128 -> 128 -> {3,4} MLP, on a compacted list of samples.
-// Replaces compute_appfeature / compute_intrinfeature (tensoRF_rotated_lights.py:167-224) + MLPRender_Fea /
-// MLPBRDF_PEandFeature (tensorBase:122-146, :182-208).
+// positional encoding -> 150 -> 128 -> 128 -> {3,4} MLP, on explicit points: the primary appearance heads, up to four
+// per launch, with optional activation dumps for the backward.  Replaces compute_appfeature / compute_intrinfeature
+// (tensoRF_rotated_lights.py:167-224) + MLPRender_Fea / MLPBRDF_PEandFeature (tensorBase:122-146, :182-208).
+// The secondary sample list goes through the wgmma kernel of tir_mlp_wgmma.cu.
 //
 // The four contractions are genuine dense GEMMs over a tile of 64 samples and run on the tensor cores with
 // error-compensated BF16: every fp32 operand x is split into hi = bf16(x), lo = bf16(x - hi) and the product is
@@ -10,7 +11,6 @@
 // resident in shared memory as split BF16 (176 KB) and stream 64-sample tiles through one in-place activation
 // buffer; fragments are fetched with ldmatrix from rows padded to an odd multiple of 16 bytes (conflict free).
 #include <cuda_bf16.h>
-#include <cstdlib>
 #include "tir_device.cuh"
 #include "tir_internal.h"
 
@@ -44,22 +44,12 @@ struct Smem {
   float lmean[K0];                           // mean light row (light_mode 2, compute_intrinfeature)
   float xn[M][3];
   float xv[M][3];
-  float wgt[M];
-  int ray[M];
   int light[M];
 };
 
 struct MlpParams {
   TirField f;
-  TirMlp mlp;
-  const TirAppSample* samples;
-  const uint32_t* sample_count;
-  int64_t max_samples;
-  const float* ray_dirs;
-  int n_dirs;
-  const int32_t* light_idx;
-  float* rgb_out;
-  // POINTS mode: up to 4 heads, CTA b works on job b % n_jobs (tir_internal.h)
+  // up to 4 heads, CTA b works on job b % n_jobs (tir_internal.h)
   HeadJobDev jobs[kMaxHeadJobs];
   int n_jobs;
   int64_t n_points;
@@ -166,19 +156,18 @@ __device__ __forceinline__ void dump_tile(const __nv_bfloat16* ah, const __nv_bf
   }
 }
 
-template <bool POINTS>
 __global__ void __launch_bounds__(NT, 1) app_mlp_kernel(const MlpParams p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem& s = *reinterpret_cast<Smem*>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int g = lane >> 2, t4 = lane & 3;
-  const int n_jobs = POINTS ? p.n_jobs : 1;
-  const int job = POINTS ? (int)(blockIdx.x % n_jobs) : 0;
+  const int n_jobs = p.n_jobs;
+  const int job = (int)(blockIdx.x % n_jobs);
   const HeadJobDev& J = p.jobs[job];
-  const TirMlp& mlp = POINTS ? J.mlp : p.mlp;
+  const TirMlp& mlp = J.mlp;
   const int out_dim = mlp.out_dim;
-  const int light_mode = POINTS ? J.light_mode : (mlp.light_line ? 1 : 0);
-  const int act = POINTS ? J.act : 0;
+  const int light_mode = J.light_mode;
+  const int act = J.act;
 
   // ---- stage split-BF16 weights once per CTA (PyTorch [out,in] layout is already the mma "col" operand)
   for (int i = tid; i < HID * SW0; i += NT) {
@@ -208,38 +197,28 @@ __global__ void __launch_bounds__(NT, 1) app_mlp_kernel(const MlpParams p) {
   }
   __syncthreads();
 
-  const int64_t total = POINTS ? list_rows(p.n_points, p.n_dev)
-                               : (int64_t)min((unsigned long long)*p.sample_count, (unsigned long long)p.max_samples);
+  const int64_t total = list_rows(p.n_points, p.n_dev);
   const int64_t n_tiles = (total + M - 1) / M;
-  const int64_t tile0 = POINTS ? (int64_t)(blockIdx.x / n_jobs) : (int64_t)blockIdx.x;
-  const int64_t tstep = POINTS ? (int64_t)(gridDim.x / n_jobs) : (int64_t)gridDim.x;
+  const int64_t tile0 = (int64_t)(blockIdx.x / n_jobs);
+  const int64_t tstep = (int64_t)(gridDim.x / n_jobs);
 
   for (int64_t tile = tile0; tile < n_tiles; tile += tstep) {
     const int64_t base = tile * M;
-    // ---- sample metadata
+    // ---- point metadata
     if (tid < M) {
       const int64_t i = base + tid;
-      float xn0 = 0.f, xn1 = 0.f, xn2 = 0.f, v0 = 0.f, v1 = 0.f, v2 = 0.f, w = 0.f;
-      int ray = -1, li = 0;
+      float xn0 = 0.f, xn1 = 0.f, xn2 = 0.f, v0 = 0.f, v1 = 0.f, v2 = 0.f;
+      int li = 0;
       if (i < total) {
-        if (POINTS) {
-          xn0 = J.xn[i * 3 + 0]; xn1 = J.xn[i * 3 + 1]; xn2 = J.xn[i * 3 + 2];
-          const int64_t r = J.x_index ? (int64_t)J.x_index[i] : i;
-          const float* xi = J.x_in + r * J.x_in_stride;
-          v0 = xi[0]; v1 = xi[1]; v2 = xi[2];
-          ray = (int)i; w = 1.f;
-          li = J.light_idx ? J.light_idx[r] : 0;
-        } else {
-          const TirAppSample sm = p.samples[i];
-          xn0 = sm.xn[0]; xn1 = sm.xn[1]; xn2 = sm.xn[2]; w = sm.weight; ray = sm.ray;
-          const int64_t di = p.n_dirs > 0 ? (int64_t)(ray % p.n_dirs) : (int64_t)ray;
-          v0 = __ldg(p.ray_dirs + di * 3 + 0); v1 = __ldg(p.ray_dirs + di * 3 + 1); v2 = __ldg(p.ray_dirs + di * 3 + 2);
-          li = p.light_idx ? __ldg(p.light_idx + (p.n_dirs > 0 ? ray / p.n_dirs : ray)) : 0;
-        }
+        xn0 = J.xn[i * 3 + 0]; xn1 = J.xn[i * 3 + 1]; xn2 = J.xn[i * 3 + 2];
+        const int64_t r = J.x_index ? (int64_t)J.x_index[i] : i;
+        const float* xi = J.x_in + r * J.x_in_stride;
+        v0 = xi[0]; v1 = xi[1]; v2 = xi[2];
+        li = J.light_idx ? J.light_idx[r] : 0;
       }
       s.xn[tid][0] = xn0; s.xn[tid][1] = xn1; s.xn[tid][2] = xn2;
       s.xv[tid][0] = v0; s.xv[tid][1] = v1; s.xv[tid][2] = v2;
-      s.wgt[tid] = w; s.ray[tid] = ray; s.light[tid] = li;
+      s.light[tid] = li;
     }
     __syncthreads();
 
@@ -249,7 +228,7 @@ __global__ void __launch_bounds__(NT, 1) app_mlp_kernel(const MlpParams p) {
       const float xn[3] = {s.xn[m][0], s.xn[m][1], s.xn[m][2]};
       const float* lrow = light_mode == 1 ? (mlp.light_line + (size_t)s.light[m] * K0)
                                           : (light_mode == 2 ? s.lmean : nullptr);
-      float* x0_dst = (POINTS && J.save_x0 && base + m < total) ? J.save_x0 + (base + m) * K0 : nullptr;
+      float* x0_dst = (J.save_x0 && base + m < total) ? J.save_x0 + (base + m) * K0 : nullptr;
 #pragma unroll
       for (int k = 0; k < 3; ++k) {
         const int m0 = kMat0[k], m1 = kMat1[k], v = kVec[k];
@@ -277,7 +256,7 @@ __global__ void __launch_bounds__(NT, 1) app_mlp_kernel(const MlpParams p) {
       }
     }
     __syncthreads();
-    if (POINTS && p.save_xl && job == 0) dump_tile(s.ah, s.al, p.save_xl, K0, base, total, tid);
+    if (p.save_xl && job == 0) dump_tile(s.ah, s.al, p.save_xl, K0, base, total, tid);
 
     // ---- phase 2: basis_mat (144 -> 27, N padded to 32): warp w -> m-tile w/2, n-tiles 2*(w%2), +1
     {
@@ -328,7 +307,7 @@ __global__ void __launch_bounds__(NT, 1) app_mlp_kernel(const MlpParams p) {
       }
     }
     __syncthreads();
-    if (POINTS && J.save_in) dump_tile(s.ah, s.al, J.save_in, IN, base, total, tid);
+    if (J.save_in) dump_tile(s.ah, s.al, J.save_in, IN, base, total, tid);
 
     // ---- phases 3/4: hidden layers.  warp w -> all 64 rows x units [16w, 16w+16)
     auto hidden_layer = [&](const __nv_bfloat16* wh, const __nv_bfloat16* wl, int sw, const float* bias, int K) {
@@ -348,11 +327,11 @@ __global__ void __launch_bounds__(NT, 1) app_mlp_kernel(const MlpParams p) {
       __syncthreads();
     };
     hidden_layer(s.w0h, s.w0l, SW0, s.b0, K1);
-    if (POINTS && J.save_h1) dump_tile(s.ah, s.al, J.save_h1, HID, base, total, tid);
+    if (J.save_h1) dump_tile(s.ah, s.al, J.save_h1, HID, base, total, tid);
     hidden_layer(s.w1h, s.w1l, SW1, s.b1, HID);
-    if (POINTS && J.save_h2) dump_tile(s.ah, s.al, J.save_h2, HID, base, total, tid);
+    if (J.save_h2) dump_tile(s.ah, s.al, J.save_h2, HID, base, total, tid);
 
-    // ---- phase 5: output layer (N padded to 8) on warps 0..3, activation, composite
+    // ---- phase 5: output layer (N padded to 8) on warps 0..3, activation
     if (warp < 4) {
       float acc[1][1][4] = {};
       warp_gemm<1, 1>(acc, s.ah, s.al, warp * 16, s.w2h, s.w2l, SW2, 0, HID, lane);
@@ -364,10 +343,7 @@ __global__ void __launch_bounds__(NT, 1) app_mlp_kernel(const MlpParams p) {
           const float a = acc[0][0][e] + s.b2[o];
           const float y = act == 0 ? 1.f / (1.f + expf(-a)) : tanhf(a);
           const int64_t i = base + row;
-          if (i < total) {
-            if (POINTS) J.out[i * J.out_stride + o] = y;
-            else atomicAdd(p.rgb_out + (int64_t)s.ray[row] * 3 + o, __fmul_rn(s.wgt[row], y));
-          }
+          if (i < total) J.out[i * J.out_stride + o] = y;
         }
       }
     }
@@ -383,107 +359,39 @@ int check_shapes(const TirField* f, const TirMlp* m) {
   return TIR_OK;
 }
 
-template <bool POINTS>
-int launch(const MlpParams& p, int64_t max_items, cudaStream_t stream) {
-  static bool configured[2] = {false, false};
+int launch(const MlpParams& p, int64_t n, cudaStream_t stream) {
+  static bool configured = false;
   const int smem = (int)sizeof(Smem);
-  if (!configured[POINTS]) {
-    cudaError_t e = cudaFuncSetAttribute(app_mlp_kernel<POINTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(app_mlp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return (int)e;
-    configured[POINTS] = true;
+    configured = true;
   }
-  int64_t tiles = (max_items + M - 1) / M;
-  const int nj = POINTS ? (p.n_jobs > 0 ? p.n_jobs : 1) : 1;
+  int64_t tiles = (n + M - 1) / M;
+  const int nj = p.n_jobs;
   int per_job = num_sms() / nj;                            // CTAs per job: one wave, one CTA per SM
   if (tiles < per_job) per_job = (int)(tiles > 0 ? tiles : 1);
-  app_mlp_kernel<POINTS><<<per_job * nj, NT, smem, stream>>>(p);
+  app_mlp_kernel<<<per_job * nj, NT, smem, stream>>>(p);
   return (int)cudaGetLastError();
 }
 
 }  // namespace
 
-extern "C" int tir_app_mlp_wgmma(const TirField* field, const TirMlp* mlp, const TirAppSample* samples,
-                                 const uint32_t* sample_count, int64_t max_samples, const float* ray_dirs,
-                                 int32_t n_dirs, const int32_t* light_idx, float* rgb_out, void* stream);
-extern "C" int tir_app_mlp_points_wgmma(const TirField* field, const TirMlp* mlp, const float* xn, const float* x_in,
-                                        const int32_t* light_idx, int64_t n, int32_t act, float* out, void* stream);
-
-// TIR_MLP_LEGACY=1 selects the round-1 mma.sync kernel for the inference entry points (A/B comparison); the default is
-// the wgmma kernel of tir_mlp_wgmma.cu.  The training forward with activation dumps always uses this file.
-static bool legacy_mlp() {
-  static const bool v = [] { const char* e = getenv("TIR_MLP_LEGACY"); return e && e[0] == '1'; }();
-  return v;
-}
-
-extern "C" int tir_app_mlp_legacy(const TirField* field, const TirMlp* mlp, const TirAppSample* samples,
-                                  const uint32_t* sample_count, int64_t max_samples, const float* ray_dirs,
-                                  int32_t n_dirs, const int32_t* light_idx, float* rgb_out, void* stream);
-
-extern "C" int tir_app_mlp(const TirField* field, const TirMlp* mlp, const TirAppSample* samples,
-                           const uint32_t* sample_count, int64_t max_samples, const float* ray_dirs, int32_t n_dirs,
-                           const int32_t* light_idx, float* rgb_out, void* stream) {
-  if (!legacy_mlp())
-    return tir_app_mlp_wgmma(field, mlp, samples, sample_count, max_samples, ray_dirs, n_dirs, light_idx, rgb_out, stream);
-  return tir_app_mlp_legacy(field, mlp, samples, sample_count, max_samples, ray_dirs, n_dirs, light_idx, rgb_out, stream);
-}
-
-extern "C" int tir_app_mlp_legacy(const TirField* field, const TirMlp* mlp, const TirAppSample* samples,
-                                  const uint32_t* sample_count, int64_t max_samples, const float* ray_dirs,
-                                  int32_t n_dirs, const int32_t* light_idx, float* rgb_out, void* stream) {
-  if (!field || !mlp || !samples || !sample_count || !ray_dirs || !rgb_out) return TIR_ERR_NULL;
-  int rc = check_shapes(field, mlp);
-  if (rc) return rc;
-  if (mlp->out_dim != 3) return TIR_ERR_SHAPE;
-  MlpParams p{};
-  p.f = *field; p.mlp = *mlp; p.samples = samples; p.sample_count = sample_count; p.max_samples = max_samples;
-  p.ray_dirs = ray_dirs; p.n_dirs = n_dirs; p.light_idx = light_idx; p.rgb_out = rgb_out;
-  return launch<false>(p, max_samples, (cudaStream_t)stream);
-}
-
-static void legacy_job(MlpParams& p, const TirMlp* mlp, const float* xn, const float* x_in, const int32_t* light_idx,
-                       int64_t n, int32_t act, float* out) {
-  p.n_jobs = 1; p.n_points = n; p.n_dev = nullptr;
-  HeadJobDev& J = p.jobs[0];
-  J = HeadJobDev{};
-  J.mlp = *mlp; J.xn = xn; J.x_in = x_in; J.x_index = nullptr; J.x_in_stride = 3; J.light_idx = light_idx;
-  J.light_mode = mlp->light_line ? 1 : 0; J.act = act; J.out = out; J.out_stride = mlp->out_dim;
-}
-
 extern "C" int tir_app_mlp_points_save(const TirField* field, const TirMlp* mlp, const float* xn, const float* x_in,
                                        const int32_t* light_idx, int64_t n, int32_t act, float* out, float* save_xl,
                                        float* save_in, float* save_h1, float* save_h2, void* stream) {
-  if (n <= 0) return TIR_OK;
-  if (!field || !mlp || !xn || !x_in || !out) return TIR_ERR_NULL;
-  int rc = check_shapes(field, mlp);
-  if (rc) return rc;
-  if (act != 0 && act != 1) return TIR_ERR_CONFIG;
-  MlpParams p{};
-  p.f = *field;
-  legacy_job(p, mlp, xn, x_in, light_idx, n, act, out);
-  p.save_xl = save_xl; p.jobs[0].save_in = save_in; p.jobs[0].save_h1 = save_h1; p.jobs[0].save_h2 = save_h2;
-  return launch<true>(p, n, (cudaStream_t)stream);
-}
-
-extern "C" int tir_app_mlp_points_legacy(const TirField* field, const TirMlp* mlp, const float* xn, const float* x_in,
-                                         const int32_t* light_idx, int64_t n, int32_t act, float* out, void* stream);
-
-extern "C" int tir_app_mlp_points(const TirField* field, const TirMlp* mlp, const float* xn, const float* x_in,
-                                  const int32_t* light_idx, int64_t n, int32_t act, float* out, void* stream) {
-  if (!legacy_mlp()) return tir_app_mlp_points_wgmma(field, mlp, xn, x_in, light_idx, n, act, out, stream);
-  return tir_app_mlp_points_legacy(field, mlp, xn, x_in, light_idx, n, act, out, stream);
-}
-
-extern "C" int tir_app_mlp_points_legacy(const TirField* field, const TirMlp* mlp, const float* xn, const float* x_in,
-                                         const int32_t* light_idx, int64_t n, int32_t act, float* out, void* stream) {
   if (n <= 0) return TIR_OK;   // empty input: nothing to do (pointers of empty tensors are NULL)
   if (!field || !mlp || !xn || !x_in || !out) return TIR_ERR_NULL;
   int rc = check_shapes(field, mlp);
   if (rc) return rc;
   if (act != 0 && act != 1) return TIR_ERR_CONFIG;
   MlpParams p{};
-  p.f = *field;
-  legacy_job(p, mlp, xn, x_in, light_idx, n, act, out);
-  return launch<true>(p, n, (cudaStream_t)stream);
+  p.f = *field; p.n_jobs = 1; p.n_points = n; p.n_dev = nullptr; p.save_xl = save_xl;
+  HeadJobDev& J = p.jobs[0];
+  J.mlp = *mlp; J.xn = xn; J.x_in = x_in; J.x_index = nullptr; J.x_in_stride = 3; J.light_idx = light_idx;
+  J.light_mode = mlp->light_line ? 1 : 0; J.act = act; J.out = out; J.out_stride = mlp->out_dim;
+  J.save_in = save_in; J.save_h1 = save_h1; J.save_h2 = save_h2;
+  return launch(p, n, (cudaStream_t)stream);
 }
 
 namespace tir {
@@ -500,6 +408,6 @@ int launch_heads_forward(const TirField& f, const HeadJobDev* jobs, int n_jobs, 
     if (jobs[j].light_mode != 0 && !jobs[j].mlp.light_line) return TIR_ERR_NULL;
     p.jobs[j] = jobs[j];
   }
-  return launch<true>(p, n, stream);
+  return launch(p, n, stream);
 }
 }  // namespace tir

@@ -16,7 +16,7 @@
 //   * two warpgroups per CTA work on different tiles, so one warpgroup's L2-latency-bound gather overlaps the other's
 //     tensor-core work;
 //   * three GEMMs per tile: basis_mat (K = 144, N = 32), layer 0 (K = 160, N = 128), layer 1 (K = 128, N = 128).
-//   The last layer (128 -> 3/4, < 1 % of the FLOPs) runs in fp32 on the CUDA cores with a quad shuffle reduction.
+//   The last layer (128 -> 3, < 1 % of the FLOPs) runs in fp32 on the CUDA cores with a quad shuffle reduction.
 #include <cuda_bf16.h>
 #include "tir_device.cuh"
 #include "tir_internal.h"
@@ -45,13 +45,11 @@ struct SmemW {
   uint8_t bsl[32 * K0 * 2];
   float w2[4 * HID];
   float b0[HID], b1[HID], b2[4];
-  float lmean[K0];
 };
 
 struct WgParams {
   TirField f;
   TirMlp mlp;
-  // sample-list mode
   const TirAppSample* samples;
   const uint32_t* sample_count;
   int64_t max_samples;
@@ -59,13 +57,6 @@ struct WgParams {
   int n_dirs;
   const int32_t* light_idx;
   float* rgb_out;
-  // points mode
-  const float* pts_xn;
-  const float* pts_x;
-  int64_t n_points;
-  float* out;
-  int act;
-  int light_mode;     // 0 none, 1 indexed row, 2 mean row
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -150,33 +141,25 @@ struct RowIn {
   bool live;
 };
 
-template <bool POINTS>
 __device__ __forceinline__ RowIn load_row(const WgParams& p, int64_t i, int64_t total) {
   RowIn r{};
   r.live = i < total;
   if (!r.live) return r;
-  if (POINTS) {
-    r.xn[0] = p.pts_xn[i * 3]; r.xn[1] = p.pts_xn[i * 3 + 1]; r.xn[2] = p.pts_xn[i * 3 + 2];
-    r.xv[0] = p.pts_x[i * 3]; r.xv[1] = p.pts_x[i * 3 + 1]; r.xv[2] = p.pts_x[i * 3 + 2];
-    r.li = p.light_idx ? p.light_idx[i] : 0;
-  } else {
-    const TirAppSample sm = p.samples[i];
-    r.xn[0] = sm.xn[0]; r.xn[1] = sm.xn[1]; r.xn[2] = sm.xn[2]; r.wgt = sm.weight; r.ray = sm.ray;
-    const int64_t di = p.n_dirs > 0 ? (int64_t)(sm.ray % p.n_dirs) : (int64_t)sm.ray;
-    r.xv[0] = __ldg(p.ray_dirs + di * 3); r.xv[1] = __ldg(p.ray_dirs + di * 3 + 1); r.xv[2] = __ldg(p.ray_dirs + di * 3 + 2);
-    r.li = p.light_idx ? __ldg(p.light_idx + (p.n_dirs > 0 ? sm.ray / p.n_dirs : sm.ray)) : 0;
-  }
+  const TirAppSample sm = p.samples[i];
+  r.xn[0] = sm.xn[0]; r.xn[1] = sm.xn[1]; r.xn[2] = sm.xn[2]; r.wgt = sm.weight; r.ray = sm.ray;
+  const int64_t di = p.n_dirs > 0 ? (int64_t)(sm.ray % p.n_dirs) : (int64_t)sm.ray;
+  r.xv[0] = __ldg(p.ray_dirs + di * 3); r.xv[1] = __ldg(p.ray_dirs + di * 3 + 1); r.xv[2] = __ldg(p.ray_dirs + di * 3 + 2);
+  r.li = p.light_idx ? __ldg(p.light_idx + (p.n_dirs > 0 ? sm.ray / p.n_dirs : sm.ray)) : 0;
   return r;
 }
 
-template <bool POINTS>
 __global__ void __launch_bounds__(NTHREADS, 1) app_mlp_wgmma_kernel(const WgParams p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   SmemW& s = *reinterpret_cast<SmemW*>(smem_raw);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int wg = warp >> 2, g = lane >> 2, t4 = lane & 3;
   const TirMlp& mlp = p.mlp;
-  const int out_dim = mlp.out_dim;
+  const bool light = mlp.light_line != nullptr;   // (plane * line) * light_line[li], or plane * line
 
   // ---- stage the split-BF16 weights (K axes permuted as described at the top), once per persistent CTA
   for (int i = tid; i < HID * K1; i += NTHREADS) {
@@ -191,28 +174,21 @@ __global__ void __launch_bounds__(NTHREADS, 1) app_mlp_wgmma_kernel(const WgPara
     const int ch = (k & ~15) + 4 * pos_t4(pp) + pos_e(pp);          // product channel at logical position k
     stage(s.bsh, s.bsl, n, k, 32, n < F ? __ldg(mlp.basis + n * K0 + ch) : 0.f);
   }
-  for (int i = tid; i < 4 * HID; i += NTHREADS) s.w2[i] = (i / HID) < out_dim ? __ldg(mlp.w2 + i) : 0.f;
+  for (int i = tid; i < 4 * HID; i += NTHREADS) s.w2[i] = (i / HID) < 3 ? __ldg(mlp.w2 + i) : 0.f;
   for (int i = tid; i < HID; i += NTHREADS) { s.b0[i] = __ldg(mlp.b0 + i); s.b1[i] = __ldg(mlp.b1 + i); }
-  if (tid < 4) s.b2[tid] = tid < out_dim ? __ldg(mlp.b2 + tid) : 0.f;
-  if (p.light_mode == 2)
-    for (int c = tid; c < K0; c += NTHREADS) {
-      float a = 0.f;
-      for (int l = 0; l < mlp.n_lights; ++l) a += __ldg(mlp.light_line + (size_t)l * K0 + c);
-      s.lmean[c] = a / (float)mlp.n_lights;
-    }
+  if (tid < 4) s.b2[tid] = tid < 3 ? __ldg(mlp.b2 + tid) : 0.f;
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to wgmma
   __syncthreads();
 
   const uint32_t a_bsh = smem_u32(s.bsh), a_bsl = smem_u32(s.bsl);
   const uint32_t a_w0h = smem_u32(s.w0h), a_w0l = smem_u32(s.w0l), a_w1h = smem_u32(s.w1h), a_w1l = smem_u32(s.w1l);
-  const int64_t total = POINTS ? p.n_points
-                               : (int64_t)min((unsigned long long)*p.sample_count, (unsigned long long)p.max_samples);
+  const int64_t total = (int64_t)min((unsigned long long)*p.sample_count, (unsigned long long)p.max_samples);
   const int64_t n_tiles = (total + ROWS - 1) / ROWS;
 
   for (int64_t tile = (int64_t)blockIdx.x * NWG + wg; tile < n_tiles; tile += (int64_t)gridDim.x * NWG) {
     // this thread's two rows of the tile: the A / accumulator fragment rows g and g + 8 of its warp's 16-row slice
     const int64_t row0 = tile * ROWS + (warp & 3) * 16 + g;
-    RowIn rw[2] = {load_row<POINTS>(p, row0, total), load_row<POINTS>(p, row0 + 8, total)};
+    RowIn rw[2] = {load_row(p, row0, total), load_row(p, row0 + 8, total)};
 
     // ---- gather: products (plane * line * light) -> split-BF16 A fragments of the basis GEMM (9 k16 steps)
     uint32_t ah[9][4], al[9][4];
@@ -225,7 +201,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) app_mlp_wgmma_kernel(const WgPara
         const Linear1 l = linear_setup(rw[h].xn[v], p.f.grid[v]);
         const float* P = p.f.aplane[k];
         const float* L = p.f.aline[k];
-        const float* lrow = p.light_mode == 1 ? (mlp.light_line + (size_t)rw[h].li * K0) : nullptr;
+        const float* lrow = light ? (mlp.light_line + (size_t)rw[h].li * K0) : nullptr;
 #pragma unroll
         for (int ks = 0; ks < AC / 16; ++ks) {
           const int c = ks * 16 + 4 * t4, col = k * AC + c;
@@ -235,18 +211,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) app_mlp_wgmma_kernel(const WgPara
                                       ldg4(P + (size_t)b.o10 * AC + c), ldg4(P + (size_t)b.o11 * AC + c), b);
             const float4 lv = lerp4(ldg4(L + (size_t)l.o0 * AC + c), ldg4(L + (size_t)l.o1 * AC + c), l);
             x = make_float4(__fmul_rn(pv.x, lv.x), __fmul_rn(pv.y, lv.y), __fmul_rn(pv.z, lv.z), __fmul_rn(pv.w, lv.w));
-            if (p.light_mode == 1) {            // (plane * line) * light  (tensoRF_rotated_lights.py:222)
+            if (light) {                        // (plane * line) * light  (tensoRF_rotated_lights.py:222)
               const float4 lc = ldg4(lrow + col);
               x.x = __fmul_rn(x.x, lc.x); x.y = __fmul_rn(x.y, lc.y); x.z = __fmul_rn(x.z, lc.z); x.w = __fmul_rn(x.w, lc.w);
-            } else if (p.light_mode == 2) {
-              x.x = __fmul_rn(x.x, s.lmean[col]); x.y = __fmul_rn(x.y, s.lmean[col + 1]);
-              x.z = __fmul_rn(x.z, s.lmean[col + 2]); x.w = __fmul_rn(x.w, s.lmean[col + 3]);
             }
           }
           split_pack(x.x, x.y, ah[k * 3 + ks][h], al[k * 3 + ks][h]);
           split_pack(x.z, x.w, ah[k * 3 + ks][2 + h], al[k * 3 + ks][2 + h]);
         }
       }
+      // keeps the next orientation's loads behind this one's: hoisted across it, they raise the kernel from 197 to
+      // ~220 registers
+      __syncwarp();
     }
 
     // ---- basis_mat on the tensor cores: feat = products @ basis^T (27 of 32 accumulator columns)
@@ -347,7 +323,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) app_mlp_wgmma_kernel(const WgPara
     wgmma_wait_all();
     fence_regs(acc);
 
-    // ---- layer 1 epilogue + output layer (128 -> out_dim, fp32 on the CUDA cores, quad reduction)
+    // ---- layer 1 epilogue + output layer (128 -> 3, fp32 on the CUDA cores, quad reduction)
     float o[2][4] = {};
 #pragma unroll
     for (int i = 0; i < 16; ++i)
@@ -365,16 +341,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) app_mlp_wgmma_kernel(const WgPara
         o[h][q] += __shfl_xor_sync(0xffffffffu, o[h][q], 1);
         o[h][q] += __shfl_xor_sync(0xffffffffu, o[h][q], 2);
       }
-    const int q = t4;                      // quad thread t4 writes output channel t4 of both rows
-    if (q < out_dim) {
+    const int q = t4;                      // quad thread t4 writes output channel t4 of both rows: weight * sigmoid
+    if (q < 3) {
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         if (!rw[h].live) continue;
-        const float z = o[h][q] + s.b2[q];
-        const float y = p.act == 0 ? 1.f / (1.f + expf(-z)) : tanhf(z);
-        const int64_t i = row0 + 8 * h;
-        if (POINTS) p.out[i * out_dim + q] = y;
-        else atomicAdd(p.rgb_out + (int64_t)rw[h].ray * 3 + q, __fmul_rn(rw[h].wgt, y));
+        const float y = 1.f / (1.f + expf(-(o[h][q] + s.b2[q])));
+        atomicAdd(p.rgb_out + (int64_t)rw[h].ray * 3 + q, __fmul_rn(rw[h].wgt, y));
       }
     }
   }
@@ -383,52 +356,32 @@ __global__ void __launch_bounds__(NTHREADS, 1) app_mlp_wgmma_kernel(const WgPara
 int check_shapes(const TirField* f, const TirMlp* m) {
   if (f->aC != AC) return TIR_ERR_SHAPE;
   if (m->feat_dim != F || m->hidden != HID || m->pe_feat != 2 || m->pe_x != 2) return TIR_ERR_SHAPE;
-  if (m->out_dim < 1 || m->out_dim > 4) return TIR_ERR_SHAPE;
+  if (m->out_dim != 3) return TIR_ERR_SHAPE;
   if (!m->w0 || !m->b0 || !m->w1 || !m->b1 || !m->w2 || !m->b2 || !m->basis) return TIR_ERR_NULL;
   return TIR_OK;
 }
 
-template <bool POINTS>
-int launch_wg(const WgParams& p, int64_t max_items, cudaStream_t stream) {
-  static bool configured[2] = {false, false};
-  const int smem = (int)sizeof(SmemW);
-  if (!configured[POINTS]) {
-    cudaError_t e = cudaFuncSetAttribute(app_mlp_wgmma_kernel<POINTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return (int)e;
-    configured[POINTS] = true;
-  }
-  const int64_t groups = ((max_items + ROWS - 1) / ROWS + NWG - 1) / NWG;
-  const int sms = num_sms();
-  const int blocks = (int)(groups < sms ? (groups > 0 ? groups : 1) : sms);
-  app_mlp_wgmma_kernel<POINTS><<<blocks, NTHREADS, smem, stream>>>(p);
-  return (int)cudaGetLastError();
-}
-
 }  // namespace
 
-extern "C" int tir_app_mlp_wgmma(const TirField* field, const TirMlp* mlp, const TirAppSample* samples,
-                                 const uint32_t* sample_count, int64_t max_samples, const float* ray_dirs,
-                                 int32_t n_dirs, const int32_t* light_idx, float* rgb_out, void* stream) {
+extern "C" int tir_app_mlp(const TirField* field, const TirMlp* mlp, const TirAppSample* samples,
+                           const uint32_t* sample_count, int64_t max_samples, const float* ray_dirs, int32_t n_dirs,
+                           const int32_t* light_idx, float* rgb_out, void* stream) {
   if (!field || !mlp || !samples || !sample_count || !ray_dirs || !rgb_out) return TIR_ERR_NULL;
   int rc = check_shapes(field, mlp);
   if (rc) return rc;
-  if (mlp->out_dim != 3) return TIR_ERR_SHAPE;
+  static bool configured = false;
+  const int smem = (int)sizeof(SmemW);
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(app_mlp_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return (int)e;
+    configured = true;
+  }
   WgParams p{};
   p.f = *field; p.mlp = *mlp; p.samples = samples; p.sample_count = sample_count; p.max_samples = max_samples;
-  p.ray_dirs = ray_dirs; p.n_dirs = n_dirs; p.light_idx = light_idx; p.rgb_out = rgb_out; p.act = 0;
-  p.light_mode = mlp->light_line ? 1 : 0;
-  return launch_wg<false>(p, max_samples, (cudaStream_t)stream);
-}
-
-extern "C" int tir_app_mlp_points_wgmma(const TirField* field, const TirMlp* mlp, const float* xn, const float* x_in,
-                                        const int32_t* light_idx, int64_t n, int32_t act, float* out, void* stream) {
-  if (n <= 0) return TIR_OK;
-  if (!field || !mlp || !xn || !x_in || !out) return TIR_ERR_NULL;
-  int rc = check_shapes(field, mlp);
-  if (rc) return rc;
-  if (act != 0 && act != 1) return TIR_ERR_CONFIG;
-  WgParams p{};
-  p.f = *field; p.mlp = *mlp; p.pts_xn = xn; p.pts_x = x_in; p.n_points = n; p.light_idx = light_idx; p.out = out;
-  p.act = act; p.light_mode = mlp->light_line ? 1 : 0;
-  return launch_wg<true>(p, n, (cudaStream_t)stream);
+  p.ray_dirs = ray_dirs; p.n_dirs = n_dirs; p.light_idx = light_idx; p.rgb_out = rgb_out;
+  const int64_t groups = ((max_samples + ROWS - 1) / ROWS + NWG - 1) / NWG;
+  const int sms = num_sms();
+  const int blocks = (int)(groups < sms ? (groups > 0 ? groups : 1) : sms);
+  app_mlp_wgmma_kernel<<<blocks, NTHREADS, smem, (cudaStream_t)stream>>>(p);
+  return (int)cudaGetLastError();
 }

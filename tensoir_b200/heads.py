@@ -58,96 +58,11 @@ def _head_forward(model, head, light, xn, x_in, li, w0, need, bufs=None):
     return out, xl, inp, h1, h2
 
 
-def _head_backward(act, light, g_out, out, xl, inp, h1, h2, w0, w1, w2, basis, light_w, li, x0):
-    """Hand-written backward of one head on its dumped activations.
-    -> (gw0, gb0, gw1, gb1, gw2, gb2, gbasis, glight or None, gx0 [n, 3*aC])."""
-    n = out.shape[0]
-    g_out = g_out.contiguous()
-    ones = torch.ones(n, device=out.device, dtype=out.dtype)
-
-    def colsum(t):                      # t.sum(0) as a cuBLAS gemv (the strided reduce kernel is 4x slower)
-        return torch.mv(t.t(), ones)
-    gz3 = g_out * (out * (1 - out) if act == 0 else 1 - out * out)
-    gw2, gb2 = _wgrad(gz3, h2), colsum(gz3)
-    gz2 = (gz3 @ w2) * (h2 > 0)
-    gw1, gb1 = _wgrad(gz2, h1), colsum(gz2)
-    gz1 = (gz2 @ w1) * (h1 > 0)
-    gw0, gb0 = _wgrad(gz1, inp), colsum(gz1)
-    gin = gz1 @ w0                                           # [n, in_dim]
-    F, pe = basis.shape[0], 2                                # fea_pe = 2 (checked by the kernel)
-    s0, c0 = F + 3, F + 3 + F * pe
-    freqs = 2.0 ** torch.arange(pe, device=out.device, dtype=inp.dtype)
-    gs, gc = gin[:, s0:s0 + F * pe].reshape(n, F, pe), gin[:, c0:c0 + F * pe].reshape(n, F, pe)
-    sn, cs = inp[:, s0:s0 + F * pe].reshape(n, F, pe), inp[:, c0:c0 + F * pe].reshape(n, F, pe)
-    gfeat = gin[:, :F] + ((gs * cs - gc * sn) * freqs).sum(-1)
-    gbasis = _wgrad(gfeat, xl)
-    gxl = gfeat @ basis                                       # [n, 3*aC]
-    if light == "none":
-        return gw0, gb0, gw1, gb1, gw2, gb2, gbasis, None, gxl
-    if light == "index":                                      # xl = x0 * light_line[li]
-        rows = light_w.index_select(0, li.long())
-        glight = torch.zeros_like(light_w).index_add_(0, li.long(), gxl * x0)
-    else:                                                     # xl = x0 * mean over lights
-        rows = light_w.mean(0, keepdim=True)
-        glight = ((gxl * x0).sum(0, keepdim=True) / light_w.shape[0]).expand_as(light_w)
-    return gw0, gb0, gw1, gb1, gw2, gb2, gbasis, glight, gxl * rows
-
-
-class _FusedHeads(torch.autograd.Function):
-    """Several heads evaluated at the SAME points: one kernel launch per head forward; in the backward the
-    appearance-product gradients of all heads are summed and scattered to the VM factors with ONE kernel."""
-
-    @staticmethod
-    def forward(ctx, model, specs, xn, basis, light_w, *rest):
-        nh = len(specs)
-        per = rest[:8 * nh]                  # per head: x_in, li, w0, b0, w1, b1, w2, b2
-        need = any(ctx.needs_input_grad)
-        outs, saved = [], []
-        for h, (head, light) in enumerate(specs):
-            x_in, li, w0, b0, w1, b1, w2, b2 = per[8 * h:8 * h + 8]
-            out, xl, inp, h1, h2 = _head_forward(model, head, light, xn, x_in, li, w0, need)
-            outs.append(out)
-            if need:
-                saved += [out, xl, inp, h1, h2, w0, w1, w2, li]
-        ctx.model, ctx.specs, ctx.need = model, specs, need
-        ctx.has_light = light_w is not None
-        ctx.save_for_backward(xn, basis, light_w if light_w is not None else torch.empty(0, device=xn.device), *saved)
-        return tuple(outs)
-
-    @staticmethod
-    def backward(ctx, *g_outs):
-        xn, basis, light_w, *saved = ctx.saved_tensors
-        model, specs = ctx.model, ctx.specs
-        n = xn.shape[0]
-        x0 = _raw_products(model, xn) if any(l != "none" for _, l in specs) else None
-        gbasis, glight, gx0 = None, None, None
-        per_grads = []
-        for h, (head, light) in enumerate(specs):
-            out, xl, inp, h1, h2, w0, w1, w2, li = saved[9 * h:9 * h + 9]
-            g = g_outs[h]
-            if g is None:
-                g = torch.zeros_like(out)
-            act = 1 if head == "renderModule_normal" else 0
-            gw0, gb0, gw1, gb1, gw2, gb2, gb_, gl_, gx_ = _head_backward(act, light, g, out, xl, inp, h1, h2, w0, w1,
-                                                                        w2, basis, light_w, li, x0)
-            per_grads += [None, None, gw0, gb0, gw1, gb1, gw2, gb2]
-            gbasis = gb_ if gbasis is None else gbasis + gb_
-            if gl_ is not None:
-                glight = gl_ if glight is None else glight + gl_
-            gx0 = gx_ if gx0 is None else gx0 + gx_
-        lib = _lib.load()
-        df = ops.device_field(model)
-        f = df.refresh(model)
-        gp, gl = _grad_shadows(df, "app")
-        gx0 = gx0.contiguous()
-        _lib.check(lib.tir_vm_app_products_bwd(C.byref(f), _lib.dptr(xn), n, _lib.dptr(gx0), _ptr_array(gp),
-                                               _ptr_array(gl), _lib.stream_ptr()), "tir_vm_app_products_bwd")
-        return (None, None, None, gbasis, glight if ctx.has_light else None, *per_grads, *_to_param_layout(gp, gl))
-
-
-def _wgrad_batched(g, a, splits=8):
-    """Per-head g_h^T @ a_h for stacked operands g [H,n,M], a [H,n,K] -> [H,M,K]; reduction over n split like _wgrad."""
+def _wgrad_batched(g, a):
+    """Per-head g_h^T @ a_h for stacked operands g [H,n,M], a [H,n,K] -> [H,M,K]; reduction over n split like _wgrad:
+    8 slices per head from three heads on, 16 for two and _wgrad's 32 for a single head."""
     H, n, M = g.shape
+    splits = 8 * max(1, 4 // H)
     per = n // splits
     if per < 64:
         return torch.bmm(g.transpose(1, 2), a)
@@ -160,8 +75,8 @@ def _wgrad_batched(g, a, splits=8):
 
 
 def _heads_backward_batched(is_tanh, g_out, out, xl, inp, h1, h2, w0, w1, w2, basis):
-    """MLP / PE / basis part of :func:`_head_backward` for H heads at once (equal sample counts) as batched GEMMs and
-    stacked elementwise ops.  is_tanh [H] bool; g_out / out [H,n,4] (3-output heads zero-padded); xl [H,n,3*aC];
+    """Hand-written backward of the MLP, PE and basis_mat of H heads at once (equal sample counts) on their dumped
+    activations, as batched GEMMs and stacked elementwise ops.  is_tanh [H] bool; g_out / out [H,n,4] (3-output heads zero-padded); xl [H,n,3*aC];
     inp [H,n,in_dim]; h1, h2 [H,n,hid]; w0 [H,hid,in_dim]; w1 [H,hid,hid]; w2 [H,4,hid] (zero-padded rows).
     -> gw0, gb0, gw1, gb1, gw2 [H,4,hid], gb2 [H,4], gbasis (summed over heads), gxl [H,n,3*aC]."""
     H, n, _ = out.shape
@@ -310,30 +225,8 @@ def _raw_products(model, xn):
     return out
 
 
-def fused_heads(model, xn, specs):
-    """Evaluate several heads at the same normalised points ``xn``.
-    specs: list of (head, x_in, light_idx or None, light) with head in {'renderModule' (x_in = view dir, sigmoid),
-    'renderModule_brdf' (x_in = position, sigmoid, 4 outputs), 'renderModule_normal' (position, tanh)} and
-    light in {'index', 'mean', 'none'}.  out_h = act(MLP_h([feat, x_in, PE(feat), PE(x_in)])) with
-    feat = basis_mat(plane*line(xn) * lightvec).  -> tuple of [n, out_dim_h]."""
-    xn = xn.detach().reshape(-1, 3).float().contiguous()
-    dev = xn.device
-    ll = getattr(model, "light_line", None)
-    use_light = ll is not None and any(s[3] != "none" for s in specs)
-    light_w = ll.weight if use_light else None
-    flat, meta = [], []
-    for head, x_in, li, light in specs:
-        mod = getattr(model, head)
-        x_in = x_in.detach().reshape(-1, 3).float().contiguous()
-        li = (torch.empty(0, dtype=torch.int32, device=dev) if li is None
-              else li.detach().reshape(-1).to(torch.int32).contiguous())
-        flat += [x_in, li, mod.mlp[0].weight, mod.mlp[0].bias, mod.mlp[2].weight, mod.mlp[2].bias, mod.mlp[4].weight,
-                 mod.mlp[4].bias]
-        meta.append((head, light if ll is not None else "none"))
-    params = list(model.app_plane) + list(model.app_line)
-    return _FusedHeads.apply(model, tuple(meta), xn, model.basis_mat.weight, light_w, *flat, *params)
-
-
 def fused_head(model, head: str, xn, x_in, light_idx=None, light: str = "index"):
-    """Single-head convenience wrapper of :func:`fused_heads`."""
-    return fused_heads(model, xn, [(head, x_in, light_idx, light)])[0]
+    """One head at the points ``xn``: head in {'renderModule' (x_in = view dir, sigmoid), 'renderModule_brdf' (x_in =
+    position, sigmoid, 4 outputs), 'renderModule_normal' (position, tanh)}, light in {'index', 'mean', 'none'}.
+    out = act(MLP([feat, x_in, PE(feat), PE(x_in)])) with feat = basis_mat(plane*line(xn) * lightvec) -> [n, out_dim]."""
+    return fused_heads_multi(model, [(head, xn, x_in, light_idx, light)])[0]

@@ -259,9 +259,9 @@ def app_mlp_points(model, xn, x_in, light_idx=None, *, head="renderModule", ligh
     li = _i32c(light_idx) if light == "index" else None
     n = xn.shape[0]
     out = torch.empty(n, mlp.out_dim, device=xn.device)
-    _lib.check(lib.tir_app_mlp_points(C.byref(f), C.byref(mlp), _lib.dptr(xn), _lib.dptr(xi),
-                                      None if li is None else _lib.dptr(li, torch.int32), n, act, _lib.dptr(out),
-                                      _lib.stream_ptr()), "tir_app_mlp_points")
+    _lib.check(lib.tir_app_mlp_points_save(C.byref(f), C.byref(mlp), _lib.dptr(xn), _lib.dptr(xi),
+                                           None if li is None else _lib.dptr(li, torch.int32), n, act, _lib.dptr(out),
+                                           None, None, None, None, _lib.stream_ptr()), "tir_app_mlp_points_save")
     return out
 
 

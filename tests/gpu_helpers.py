@@ -55,3 +55,38 @@ def model_from_fixture(fx, device, with_mask=True):
     if with_mask:
         m.alphaMask = AlphaGridMask(device, fx["alpha_aabb"].to(device), fx["alpha_volume"].to(device))
     return m
+
+
+def app_sample_list(xn, weight, ray, sample=None):
+    """A TirAppSample list (24 B per row: xn[3], weight f32, ray, sample i32) for tir_app_mlp, on xn's device
+    -> (uint8 buffer, int32 [1] count).  With one sample per ray at weight 1 and n_dirs = 0, the list kernel writes
+    exactly the per-point MLP output into a zeroed rgb_out."""
+    n = xn.shape[0]
+    if sample is None:
+        sample = torch.zeros(n, dtype=torch.int32, device=xn.device)
+    f = torch.cat([xn.reshape(n, 3).float(), weight.reshape(n, 1).float()], 1).contiguous()
+    i = torch.stack([ray.reshape(n).to(torch.int32), sample.reshape(n).to(torch.int32)], 1).contiguous()
+    buf = torch.cat([f.view(torch.uint8), i.view(torch.uint8)], 1).reshape(-1).contiguous()
+    return buf, torch.tensor([n], dtype=torch.int32, device=xn.device)
+
+
+def app_mlp_list(model, mlp, xn, dirs, light_idx, weight=None, ray=None, n_rays=None):
+    """The wgmma list kernel (tir_app_mlp) on a hand-built list with n_dirs = 0: sample i at xn[i] on ray ray[i] (default
+    i) with weight[i] (default 1), view dir dirs[ray], light light_idx[ray] (or None) -> rgb [n_rays, 3]."""
+    import ctypes as C
+    from tensoir_b200 import _lib, ops
+    n = xn.shape[0]
+    dev = xn.device
+    ray = torch.arange(n, device=dev) if ray is None else ray
+    weight = torch.ones(n, device=dev) if weight is None else weight
+    n_rays = n if n_rays is None else n_rays
+    buf, count = app_sample_list(xn, weight, ray)
+    d = dirs.reshape(-1, 3).float().contiguous()
+    li = None if light_idx is None else light_idx.reshape(-1).to(torch.int32).contiguous()
+    rgb = torch.zeros(n_rays, 3, device=dev)
+    f = ops.device_field(model).refresh(model)
+    _lib.check(_lib.load().tir_app_mlp(C.byref(f), C.byref(mlp), _lib.dptr(buf, torch.uint8),
+                                       _lib.dptr(count, torch.int32), n, _lib.dptr(d), 0,
+                                       None if li is None else _lib.dptr(li, torch.int32), _lib.dptr(rgb),
+                                       _lib.stream_ptr()), "tir_app_mlp")
+    return rgb

@@ -56,6 +56,11 @@ def test_unit_kernels(rot):
     close(ops.app_mlp_points(m, xn, vd, li, head="renderModule"), fx["mlp_rgb"], 5e-5, "mlp_rgb")
     close(ops.app_mlp_points(m, xn, xn, None, head="renderModule_brdf", light="mean"), fx["mlp_brdf"], 5e-5, "brdf")
     close(ops.app_mlp_points(m, xn, xn, None, head="renderModule_normal", light="mean"), fx["mlp_normal"], 5e-5, "nrm")
+    # the wgmma list kernel pinned to the same golden: one sample per ray at weight 1 composes exactly the point output
+    from tensoir_b200.device_field import mlp_struct
+    from gpu_helpers import app_mlp_list
+    keep = []
+    close(app_mlp_list(m, mlp_struct(m, "renderModule", keep), xn, vd, li), fx["mlp_rgb"], 5e-5, "mlp_rgb list")
     # derived normals: compare the raw gradient (absolute, vs its scale) and the unit normals where the gradient
     # is well conditioned (a normalised ~0 gradient amplifies summation-order noise by up to 1e6)
     from tensoir_b200.primary import _derived_normals
@@ -732,34 +737,37 @@ def test_fused_primary_matches_modular_path(golden_rotated, kind):
 
 
 def test_wgmma_mlp_matches_mma_sync_kernel(rot):
-    """The sm_90a-native appearance MLP (wgmma.mma_async, A operand + accumulator in registers, csrc/tir_mlp_wgmma.cu)
-    against the round-1 mma.sync kernel: explicit points for the three heads (ragged sizes incl. a partial tile and an
-    odd number of tiles), and the secondary appearance list."""
-    import ctypes as C
-    from tensoir_b200 import _lib, ops
+    """The sm_90a-native list kernel (wgmma.mma_async, A operand + accumulator in registers, csrc/tir_mlp_wgmma.cu,
+    through tir_app_mlp) against the mma.sync heads kernel (csrc/tir_mlp.cu, through tir_app_mlp_points_save) composed
+    with index_add: hand-built lists of ragged sizes (a partial tile, an odd number of tiles) with one sample per ray at
+    weight 1 and with several samples per ray at random weights, in both light modes of the list kernel; and the
+    secondary appearance list of a real march."""
+    from tensoir_b200 import ops
     from tensoir_b200.device_field import mlp_struct
+    from gpu_helpers import app_mlp_list
     fx, m = rot
-    lib = _lib.load()
-    f = ops.device_field(m).refresh(m)
+    n_lights = m.light_line.weight.shape[0]
     g = torch.Generator().manual_seed(7)
     for n in (1, 127, 128, 300, 5000):
         xn = (torch.rand(n, 3, generator=g) * 1.9 - 0.95).to(DEV)
         xi = torch.nn.functional.normalize(torch.randn(n, 3, generator=g), dim=-1).to(DEV)
-        li = torch.zeros(n, dtype=torch.int32, device=DEV)
-        for head, light, act in (("renderModule", "index", 0), ("renderModule_brdf", "mean", 0),
-                                 ("renderModule_normal", "mean", 1)):
+        li = torch.randint(0, n_lights, (n,), generator=g, dtype=torch.int32).to(DEV)
+        n_rays = max(1, n // 3)
+        ray = torch.randint(0, n_rays, (n,), generator=g).to(DEV)
+        w = torch.rand(n, generator=g).to(DEV)
+        for light in ("index", "none"):
             keep = []
-            mlp = mlp_struct(m, head, keep, light=light)
-            outs = []
-            for fn in (lib.tir_app_mlp_points_legacy, lib.tir_app_mlp_points_wgmma):
-                out = torch.full((n, mlp.out_dim), -7.0, device=DEV)
-                _lib.check(fn(C.byref(f), C.byref(mlp), _lib.dptr(xn), _lib.dptr(xi),
-                              _lib.dptr(li, torch.int32) if light == "index" else None, n, act, _lib.dptr(out),
-                              _lib.stream_ptr()), "mlp points")
-                outs.append(out)
-            torch.cuda.synchronize()
-            close(outs[1], outs[0], 2e-5, f"{head} n={n}")
-    # sample-list form on a real secondary march
+            mlp = mlp_struct(m, "renderModule", keep, light=light)
+            l_pt = li if light == "index" else None
+            want = ops.app_mlp_points(m, xn, xi, l_pt, head="renderModule", light=light)
+            got = app_mlp_list(m, mlp, xn, xi, l_pt)
+            close(got, want, 2e-5, f"one sample per ray, light {light} n={n}")
+            # several samples per ray: view dir and light of the sample's ray
+            y = ops.app_mlp_points(m, xn, xi[ray], None if l_pt is None else li[ray], head="renderModule", light=light)
+            want = torch.zeros(n_rays, 3, device=DEV).index_add_(0, ray, w[:, None] * y)
+            got = app_mlp_list(m, mlp, xn, xi, l_pt, weight=w, ray=ray, n_rays=n_rays)
+            close(got, want, 2e-5, f"weighted samples, light {light} n={n}")
+    # sample-list form on a real secondary march (n_dirs > 0: view dir dirs[ray % n_dirs], light li[ray // n_dirs])
     with torch.no_grad():
         out = m(fx["rays"].to(DEV), fx["light_idx"].to(DEV), is_train=False, is_relight=True, N_samples=-1)
     rays = fx["rays"].to(DEV)
@@ -768,16 +776,15 @@ def test_wgmma_mlp_matches_mma_sync_kernel(rot):
     dirs = m.gen_light_incident_dirs(method='fixed_envirmap').to(DEV)
     st = ops.SecondaryStages(m, surf, out[2][mask], fx["light_idx"].to(DEV)[mask], dirs, n_sample=24)
     st.march()
-    res = []
-    for fn in (lib.tir_app_mlp_legacy, lib.tir_app_mlp_wgmma):
-        st.ind.zero_()
-        _lib.check(fn(C.byref(st.f), C.byref(st.mlp_s), _lib.dptr(st.sc.buf, torch.uint8),
-                      _lib.dptr(st.sc.count, torch.int32), st.sc.capacity, _lib.dptr(st.dr), st.n_dirs,
-                      _lib.dptr(st.li, torch.int32), _lib.dptr(st.ind), _lib.stream_ptr()), "mlp list")
-        res.append(st.ind.clone())
+    st.ind.zero_()
+    st.mlp()
+    sm = st.sc.samples()
+    assert sm["ray"].shape[0] > 100
+    r = sm["ray"].long()
+    y = ops.app_mlp_points(m, sm["xn"], st.dr[r % st.n_dirs], st.li[r // st.n_dirs], head="renderModule")
+    want = torch.zeros(st.n_pts * st.n_dirs, 3, device=DEV).index_add_(0, r, sm["weight"][:, None] * y)
     torch.cuda.synchronize()
-    assert int(st.sc.count.item()) > 100
-    close(res[1], res[0], 2e-5, "indirect light")
+    close(st.ind.reshape(-1, 3), want, 2e-5, "indirect light")
 
 
 def _lego_pair(grid):

@@ -1,7 +1,8 @@
 """CPU test of the autograd plumbing of heads._FusedHeadsMulti (H heads, own points per head, ONE stacked backward):
 the CUDA entry points are replaced by torch emulations of what they compute, and every gradient the node returns is
 compared with torch autograd of the same composition.  Exercises slot ordering, zero-padding of 3-output heads, the
-three light modes, group-wise summation before the appearance scatter and weight sharing between two heads."""
+three light modes, group-wise summation before the appearance scatter and weight sharing between two heads, and the
+single-head wrapper on a model without light_line (the light-free radiance head of TensorVMSplitInit)."""
 import types
 
 import pytest
@@ -57,7 +58,8 @@ def world(monkeypatch):
     def head_forward(_model, head, light, xn, x_in, li, w0, need, bufs=None):
         mod = getattr(_model, head)
         x0 = raw_products(_model, xn)
-        rows = _light_rows(light, _model.light_line.weight.detach(), li, xn.shape[0])
+        ll = getattr(_model, "light_line", None)
+        rows = None if ll is None else _light_rows(light, ll.weight.detach(), li, xn.shape[0])
         xl = x0 if rows is None else x0 * rows
         inp = _mlp_input(xl @ _model.basis_mat.weight.detach().t(), x_in)
         h1 = torch.relu(inp @ mod.mlp[0].weight.detach().t() + mod.mlp[0].bias.detach())
@@ -90,29 +92,27 @@ def world(monkeypatch):
     return model, proj, scattered
 
 
-def test_multi_head_backward_matches_autograd(world):
-    model, proj, scattered = world
-    n = 300
-    x_a, x_j = torch.rand(n, 3) * 2 - 1, torch.rand(n, 3) * 2 - 1
-    vd = torch.nn.functional.normalize(torch.randn(n, 3), dim=-1)
-    li = torch.randint(0, 3, (n,), dtype=torch.int32)
-    specs = [("renderModule", x_a, vd, li, "index"), ("renderModule_brdf", x_a, x_a, None, "mean"),
-             ("renderModule_normal", x_a, x_a, None, "mean"), ("renderModule_brdf", x_j, x_j, None, "mean")]
-    outs = heads.fused_heads_multi(model, specs)
+def _check_against_autograd(model, proj, scattered, specs, outs):
+    """Every gradient of the node against torch autograd of the same composition, and one appearance scatter per point
+    set fed with the summed d loss / d x0 of the heads at those points."""
+    n = specs[0][1].shape[0]
+    ll = getattr(model, "light_line", None)
+    mods = [getattr(model, h) for h in dict.fromkeys(s[0] for s in specs)]
+    params = [p for m in mods for p in m.parameters()] + [model.basis_mat.weight] + ([] if ll is None else [ll.weight])
     G = [torch.randn_like(o) for o in outs]
-    params = ([p for m in (model.renderModule, model.renderModule_brdf, model.renderModule_normal) for p in m.parameters()]
-              + [model.basis_mat.weight, model.light_line.weight])
     torch.autograd.backward(outs, G)
     got = [p.grad.clone() for p in params]
     for p in params:
         p.grad = None
 
     # reference: the same composition, differentiated by autograd (x0 of each point set as a leaf to get d/d x0)
-    x0s = {id(x_a): torch.tanh(x_a @ proj).requires_grad_(True), id(x_j): torch.tanh(x_j @ proj).requires_grad_(True)}
+    x0s = {}
+    for _, xn, _, _, _ in specs:
+        x0s.setdefault(id(xn), torch.tanh(xn @ proj).requires_grad_(True))
     ref = []
     for head, xn, x_in, l, light in specs:
         mod = getattr(model, head)
-        rows = _light_rows(light, model.light_line.weight, l if l is not None else torch.empty(0), n)
+        rows = None if ll is None else _light_rows(light, ll.weight, l if l is not None else torch.empty(0), n)
         xl = x0s[id(xn)] if rows is None else x0s[id(xn)] * rows
         z = mod.mlp(_mlp_input(model.basis_mat(xl), x_in))
         ref.append(torch.tanh(z) if head == "renderModule_normal" else torch.sigmoid(z))
@@ -121,7 +121,28 @@ def test_multi_head_backward_matches_autograd(world):
     torch.autograd.backward(ref, G)
     for p, g in zip(params, got):
         assert torch.allclose(g, p.grad, rtol=2e-4, atol=2e-5), tuple(p.shape)
-    # one appearance scatter per point set, fed with the summed d loss / d x0 of the heads at those points
-    assert len(scattered) == 2
-    assert torch.allclose(scattered[0], x0s[id(x_a)].grad, rtol=2e-4, atol=2e-5)
-    assert torch.allclose(scattered[1], x0s[id(x_j)].grad, rtol=2e-4, atol=2e-5)
+    assert len(scattered) == len(x0s)
+    for sc, x0 in zip(scattered, x0s.values()):
+        assert torch.allclose(sc, x0.grad, rtol=2e-4, atol=2e-5)
+
+
+def test_multi_head_backward_matches_autograd(world):
+    model, proj, scattered = world
+    n = 300
+    x_a, x_j = torch.rand(n, 3) * 2 - 1, torch.rand(n, 3) * 2 - 1
+    vd = torch.nn.functional.normalize(torch.randn(n, 3), dim=-1)
+    li = torch.randint(0, 3, (n,), dtype=torch.int32)
+    specs = [("renderModule", x_a, vd, li, "index"), ("renderModule_brdf", x_a, x_a, None, "mean"),
+             ("renderModule_normal", x_a, x_a, None, "mean"), ("renderModule_brdf", x_j, x_j, None, "mean")]
+    _check_against_autograd(model, proj, scattered, specs, heads.fused_heads_multi(model, specs))
+
+
+def test_single_head_without_light_matches_autograd(world):
+    """heads.fused_head on a model without light_line, light "none": one head through the same stacked node."""
+    model, proj, scattered = world
+    del model.light_line
+    n = 300
+    x_a = torch.rand(n, 3) * 2 - 1
+    vd = torch.nn.functional.normalize(torch.randn(n, 3), dim=-1)
+    out = heads.fused_head(model, "renderModule", x_a, vd, None, light="none")
+    _check_against_autograd(model, proj, scattered, [("renderModule", x_a, vd, None, "none")], (out,))

@@ -6,8 +6,6 @@ grid with a symmetric box a swapped axis, scale or box would go unnoticed.
 The checks and tolerances are test_gpu_parity.py's: unit kernels 2e-5 / 5e-5 relative, maps 1e-4 relative, every
 parameter gradient 5e-4 of its max, sample lists and counts exact.  The oracle (bit-exact against this fixture on the
 CPU, test_oracle_shrunk_golden.py) supplies the references the fixture does not store."""
-import ctypes as C
-
 import pytest
 import torch
 
@@ -15,7 +13,7 @@ pytestmark = pytest.mark.gpu
 
 from oracle import tensoir_oracle as O                        # noqa: E402
 from helpers import oracle_field                             # noqa: E402
-from gpu_helpers import load_shrunk_state, model_from_fixture, renderer_args   # noqa: E402
+from gpu_helpers import app_mlp_list, load_shrunk_state, model_from_fixture, renderer_args   # noqa: E402
 from test_gpu_parity import DEV, TOL, _train_loss, close      # noqa: E402
 
 
@@ -48,7 +46,7 @@ def test_device_geometry_follows_every_axis(shr):
 
 
 def test_unit_kernels(shr):
-    from tensoir_b200 import _lib, ops
+    from tensoir_b200 import ops
     from tensoir_b200.device_field import mlp_struct
     fx, m = shr
     pts = fx["pts"].to(DEV)
@@ -63,23 +61,16 @@ def test_unit_kernels(shr):
     close(intr, fx["intr_feat"], 2e-5, "intr")
     close(m.compute_appfeature(xn, li), fx["app_feat"], 2e-5, "app")
     close(m.compute_intrinfeature(xn), fx["intrin_only"], 2e-5, "intrin")
-    # the three heads on both MLP kernels (wgmma and mma.sync), through the C ABI
-    lib = _lib.load()
-    f = ops.device_field(m).refresh(m)
+    # the three heads on the mma.sync kernel (tir_app_mlp_points_save), renderModule on the wgmma list kernel
+    # (tir_app_mlp, one sample per ray at weight 1)
     vd = fx["viewdirs"].to(DEV)
-    li32 = li.reshape(-1).to(torch.int32).contiguous()
-    for head, light, act, x_in, want in (("renderModule", "index", 0, vd, fx["mlp_rgb"]),
-                                         ("renderModule_brdf", "mean", 0, xn, fx["mlp_brdf"]),
-                                         ("renderModule_normal", "mean", 1, xn, fx["mlp_normal"])):
-        keep = []
-        mlp = mlp_struct(m, head, keep, light=light)
-        for kernel, fn in (("mma.sync", lib.tir_app_mlp_points_legacy), ("wgmma", lib.tir_app_mlp_points_wgmma)):
-            out = torch.full((xn.shape[0], mlp.out_dim), -7.0, device=DEV)
-            _lib.check(fn(C.byref(f), C.byref(mlp), _lib.dptr(xn.contiguous()), _lib.dptr(x_in.contiguous()),
-                          _lib.dptr(li32, torch.int32) if light == "index" else None, xn.shape[0], act,
-                          _lib.dptr(out), _lib.stream_ptr()), "mlp points")
-            torch.cuda.synchronize()
-            close(out, want, 5e-5, f"{head} {kernel}")
+    for head, light, x_in, want in (("renderModule", "index", vd, fx["mlp_rgb"]),
+                                    ("renderModule_brdf", "mean", xn, fx["mlp_brdf"]),
+                                    ("renderModule_normal", "mean", xn, fx["mlp_normal"])):
+        out = ops.app_mlp_points(m, xn, x_in, li if light == "index" else None, head=head, light=light)
+        close(out, want, 5e-5, f"{head} mma.sync")
+    keep = []
+    close(app_mlp_list(m, mlp_struct(m, "renderModule", keep), xn, vd, li), fx["mlp_rgb"], 5e-5, "renderModule wgmma")
     # derived-normal gradient, absolute vs its scale (as in test_gpu_parity.test_unit_kernels)
     from tensoir_b200.primary import _derived_normals
     from tensoir_b200 import vm_autograd as vm
