@@ -60,6 +60,9 @@ class StaticTrainStep:
         self.grow_at, self.headroom, self.lag = float(grow_at), float(headroom), max(1, int(lag))
         self.rays = torch.zeros(n_rays, 6, device=dev)
         self.light_idx = torch.zeros(n_rays, 1, dtype=torch.int32, device=dev)
+        # per-step loss target (the batch's rgb), staged by run(..., target) with the rays so that a redone step gets
+        # its own batch's target back; loss_fn reads it
+        self.target = torch.zeros(n_rays, 3, device=dev)
         n_dirs = model.envmap_h * model.envmap_w
         self.static = {"cap_valid": int(cap_valid or 256 * n_rays), "cap_app": int(cap_app or 16 * n_rays),
                        "sec_per_slot": 4,
@@ -195,16 +198,20 @@ class StaticTrainStep:
         return (id(m.alphaMask), tuple((p.data_ptr(), tuple(p.shape)) for p in vm))
 
     # ------------------------------------------------------------------------------------------------ replay
-    def _launch(self, rays, light_idx, slot):
+    def _launch(self, rays, light_idx, slot, target=None, seed=None):
         self.rays.copy_(rays, non_blocking=True)
         self.light_idx.copy_(light_idx.reshape(-1, 1), non_blocking=True)
+        if target is not None:
+            self.target.copy_(target, non_blocking=True)
+        if seed is not None:
+            torch.manual_seed(seed)
         self._stage_host_randoms(slot)
         self.graph.replay()
         slot["stats"][:4].copy_(self.static["stats"], non_blocking=True)
         slot["stats"][4:5].copy_(self.static["overflow_step"].reshape(1), non_blocking=True)
         ev = torch.cuda.Event()
         ev.record()
-        slot["event"], slot["batch"] = ev, (rays, light_idx)
+        slot["event"], slot["batch"] = ev, (rays, light_idx, target, seed)
         mark_parameters_updated()        # the replayed optimizer step is invisible to the host-side bookkeeping
         _lib.launch_count += self.launches_per_replay
 
@@ -262,17 +269,20 @@ class StaticTrainStep:
                 if o:
                     redo.append(s["batch"])
             self._recapture(grow)
-            for rays, li in redo:
+            for rays, li, target, seed in redo:
                 self.redone += 1
-                self._launch(rays, li, self._slots[0])
+                self._launch(rays, li, self._slots[0], target, seed)
                 self._settle_now(self._slots[0])
 
     def _settle_now(self, slot):
         torch.cuda.synchronize()
         self._settle(slot)
 
-    def run(self, rays, light_idx):
-        """One training step.  ``rays`` / ``light_idx`` may live on the host (pinned) or on the device."""
+    def run(self, rays, light_idx, target=None, seed=None):
+        """One training step.  ``rays`` / ``light_idx`` / ``target`` (copied into :attr:`target` for ``loss_fn``;
+        None leaves it as it is) may live on the host (pinned) or on the device; they must stay unchanged for
+        ``lag + 1`` further calls, since an overflowed step is redone from them.  With ``seed``, the step's host randoms
+        are drawn right after ``torch.manual_seed(seed)`` (a redo draws the same ones), whatever re-capture runs first."""
         if self.graph is None:
             raise RuntimeError("StaticTrainStep.run() before capture()")
         if self._model_signature() != self._captured_for:
@@ -281,7 +291,7 @@ class StaticTrainStep:
         slot = self._slots[self._step % len(self._slots)]
         self._settle(slot)                          # the step that used this slot `lag + 1` calls ago
         self._step += 1
-        self._launch(rays, light_idx, slot)
+        self._launch(rays, light_idx, slot, target, seed)
         return self.loss
 
     def reserve(self, factor=2.0):

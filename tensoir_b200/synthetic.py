@@ -293,3 +293,25 @@ class SyntheticViews:
             normals_white[hit] = normal[hit]
             item['normals_white'] = normals_white
         return item
+
+
+class SyntheticTrainViews(SyntheticViews):
+    """A training split of the lego box scene in the reference's train-dataset contract
+    (dataLoader/tensoIR_rotation_setting.py:48-55, :86-140): every pixel of every view flattened into ``all_rays``
+    [N,6], ``all_rgbs`` [N,3], ``all_masks`` [N,1] and ``all_light_idx`` [N,1] (long, all lights of a view in turn),
+    plus ``scene_bbox``, ``near_far`` and ``white_bg``."""
+
+    def __init__(self, poses: torch.Tensor, H: int, W: int, n_lights: int = 1, **kw):
+        super().__init__(poses, H, W, n_lights=n_lights, **kw)
+        self.split = 'train'
+        self.scene_bbox = torch.tensor([[-1.5, -1.5, -1.5], [1.5, 1.5, 1.5]])
+        rays, rgbs, masks, lights = [], [], [], []
+        for i in range(len(self)):
+            item = SyntheticViews.__getitem__(self, i)
+            for l in range(self.n_lights):
+                rays.append(item['rays'])
+                rgbs.append(item['rgbs'][l])
+                masks.append(item['rgbs_mask'])
+                lights.append(item['light_idx'][l].long())
+        self.all_rays, self.all_rgbs = torch.cat(rays), torch.cat(rgbs)
+        self.all_masks, self.all_light_idx = torch.cat(masks), torch.cat(lights)
