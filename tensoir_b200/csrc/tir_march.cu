@@ -5,6 +5,8 @@
 // alpha-mask > 0) are compacted into a per-warp shared-memory queue and the expensive gather runs on
 // full 32-lane batches; invalid samples have sigma = 0 => alpha = 0 => T factor (1 - 0 + 1e-10) == 1.0f
 // in fp32, so dropping them is exact (raw2alpha, tensorBase:21-28).
+#include <type_traits>
+
 #include "tir_device.cuh"
 
 using namespace tir;
@@ -13,7 +15,12 @@ namespace {
 
 constexpr int kWarpsPerBlock = 8;
 constexpr int kQueue = 64;
-constexpr int kBlocksPerSM = 2;
+// Resident CTAs per SM.  The dense VOL instance with a z table (the secondary march of the training step) has no factor
+// gather and fits in 80 registers, so it runs 3 CTAs (24 warps) per SM to hide the latency of its mask, volume and
+// queue loads; the other instances need more registers and run 2.
+template <int SAMPLING, bool DENSE, bool VOL>
+constexpr bool kThreeCtas = DENSE && VOL && SAMPLING == TIR_SAMPLE_TABLE;
+template <int SAMPLING, bool DENSE, bool VOL> constexpr int kBlocksPerSM = kThreeCtas<SAMPLING, DENSE, VOL> ? 3 : 2;
 
 // Work counter of the dense secondary march: the next surface point a CTA takes.  The last CTA of a launch to finish
 // puts it back to 0, so consecutive launches on a stream (and CUDA-graph replays) start from a zeroed counter without a
@@ -108,7 +115,8 @@ __device__ __forceinline__ float seg_scan_add(float v, bool head, int lane) {
 }
 
 template <int C, int SAMPLING, bool WITH_APP, bool DENSE, bool VOL>
-__global__ void __launch_bounds__(kWarpsPerBlock * 32, kBlocksPerSM) march_kernel(const MarchParams p) {
+__global__ void __launch_bounds__(kWarpsPerBlock * 32, kBlocksPerSM<SAMPLING, DENSE, VOL>)
+    march_kernel(const MarchParams p) {
   __shared__ QEntry queue[kWarpsPerBlock][kQueue];
   __shared__ uint32_t brick_bits[kBrickMaxWords];
   const int lane = threadIdx.x & 31;
@@ -126,7 +134,9 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, kBlocksPerSM) march_kerne
   const int N = p.cfg.n_samples;
   const float scale = f.distance_scale;
   const bool need_sums = (p.acc != nullptr) | (p.depth != nullptr);
-  unsigned long long c_mask = 0, c_density = 0, c_app = 0, c_rays = 0, c_over = 0;
+  // per-lane counts; 32 bits in the 3-CTA instance, which needs the registers (launch_instance bounds the counts)
+  using Count = typename std::conditional<kThreeCtas<SAMPLING, DENSE, VOL>, unsigned, unsigned long long>::type;
+  Count c_mask = 0, c_density = 0, c_app = 0, c_rays = 0, c_over = 0;
 
   // Valid samples of CONSECUTIVE rays share 32-lane gather batches (a ray rarely has a multiple of 32 valid samples;
   // flushing per ray left the 72-load gather ~40 % occupied).  The compositing scan is segmented by ray; the state of
@@ -186,8 +196,10 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, kBlocksPerSM) march_kerne
         if (app) {
           const unsigned slot = base + __popc(m & ((1u << lane) - 1u));
           if ((int64_t)slot < p.capacity) {
+            // re-read from the queue rather than kept in registers across the gather and the scans
+            const volatile QEntry& r = q[lane];
             TirAppSample sm;
-            sm.xn[0] = e.x; sm.xn[1] = e.y; sm.xn[2] = e.z; sm.weight = w; sm.ray = e.ray; sm.sample = e.s;
+            sm.xn[0] = r.x; sm.xn[1] = r.y; sm.xn[2] = r.z; sm.weight = w; sm.ray = r.ray; sm.sample = r.s;
             p.samples[slot] = sm;
             c_app += 1;
           } else {
@@ -375,15 +387,29 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, kBlocksPerSM) march_kerne
   }
   if (qn > 0) process(qn, -1);
 
-  c_mask = warp_sum_u64(c_mask); c_density = warp_sum_u64(c_density); c_app = warp_sum_u64(c_app);
-  c_rays = warp_sum_u64(c_rays); c_over = warp_sum_u64(c_over);
+  const unsigned long long t_mask = warp_sum_u64(c_mask), t_density = warp_sum_u64(c_density),
+                           t_app = warp_sum_u64(c_app), t_rays = warp_sum_u64(c_rays), t_over = warp_sum_u64(c_over);
   if (lane == 0 && p.counters) {
-    if (c_mask) atomicAdd(p.counters + TIR_CNT_MASK, c_mask);
-    if (c_density) atomicAdd(p.counters + TIR_CNT_DENSITY, c_density);
-    if (c_app) atomicAdd(p.counters + TIR_CNT_APP, c_app);
-    if (c_rays) atomicAdd(p.counters + TIR_CNT_RAYS, c_rays);
-    if (c_over) atomicAdd(p.counters + TIR_CNT_OVERFLOW, c_over);
+    if (t_mask) atomicAdd(p.counters + TIR_CNT_MASK, t_mask);
+    if (t_density) atomicAdd(p.counters + TIR_CNT_DENSITY, t_density);
+    if (t_app) atomicAdd(p.counters + TIR_CNT_APP, t_app);
+    if (t_rays) atomicAdd(p.counters + TIR_CNT_RAYS, t_rays);
+    if (t_over) atomicAdd(p.counters + TIR_CNT_OVERFLOW, t_over);
   }
+}
+
+template <int SAMPLING, bool WITH_APP, bool DENSE, bool VOL>
+int launch_instance(const MarchParams& p, cudaStream_t stream) {
+  // a lane's count grows by at most 2 per 32-sample chunk its warp walks: the 32-bit counts of the 3-CTA instance stay
+  // exact even if one warp walked every ray
+  if (kThreeCtas<SAMPLING, DENSE, VOL> && (uint64_t)p.n_rays * ((p.cfg.n_samples + 31) / 32) * 2 > 0xffffffffull)
+    return TIR_ERR_SHAPE;
+  // persistent: every resident CTA slot; grid-stride over rays, or (dense) one surface point per CTA at a time
+  int64_t blocks = DENSE ? p.n_pts : (p.n_rays + kWarpsPerBlock - 1) / kWarpsPerBlock;
+  const int64_t max_blocks = (int64_t)num_sms() * kBlocksPerSM<SAMPLING, DENSE, VOL>;
+  if (blocks > max_blocks) blocks = max_blocks;
+  march_kernel<16, SAMPLING, WITH_APP, DENSE, VOL><<<(int)blocks, kWarpsPerBlock * 32, 0, stream>>>(p);
+  return (int)cudaGetLastError();
 }
 
 template <bool WITH_APP, bool DENSE, bool VOL = false>
@@ -391,32 +417,29 @@ int launch_march(const MarchParams& p, cudaStream_t stream) {
   if (p.n_rays <= 0) return TIR_OK;
   if (p.f.dC != 16) return TIR_ERR_SHAPE;
   if (p.cfg.n_samples <= 0) return TIR_ERR_CONFIG;
-  // persistent: every resident CTA slot; grid-stride over rays, or (dense) one surface point per CTA at a time
-  int64_t blocks = DENSE ? p.n_pts : (p.n_rays + kWarpsPerBlock - 1) / kWarpsPerBlock;
-  const int64_t max_blocks = (int64_t)num_sms() * kBlocksPerSM;
-  if (blocks > max_blocks) blocks = max_blocks;
-  if (p.cfg.sampling == TIR_SAMPLE_STEP) {
-    march_kernel<16, TIR_SAMPLE_STEP, WITH_APP, DENSE, VOL><<<(int)blocks, kWarpsPerBlock * 32, 0, stream>>>(p);
-  } else if (p.cfg.sampling == TIR_SAMPLE_TABLE) {
+  if (p.cfg.sampling == TIR_SAMPLE_STEP) return launch_instance<TIR_SAMPLE_STEP, WITH_APP, DENSE, VOL>(p, stream);
+  if (p.cfg.sampling == TIR_SAMPLE_TABLE) {
     if (!p.cfg.z_table) return TIR_ERR_NULL;
-    march_kernel<16, TIR_SAMPLE_TABLE, WITH_APP, DENSE, VOL><<<(int)blocks, kWarpsPerBlock * 32, 0, stream>>>(p);
-  } else {
-    return TIR_ERR_CONFIG;
+    return launch_instance<TIR_SAMPLE_TABLE, WITH_APP, DENSE, VOL>(p, stream);
   }
-  return (int)cudaGetLastError();
+  return TIR_ERR_CONFIG;
 }
 
 // Density volume builder: D[x,y,z] = sum_k sum_c plane_k[c] * line_k[c] at the grid vertices of the box.  A CTA is a
 // 32 (x) x 8 (y) tile of vertices and walks kVolZ consecutive z.  The three factor rows that do not depend on z
-// (plane 0 at (x,y), line 1 at y, line 2 at x) stay in registers for the whole walk; per z a warp reads line 0 at z
-// (one row for the CTA), plane 2 at (y,z) (one row per warp) and plane 1 at (x,z) (coalesced along x).
+// (plane 0 at (x,y), line 1 at y, line 2 at x) stay in registers for the whole walk.  The rows that do (line 0 at z,
+// plane 1 at (x,z), plane 2 at (y,z)) are read from global memory once per CTA, all loads in flight together, into
+// shared memory, where every warp of the tile finds them: each plane-1 row serves the tile's 8 y.
 constexpr int kVolTileX = 32, kVolTileY = 8, kVolZ = 8;
+// plane-1 row stride in shared memory: 20 floats, so the 8 lanes of a quarter warp reading 16 B of 8 consecutive rows
+// hit 8 distinct 4-bank groups (a 16-float stride would put them on 2)
+constexpr int kVolRow = 20;
 
 __device__ __forceinline__ float dot16(const float (&a)[16], const float* b) {
   float s = 0.f;
 #pragma unroll
   for (int c = 0; c < 16; c += 4) {           // channel order, like density_feature
-    const float4 v = ldg4(b + c);
+    const float4 v = *reinterpret_cast<const float4*>(b + c);
     s = __fadd_rn(s, __fmul_rn(a[c + 0], v.x));
     s = __fadd_rn(s, __fmul_rn(a[c + 1], v.y));
     s = __fadd_rn(s, __fmul_rn(a[c + 2], v.z));
@@ -434,22 +457,50 @@ __device__ __forceinline__ void load16(float (&a)[16], const float* src) {
 }
 
 __global__ void __launch_bounds__(kVolTileX * kVolTileY) density_volume_kernel(const TirField f, TirDensityVolume v) {
-  const int xi = blockIdx.x * kVolTileX + threadIdx.x, yi = blockIdx.y * kVolTileY + threadIdx.y;
-  if (xi >= v.n[0] || yi >= v.n[1]) return;
+  __shared__ __align__(16) float s_p1[kVolZ][kVolTileX][kVolRow];
+  __shared__ __align__(16) float s_p2[kVolZ][kVolTileY][16];
+  __shared__ __align__(16) float s_l0[kVolZ][16];
   const int X = f.grid[0], Y = f.grid[1];
-  const int x = v.lo[0] + xi, y = v.lo[1] + yi;
+  const int xi0 = blockIdx.x * kVolTileX, yi0 = blockIdx.y * kVolTileY, zi0 = blockIdx.z * kVolZ;
+  const int tx = min(kVolTileX, v.n[0] - xi0), ty = min(kVolTileY, v.n[1] - yi0), tz = min(kVolZ, v.n[2] - zi0);
+  const int x0 = v.lo[0] + xi0, y0 = v.lo[1] + yi0, z0 = v.lo[2] + zi0;
+  const int tid = threadIdx.y * kVolTileX + threadIdx.x;
+  // stage the z-dependent rows of the tile, 16 B per load, consecutive threads on consecutive 16 B of a row
   // matMode {0,1},{0,2},{1,2}, vecMode {2,1,0}: plane k is [G[m1]][G[m0]][C], line k is [G[v]][C]
+  for (int i = tid; i < kVolZ * kVolTileX * 4; i += kVolTileX * kVolTileY) {
+    const int c = (i & 3) * 4, xl = (i >> 2) % kVolTileX, zl = (i >> 2) / kVolTileX;
+    if (xl < tx && zl < tz)
+      *reinterpret_cast<float4*>(&s_p1[zl][xl][c]) = ldg4(f.dplane[1] + ((size_t)(z0 + zl) * X + x0 + xl) * 16 + c);
+  }
+  for (int i = tid; i < kVolZ * kVolTileY * 4; i += kVolTileX * kVolTileY) {
+    const int c = (i & 3) * 4, yl = (i >> 2) % kVolTileY, zl = (i >> 2) / kVolTileY;
+    if (yl < ty && zl < tz)
+      *reinterpret_cast<float4*>(&s_p2[zl][yl][c]) = ldg4(f.dplane[2] + ((size_t)(z0 + zl) * Y + y0 + yl) * 16 + c);
+  }
+  if (tid < kVolZ * 4) {
+    const int c = (tid & 3) * 4, zl = tid >> 2;
+    if (zl < tz) *reinterpret_cast<float4*>(&s_l0[zl][c]) = ldg4(f.dline[0] + (size_t)(z0 + zl) * 16 + c);
+  }
+  const bool in_box = (int)threadIdx.x < tx && (int)threadIdx.y < ty;
+  const int x = x0 + threadIdx.x, y = y0 + threadIdx.y;
   float p0[16], l1[16], l2[16];
-  load16(p0, f.dplane[0] + ((size_t)y * X + x) * 16);
-  load16(l1, f.dline[1] + (size_t)y * 16);
-  load16(l2, f.dline[2] + (size_t)x * 16);
-  const int z_end = min(v.n[2], (int)(blockIdx.z + 1) * kVolZ);
-  for (int zi = blockIdx.z * kVolZ; zi < z_end; ++zi) {
-    const int z = v.lo[2] + zi;
-    const float s0 = dot16(p0, f.dline[0] + (size_t)z * 16);
-    const float s1 = dot16(l1, f.dplane[1] + ((size_t)z * X + x) * 16);
-    const float s2 = dot16(l2, f.dplane[2] + ((size_t)z * Y + y) * 16);
-    v.data[((size_t)zi * v.n[1] + yi) * v.n[0] + xi] = __fadd_rn(__fadd_rn(s0, s1), s2);
+  if (in_box) {
+    load16(p0, f.dplane[0] + ((size_t)y * X + x) * 16);
+    load16(l1, f.dline[1] + (size_t)y * 16);
+    load16(l2, f.dline[2] + (size_t)x * 16);
+  }
+  __syncthreads();
+  if (!in_box) return;
+  float* out = v.data + ((size_t)zi0 * v.n[1] + yi0 + threadIdx.y) * v.n[0] + xi0 + threadIdx.x;
+  const size_t z_stride = (size_t)v.n[1] * v.n[0];
+#pragma unroll
+  for (int zl = 0; zl < kVolZ; ++zl) {
+    if (zl < tz) {
+      const float s0 = dot16(p0, s_l0[zl]);
+      const float s1 = dot16(l1, s_p1[zl][threadIdx.x]);
+      const float s2 = dot16(l2, s_p2[zl][threadIdx.y]);
+      out[zl * z_stride] = __fadd_rn(__fadd_rn(s0, s1), s2);
+    }
   }
 }
 
