@@ -252,6 +252,7 @@ class SyntheticViews:
         self.white_bg = True
         self.lights_probes = None
         self.n_lights = int(n_lights)
+        self.light_num = self.n_lights           # the reference datasets' name for the light count
         self.cam_angle_x = cam_angle_x
         self.focal = 0.5 * W / math.tan(0.5 * cam_angle_x)
 

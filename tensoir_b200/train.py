@@ -25,11 +25,27 @@ iteration is one graph replay plus its input copies; nothing on the per-step pat
 
 ``graphed=False`` runs the same schedule with the eager ``Renderer_TensoIR_train`` and ``torch.optim.Adam``: it is the
 reference the GPU tests compare the graphed run against, not a user option.
+
+One loop serves the reference's four training scripts; ``variant`` (the names of ``evaluation._evaluate``) picks only
+the model's light kwargs, the evaluation function and the final evaluation block:
+
+* ``"full"``: train_tensoIR.py, and train_tensoIR_rotated_multi_lights.py, which is the same loop.
+* ``"general"``: train_tensoIR_general_multi_lights.py.  The model gets ``light_name_list``; evaluations go through
+  ``evaluation_iter_TensoIR_general_multi_lights``, whose per-view ``np.random.randint(light_num)`` draws come from the
+  numpy stream the sampler permutes with, between the same two sampler calls as in the reference; the final evaluation
+  runs once per light into ``imgs_test_all/{light_name}/``.
+* ``"simple"``: train_tensoIR_simple.py (NeRF-synthetic scenes): ``evaluation_iter_TensoIR_simple``, no MAE or albedo
+  metrics.
+
+:func:`render_test` is the scripts' ``--render_only 1 --render_test 1`` path on a checkpoint, and :func:`main` their
+``__main__`` block (mesh export, then rendering or training).
 """
 from __future__ import annotations
 
+import datetime
 import gc
 import os
+import random
 import shutil
 import sys
 import time
@@ -60,8 +76,29 @@ class TVLoss(torch.nn.Module):
         self.TVLoss_weight = TVLoss_weight
 
 
-def check_supported(args):
-    """Reject what the native trainer does not run, before any work is done."""
+VARIANTS = ("full", "general", "simple")
+
+
+def _reject_render_path(args):
+    if getattr(args, "render_path", 0):
+        raise ValueError("render_path: the reference scripts have no camera-path rendering (their render_path block is "
+                         "commented out); use --render_only 1 --render_test 1 to render the test views")
+
+
+def check_supported(args, variant="full", train_dataset=None):
+    """Reject what the native trainer does not run, before any work is done.  With ``train_dataset``, a general run's
+    ``light_name_list`` must name one light per light of the training set (its ``light_num``)."""
+    if variant not in VARIANTS:
+        raise ValueError(f"variant {variant!r}: expected one of {VARIANTS}")
+    _reject_render_path(args)
+    if variant == "general":
+        names = list(args.light_name_list or [])
+        if not names:
+            raise ValueError("the general multi-light trainer needs light_name_list (one name per training light)")
+        n = getattr(train_dataset, "light_num", None)
+        if train_dataset is not None and n != len(names):
+            raise ValueError(f"light_name_list {names} names {len(names)} lights; the training set has "
+                             f"light_num = {n}")
     if args.ndc_ray:
         raise ValueError("ndc_ray: the native trainer supports the synthetic (non-NDC) scenes only")
     if args.model_name != "TensorVMSplit" or args.shadingMode != "MLP_Fea":
@@ -110,15 +147,22 @@ class _Rays:
         return [(self.rays[i], self.li[i]) for i in ids]
 
 
-def _new_model(args, train_dataset, device):
+def _load_model(path, device):
+    """The checkpoint at ``path`` (:163-168); its kwargs carry the light_name_list of a general model."""
+    ckpt = torch.load(path, map_location=device, weights_only=False)
+    kwargs = ckpt['kwargs']
+    kwargs.update({'device': device})
+    model = TensorVMSplit(**kwargs)
+    model.load(ckpt)
+    return model
+
+
+def _new_model(args, train_dataset, device, variant="full"):
     if args.ckpt is not None:                                                                # :163-168
-        ckpt = torch.load(args.ckpt, map_location=device, weights_only=False)
-        kwargs = ckpt['kwargs']
-        kwargs.update({'device': device})
-        model = TensorVMSplit(**kwargs)
-        model.load(ckpt)
-        return model
+        return _load_model(args.ckpt, device)
     aabb = train_dataset.scene_bbox.to(device)
+    # the general script adds light_name_list (train_tensoIR_general_multi_lights.py:223)
+    lights = {"light_name_list": args.light_name_list} if variant == "general" else {}
     return TensorVMSplit(aabb, n_to_reso(args.N_voxel_init, aabb), device,                 # :170-192
                          density_n_comp=args.n_lamb_sigma, appearance_n_comp=args.n_lamb_sh,
                          app_dim=args.data_dim_color, near_far=train_dataset.near_far, shadingMode=args.shadingMode,
@@ -127,7 +171,7 @@ def _new_model(args, train_dataset, device):
                          fea_pe=args.fea_pe, featureC=args.featureC, step_ratio=args.step_ratio,
                          fea2denseAct=args.fea2denseAct, normals_kind=args.normals_kind,
                          light_rotation=args.light_rotation, light_kind=args.light_kind, dataset=train_dataset,
-                         numLgtSGs=args.numLgtSGs)
+                         numLgtSGs=args.numLgtSGs, **lights)
 
 
 def _loss(args, ret, target, model, w, relight, terms):
@@ -192,19 +236,61 @@ class _Timer:
         self.t[key] = self.t.get(key, 0.0) + seconds
 
 
-def reconstruction(args, train_dataset, test_dataset, logfolder, *, graphed=True, device=None, out=sys.stdout):
+# the evaluation each script calls (:350-353; general :388, simple :362)
+_EVAL = {"full": evaluation.evaluation_iter_TensoIR, "general": evaluation.evaluation_iter_TensoIR_general_multi_lights,
+         "simple": evaluation.evaluation_iter_TensoIR_simple}
+
+
+def _five(r):
+    """An evaluation's result as (psnr, psnr_brdf, mae, psnr_albedo_single, psnr_albedo_three); the simple
+    evaluation has no MAE or albedo metrics (None)."""
+    return tuple(r) + (None,) * (5 - len(r))
+
+
+def _metric_tags(variant, suffix, psnr, psnr_brdf, mae, pa1, pa3):
+    """The test scalars a script logs (:366-372 / :449-453; the simple script drops MAE and the albedo PSNRs)."""
+    tags = [('test/psnr_rgb', np.mean(psnr)), ('test/psnr_rgb_brdf', np.mean(psnr_brdf))]
+    if variant != "simple":
+        tags += [('test/mae', mae), ('test/psnr_albedo_single', pa1), ('test/psnr_albedo_three', pa3)]
+    return [(t + suffix, v) for t, v in tags]
+
+
+def _test_all(variant, test_dataset, model, args, savedir, device, white_bg=True):
+    """The final evaluation of every test view into ``savedir`` (:433-453), once per light into
+    ``{savedir}{light_name}/`` for the general model (general script :470-491) -> the 5-tuple of :func:`_five`.  For
+    the general model the two PSNRs are the means over lights of the per-light means, and MAE and the albedo PSNRs are
+    those of the last light, as the reference prints them."""
+    kw = dict(N_samples=-1, white_bg=white_bg, ndc_ray=False, device=device, test_all=True)
+    if variant != "general":
+        return _five(_EVAL[variant](test_dataset, model, args, Renderer_TensoIR_train, savedir, **kw))
+    psnr, psnr_brdf = [], []
+    for light, name in enumerate(model.light_name_list):
+        os.makedirs(f'{savedir}{name}', exist_ok=True)
+        p, pb, mae, pa1, pa3 = evaluation.evaluation_iter_TensoIR_general_multi_lights(
+            test_dataset, model, args, Renderer_TensoIR_train, f'{savedir}{name}/', light_idx_to_test=light, **kw)
+        psnr.append(np.mean(p))
+        psnr_brdf.append(np.mean(pb))
+    return np.mean(psnr), np.mean(psnr_brdf), mae, pa1, pa3
+
+
+def _device(args, device):
+    return torch.device(device or (f"cuda:{args.local_rank}" if torch.cuda.is_available() else "cpu"))
+
+
+def reconstruction(args, train_dataset, test_dataset, logfolder, *, variant="full", graphed=True, device=None,
+                   out=sys.stdout):
     """Train ``args`` (the reference's option namespace, opt.config_parser) on ``train_dataset`` and evaluate on
-    ``test_dataset`` (the reference's dataset contracts), writing into ``logfolder`` what train_tensoIR.py writes:
-    ``checkpoints/{expname}_{it}.th``, ``imgs_vis/``, ``{expname}.th``, ``imgs_test_all/`` (with ``render_test``) and
-    TensorBoard scalars when tensorboard is importable.
+    ``test_dataset`` (the reference's dataset contracts), writing into ``logfolder`` what the ``variant``'s script
+    writes: ``checkpoints/{expname}_{it}.th``, ``imgs_vis/``, ``{expname}.th``, ``imgs_test_all/`` (with
+    ``render_test``; one subfolder per light for ``general``) and TensorBoard scalars when tensorboard is importable.
 
     Returns a dict: ``losses`` [n_iters, len(TERMS)] (float32, read from the device ring), ``events`` (the grid, save
     and evaluation calls, in order, as ``(iteration, name, ...)``), ``redone`` / ``recaptures`` of the captured steps,
     ``psnr_test`` of the final evaluation and ``times`` (seconds per phase, per event kind, evaluation)."""
-    check_supported(args)
+    check_supported(args, variant, train_dataset)
     if not train_dataset.white_bg:
         raise ValueError("the training step renders over a white background; this dataset has white_bg = False")
-    dev = torch.device(device or (f"cuda:{args.local_rank}" if torch.cuda.is_available() else "cpu"))
+    dev = _device(args, device)
     if dev.type != "cuda":
         raise RuntimeError("the native trainer needs a CUDA device")
     os.makedirs(f'{logfolder}/imgs_vis', exist_ok=True)
@@ -213,7 +299,7 @@ def reconstruction(args, train_dataset, test_dataset, logfolder, *, graphed=True
     if getattr(args, "config", None):
         shutil.copy(args.config, logfolder)
 
-    model = _new_model(args, train_dataset, dev)
+    model = _new_model(args, train_dataset, dev, variant)
     events = []
     timer = _Timer()
     sched = TrainSchedule(args, train_dataset.scene_bbox.to(dev),
@@ -345,15 +431,15 @@ def reconstruction(args, train_dataset, test_dataset, logfolder, *, graphed=True
             if st is not None:
                 st.flush()
                 st.release()
-            psnr_test, psnr_brdf_test, mae, pa1, pa3 = evaluation.evaluation_iter_TensoIR(
+            # the general evaluation draws one light per view from numpy's global stream, after this iteration's
+            # sampler call and before the next one's, as in the reference
+            psnr_test, psnr_brdf_test, mae, pa1, pa3 = _five(_EVAL[variant](
                 test_dataset, model, args, Renderer_TensoIR_train, f'{logfolder}/imgs_vis/', prtx=f'{it:06d}_',
                 N_samples=w.n_samples, white_bg=True, ndc_ray=False, compute_extra_metrics=False,
-                logger=writer, step=it, device=dev)
+                logger=writer, step=it, device=dev))
             events.append((it, "evaluation", "imgs_vis", f'{it:06d}_', int(w.n_samples), False, False))
             if writer is not None:
-                for tag, v in (('test/psnr_rgb', np.mean(psnr_test)), ('test/psnr_rgb_brdf', np.mean(psnr_brdf_test)),
-                               ('test/mae', mae), ('test/psnr_albedo_single', pa1),
-                               ('test/psnr_albedo_three', pa3)):
+                for tag, v in _metric_tags(variant, '', psnr_test, psnr_brdf_test, mae, pa1, pa3):
                     writer.add_scalar(tag, v, global_step=it)
             if st is not None and not end.grid:
                 st.capture(warmup=1)             # the eager forwards may have re-sized buffers the graph points into
@@ -406,22 +492,85 @@ def reconstruction(args, train_dataset, test_dataset, logfolder, *, graphed=True
     if args.render_test:                                                                     # :433-453
         t0 = sync_time()
         os.makedirs(f'{logfolder}/imgs_test_all', exist_ok=True)
-        psnr_test, psnr_brdf_test, mae, pa1, pa3 = evaluation.evaluation_iter_TensoIR(
-            test_dataset, model, args, Renderer_TensoIR_train, f'{logfolder}/imgs_test_all/', N_samples=-1,
-            white_bg=True, ndc_ray=False, device=dev, test_all=True)
+        psnr_test, psnr_brdf_test, mae, pa1, pa3 = _test_all(variant, test_dataset, model, args,
+                                                             f'{logfolder}/imgs_test_all/', dev)
         events.append((args.n_iters - 1, "evaluation", "imgs_test_all", '', -1, True, True))
         res["psnr_test"] = float(np.mean(psnr_test))
         if writer is not None:
-            for tag, v in (('test/psnr_rgb_all', np.mean(psnr_test)),
-                           ('test/psnr_rgb_brdf_all', np.mean(psnr_brdf_test)), ('test/mae_all', mae),
-                           ('test/psnr_albedo_single_all', pa1), ('test/psnr_albedo_three_all', pa3)):
+            for tag, v in _metric_tags(variant, '_all', psnr_test, psnr_brdf_test, mae, pa1, pa3):
                 writer.add_scalar(tag, v, global_step=args.n_iters - 1)
+        mae_part = '' if variant == "simple" else f', MAE: {mae}'
         out.write(f'======> {args.expname} test all: nvs psnr: {np.mean(psnr_test)}, nvs with brdf psnr: '
-                  f'{np.mean(psnr_brdf_test)}, MAE: {mae}  <========================\n')
+                  f'{np.mean(psnr_brdf_test)}{mae_part}  <========================\n')
         timer.add("final_evaluation", sync_time() - t0)
     if writer is not None:
         writer.close()
     res["times"] = timer.t
+    return res
+
+
+def render_test(args, test_dataset, logfolder, *, variant, device=None):
+    """render_test(args) of the ``variant``'s script (train_tensoIR.py:65-106, general :71-127, simple :66-103): the
+    checkpoint ``args.ckpt`` evaluated on every test view into ``{logfolder}/imgs_test_all/`` (one subfolder per light
+    for ``general``, the lights taken from the checkpoint), with the script's printed lines.  The scripts'
+    ``logfolder`` is ``{basedir}/test_{expname}-{timestamp}`` (:84).  Returns the 5-tuple of :func:`_five`, or None
+    after the reference's message when the checkpoint does not exist (nothing is written then)."""
+    if variant not in VARIANTS:
+        raise ValueError(f"variant {variant!r}: expected one of {VARIANTS}")
+    if not args.ckpt or not os.path.exists(args.ckpt):
+        print('the ckpt path does not exists!!')
+        return None
+    dev = _device(args, device)
+    model = _load_model(args.ckpt, dev)
+    r = _test_all(variant, test_dataset, model, args, f'{logfolder}/imgs_test_all/', dev,
+                  white_bg=test_dataset.white_bg)
+    print(f'PSNRs_test: {r[0]}')
+    print(f'PSNRs_rgb_brdf_test: {r[1]}')
+    if variant != "simple":                  # the general script prints the last light's (:129-131)
+        print(f'MAE_test: {r[2]}')
+        print(f'PSNR_albedo_single: {r[3]}')
+        print(f'PSNR_albedo_three: {r[4]}')
+    return r
+
+
+@torch.no_grad()
+def export_mesh(args, device=None):
+    """export_mesh(args) of the reference's scripts (train_tensoIR.py:52-61): the mesh of ``args.ckpt`` written to
+    ``{ckpt[:-3]}.ply`` by mesh.export_mesh.  Returns the path."""
+    from . import mesh
+    path = f'{args.ckpt[:-3]}.ply'
+    mesh.export_mesh(_load_model(args.ckpt, _device(args, device)), path)
+    return path
+
+
+def main(args, variant, datasets, render_dataset, *, device=None):
+    """The ``__main__`` block of the ``variant``'s script (train_tensoIR.py:464-481): the reference's seeds, then with
+    ``--export_mesh`` the mesh of ``--ckpt`` first, then :func:`render_test` when ``render_only`` and ``render_test``
+    are set and :func:`reconstruction` otherwise.  ``datasets()`` returns the (train, test) datasets of the script's
+    ``reconstruction``, ``render_dataset()`` the test set of its ``render_test``; each entry script builds them with its
+    reference script's constructor arguments.  Returns what render_test or reconstruction returns.  A render-only run
+    takes the model, and a general model's lights, from the checkpoint, so only a training run is checked against
+    :func:`check_supported`; ``render_path`` is rejected in both."""
+    rendering = bool(args.render_only and args.render_test)
+    if rendering:
+        _reject_render_path(args)
+    else:
+        check_supported(args, variant)
+    torch.set_default_dtype(torch.float32)
+    torch.manual_seed(SEED)
+    torch.cuda.manual_seed_all(SEED)
+    np.random.seed(SEED)
+    random.seed(SEED)
+    if args.export_mesh:
+        export_mesh(args, device)
+    stamp = datetime.datetime.now().strftime("-%Y%m%d-%H%M%S")
+    if rendering:
+        return render_test(args, render_dataset(), f'{args.basedir}/test_{args.expname}{stamp}', variant=variant,
+                           device=device)
+    train_dataset, test_dataset = datasets()
+    logfolder = f'{args.basedir}/{args.expname}' + (stamp if args.add_timestamp else '')
+    res = reconstruction(args, train_dataset, test_dataset, logfolder, variant=variant, device=device)
+    print(f"steps redone after a list overflow: {res['redone']}, re-captures: {res['recaptures']}")
     return res
 
 
