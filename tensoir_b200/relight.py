@@ -24,6 +24,15 @@ def read_hdr(path):
     return cv2.cvtColor(bgr, cv2.COLOR_BGR2RGB)
 
 
+def write_hdr(path, rgb):
+    """Write float [H,W,3] RGB radiance as a Radiance .hdr (RGBE, cv2) that read_hdr reads back to within RGBE precision:
+    each channel to one mantissa step, 2^-8 of the power of two above the pixel's largest channel."""
+    import cv2
+    bgr = np.ascontiguousarray(np.asarray(rgb, dtype=np.float32)[..., ::-1])
+    if not cv2.imwrite(path, bgr):
+        raise OSError(f"could not write {path}")
+
+
 class Environment_Light:
     """Same tables as the reference class (hdr_rgbs / hdr_pdf_sample / hdr_pdf_return / hdr_dir per light name);
     ``hdr_path`` may be a directory of .hdr files (reference behaviour) or a dict {name: [H,W,3] array}."""

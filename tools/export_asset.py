@@ -1,0 +1,49 @@
+"""Export a relightable asset of a checkpoint with the command line of tools/export_mesh.py (opt.config_parser, the
+same seeds, the checkpoint loaded with tensoir_b200.relighting._load_model): ``{ckpt[:-3]}_asset.ply`` holds the mesh
+of tools/export_mesh.py with per-vertex albedo, roughness and predicted normal, and ``{ckpt[:-3]}_asset_envmap_{k}.hdr``
+the radiance of light k (tensoir_b200.mesh.export_asset, level 0.005).  A general multi-light checkpoint
+(``light_name_list``) gets no .hdr files: its SG lights (lgtSGs_list) are not in the state_dict, so the checkpoint does
+not hold them and the loaded model's lights are their random initialisation; the tool says so.  Run it with a TensoIR
+checkout on PYTHONPATH (for opt):
+
+    PYTHONPATH=<TensoIR checkout>:. python tools/export_asset.py --config <config> --ckpt <ckpt>
+"""
+import os
+import sys
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if ROOT not in sys.path:
+    sys.path.append(ROOT)
+
+
+@torch.no_grad()
+def main(args):
+    """export_asset on ``args.ckpt``, on ``cuda:{args.local_rank}`` (device 0 when args has no local_rank); returns the
+    PLY path written (None without a checkpoint)."""
+    from tensoir_b200.mesh import export_asset
+    from tensoir_b200.relighting import _load_model
+    tensoIR = _load_model(args, torch.device(f"cuda:{getattr(args, 'local_rank', 0)}"))
+    if tensoIR is None:
+        return None
+    path = f'{args.ckpt[:-3]}_asset.ply'
+    learned_lights = not tensoIR.general_lights
+    export_asset(tensoIR, path, level=0.005, envmaps=learned_lights)
+    if not learned_lights:
+        print(f"{args.ckpt} is a general multi-light checkpoint: its lights (lgtSGs_list) are not saved in the "
+              "checkpoint, so no environment map is written")
+    return path
+
+
+if __name__ == "__main__":
+    from opt import config_parser
+
+    args = config_parser()
+    print(args)
+    torch.set_default_dtype(torch.float32)
+    torch.manual_seed(20211202)
+    torch.cuda.manual_seed_all(20211202)
+    np.random.seed(20211202)
+    main(args)

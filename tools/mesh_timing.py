@@ -1,6 +1,6 @@
 """Time the native mesh export on the 300^3 synthetic lego scene and print one JSON line.
 
-    python tools/mesh_timing.py [--grid 300] [--reps 20] [--host]
+    python tools/mesh_timing.py [--grid 300] [--reps 20] [--host] [--asset]
 
 Reports getDenseAlpha, the marching-cubes calls (tir_marching_cubes_count + _emit, CUDA events over repeated
 launches after warm-up, outputs preallocated: the calls are issued back to back, so host launch overhead can show in
@@ -8,8 +8,11 @@ these figures and they are an upper bound on the kernels' time), the device time
 (torch.profiler, same launches), the device-to-host copy of the PLY body, the PLY write, V and F, the
 achieved read bandwidth against the volume's X*Y*Z*4 bytes, and the card name and power limit read in the same run.
 --host also times the host build of the same C ABI (tests/host_mesh.cpp, g++ -O2, one thread) on the same volume: our
-CPU build, not the reference (whose skimage path is not measured here).  Compiled artefacts go to a temporary
-directory.
+CPU build, not the reference (whose skimage path is not measured here).  --asset also times the steps of
+mesh.export_asset on the same model, three runs after a warm-up, each step synchronised, wall clock, with each run's
+total: the surface (getDenseAlpha and the two marching-cubes calls), the derived normals at the vertices, the probe
+forward, the record packing with its device-to-host copy, the PLY write, the environment maps with their .hdr writes;
+plus V and the unprobed count.  Compiled artefacts and written files go to a temporary directory.
 """
 import argparse
 import ctypes as C
@@ -65,11 +68,54 @@ def _kernel_times(fn, reps):
     return {k: round(v, 4) for k, v in out.items()}
 
 
+def _wall(fn):
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    out = fn()
+    torch.cuda.synchronize()
+    return out, round((time.perf_counter() - t0) * 1e3, 3)
+
+
+def _asset_timing(model, tmp, runs=3):
+    """mesh.export_asset's steps in its order, as it runs them (the PLY written without fsync), after one warm-up run:
+    per timed run the wall time of each step (synchronised before and after) and of the whole run, so that the steps of
+    a run add up to its total"""
+    from tensoir_b200 import mesh
+    from tensoir_b200.relight import write_hdr
+    path = os.path.join(tmp, "lego_asset.ply")
+
+    def write():
+        with open(path, "wb") as f:
+            f.write(data)
+
+    def envmaps():
+        for q, rgb in zip(mesh.envmap_paths(path, model.light_num), mesh.light_envmaps(model).cpu().numpy()):
+            write_hdr(q, rgb)
+    out = []
+    for _ in range(runs + 1):
+        t = {}
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        (pts, faces, v), t["surface_ms"] = _wall(lambda: mesh.asset_surface(model))
+        n, t["normals_ms"] = _wall(lambda: mesh.vertex_normals(model, v))
+        p, t["probe_forward_ms"] = _wall(lambda: mesh.probe(model, v, n))
+        data, t["pack_and_d2h_ms"] = _wall(lambda: mesh.asset_ply_bytes(pts, faces, p["normal"], p["albedo"],
+                                                                      p["roughness"], p["probed"]))
+        _, t["ply_write_ms"] = _wall(write)
+        _, t["envmaps_ms"] = _wall(envmaps)
+        t["total_ms"] = round((time.perf_counter() - t0) * 1e3, 3)
+        out.append(t)
+    return dict(runs=out[1:], V=int(pts.shape[0]), rays=int(mesh.has_normal(n).sum()),
+                unprobed=int(pts.shape[0] - p["probed"].sum()), asset_ply_bytes=len(data),
+                probe_offset=mesh.probe_offset(model))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--grid", type=int, default=300)
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--host", action="store_true")
+    ap.add_argument("--asset", action="store_true")
     a = ap.parse_args()
     from tensoir_b200 import _lib, mesh
     from tensoir_b200.synthetic import make_lego_model
@@ -135,6 +181,7 @@ def main():
             hv, hf = host_marching_cubes(hl, v_np, level, sp)
             host_ms = (time.perf_counter() - t0) * 1e3
             assert torch.equal(torch.from_numpy(hv), verts.cpu()) and torch.equal(torch.from_numpy(hf), faces.cpu())
+        asset = _asset_timing(model, tmp) if a.asset else None
     name, power = _card()
     vol_bytes = X * Y * Z * 4
     print(json.dumps(dict(
@@ -144,7 +191,7 @@ def main():
         ply_bytes=len(body_dev), volume_bytes=vol_bytes,
         mc_volume_read_GBps=round(vol_bytes / (t_both * 1e-3) / 1e9, 1),
         mc_kernels_ms=kernels, mc_kernels_total_ms=round(sum(kernels.values()), 4),
-        host_build_ms=None if host_ms is None else round(host_ms, 1))))
+        host_build_ms=None if host_ms is None else round(host_ms, 1), asset=asset)))
 
 
 if __name__ == "__main__":
