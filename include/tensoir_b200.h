@@ -596,6 +596,42 @@ int tir_relight_shade(const TirEnvMap* envs, int32_t n_lights, const float* rays
                       int32_t vis_kind, float* with_bg, float* without_bg, int64_t out_rows, int64_t row0,
                       void* stream);
 
+/* ---- material editing: the BRDF parameters of n surface points, edited by a table of rules, for tir_relight_shade
+ * (or any other consumer) ----------------------------------------------------------------------------------------------
+ * The point of row i is points[i] when `points` is given, else rays[i].o + depth[i] * rays[i].d rounded as
+ * tir_relight_sample rounds it (the same bits as the visibility list's origin).  a0 = albedo[i] * scale (one fp32
+ * multiply per channel) is the unedited scaled albedo.
+ *   Rows with acc[i] > acc_threshold are edited: the rules are visited in order; rule k selects the row when the point
+ *   lies inside its box (box_lo <= p <= box_hi on every axis, when TIR_EDIT_BOX) and max_c |a0[c] - key[c]| <= key_tol
+ *   (when TIR_EDIT_KEY); a rule with neither flag selects every row.  A selecting rule applies its albedo, roughness and
+ *   fresnel ops to the running values (SET: the rule's value, MUL: value * rule's value, fp32), each op followed by a
+ *   clamp of the value it wrote: albedo and fresnel to [0, 1], roughness to [TIR_EDIT_ROUGH_MIN, TIR_EDIT_ROUGH_MAX]
+ *   (the model's valid_brdf * 0.9 + 0.09 range); the roughness value applies to every channel of a [n,3] roughness.
+ *   Selection always tests the unedited a0.  sel[i] gets bit k when rule k selected the row.
+ *   Every other row is passed through: albedo_out = a0, roughness and fresnel copied, sel = 0.
+ * Outputs are out of place: albedo_out [n,3], rough_out [n,rough_stride], fresnel_out [n,3], sel [n] int32.  Since
+ * albedo_out already holds the scale, pass rescale (1,1,1) to tir_relight_shade: an edit table without rules then
+ * shades to the same bits as the unedited call with rescale = scale.  One thread per row, no atomics: reruns are
+ * bit-identical.  TIR_ERR_SHAPE for n < 0, more than TIR_EDIT_MAX_RULES rules or a stride other than 1 or 3;
+ * TIR_ERR_CONFIG for an unknown op or flag. */
+#define TIR_EDIT_MAX_RULES 16
+#define TIR_EDIT_ROUGH_MIN 0.09f
+#define TIR_EDIT_ROUGH_MAX 0.99f
+enum { TIR_EDIT_NONE = 0, TIR_EDIT_SET = 1, TIR_EDIT_MUL = 2 };
+enum { TIR_EDIT_BOX = 1, TIR_EDIT_KEY = 2 };
+typedef struct TirEditRule {
+  int32_t flags;                                  /* TIR_EDIT_BOX | TIR_EDIT_KEY */
+  int32_t albedo_op, rough_op, fresnel_op;        /* TIR_EDIT_NONE / SET / MUL */
+  float box_lo[3], box_hi[3];
+  float key[3], key_tol;
+  float albedo[3], rough, fresnel[3];
+} TirEditRule;
+int tir_material_edit(const TirEditRule* rules /* host array [n_rules] */, int32_t n_rules, const float* rays,
+                      const float* depth, const float* points /* [n,3] or NULL: use rays and depth */,
+                      const float* albedo, const float* rough, int32_t rough_stride, const float* fresnel,
+                      const float* acc, int64_t n, float acc_threshold, const float* scale /* [3] */,
+                      float* albedo_out, float* rough_out, float* fresnel_out, int32_t* sel, void* stream);
+
 /* ---- mesh export: marching cubes over a dense volume (utils.py:165-225, skimage.measure.marching_cubes on
  * TensorBase.getDenseAlpha(), tensorBase_rotated_lights.py:737-753) ---------------------------------------------------
  * volume [X,Y,Z] fp32 C-contiguous, X, Y, Z >= 2 and X*Y*Z <= INT32_MAX (TIR_ERR_SHAPE otherwise).  A point is inside

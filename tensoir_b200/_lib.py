@@ -126,6 +126,18 @@ class TirEnvMap(C.Structure):
 
 RELIGHT_MAX_LIGHTS = 16   # TIR_RELIGHT_MAX_LIGHTS
 
+
+# ---- material editing (csrc/tir_edit.cu) -------------------------------------------------------------------------------
+class TirEditRule(C.Structure):
+    _fields_ = [("flags", C.c_int32), ("albedo_op", C.c_int32), ("rough_op", C.c_int32), ("fresnel_op", C.c_int32),
+                ("box_lo", C.c_float * 3), ("box_hi", C.c_float * 3), ("key", C.c_float * 3), ("key_tol", C.c_float),
+                ("albedo", C.c_float * 3), ("rough", C.c_float), ("fresnel", C.c_float * 3)]
+
+
+EDIT_MAX_RULES = 16       # TIR_EDIT_MAX_RULES
+EDIT_NONE, EDIT_SET, EDIT_MUL = 0, 1, 2
+EDIT_BOX, EDIT_KEY = 1, 2
+
 EXPORTS = {
     "tir_abi_version": (C.c_int, []),
     "tir_pack_channels_last": (C.c_int, [f32p, f32p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
@@ -225,6 +237,8 @@ EXPORTS = {
     "tir_relight_shade": (C.c_int, [C.POINTER(TirEnvMap), C.c_int32, f32p, f32p, f32p, f32p, C.c_int32, f32p, f32p,
                                     C.c_int64, C.c_int32, C.c_float, f32p, C.c_void_p, C.c_void_p, f32p, C.c_int32,
                                     f32p, f32p, C.c_int64, C.c_int64, C.c_void_p]),
+    "tir_material_edit": (C.c_int, [C.POINTER(TirEditRule), C.c_int32, f32p, f32p, f32p, f32p, f32p, C.c_int32, f32p,
+                                    f32p, C.c_int64, C.c_float, f32p, f32p, f32p, f32p, C.c_void_p, C.c_void_p]),
     "tir_marching_cubes_work_size": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int64)]),
     "tir_marching_cubes_count": (C.c_int, [f32p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_int64,
                                            C.c_void_p, C.c_void_p]),
@@ -246,7 +260,7 @@ KERNELS_PER_CALL = {"tir_pack_channels_last": 1, "tir_unpack_channels_last_add":
                     "tir_primary_backward": 9, "tir_primary_radiance": 2, "tir_primary_radiance_backward": 6,
                     "tir_composite_bwd": 1, "tir_tail_fwd": 1, "tir_tail_bwd": 1, "tir_epilogue_fwd": 1,
                     "tir_epilogue_bwd": 1, "tir_eval_view": 3, "tir_relight_sample": 1, "tir_relight_shade": 1,
-                    "tir_marching_cubes_count": 7, "tir_marching_cubes_emit": 2}
+                    "tir_material_edit": 1, "tir_marching_cubes_count": 7, "tir_marching_cubes_emit": 2}
 launch_count = 0
 
 _lib = None

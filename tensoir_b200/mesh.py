@@ -316,17 +316,40 @@ def light_envmaps(tensoIR):
     return rgbs.detach().float().clamp(min=0).reshape(tensoIR.light_num, H, W, 3)
 
 
+def _check_asset_edits(edits):
+    if any(e.fresnel_set is not None or e.fresnel_mul is not None for e in edits):
+        raise ValueError("the asset has no fresnel column: fresnel edits cannot be exported")
+
+
+def edit_vertices(p, v, edits):
+    """The probe outputs ``p`` (``probe``) at field positions ``v`` with the material rules ``edits`` (a list of
+    tensoir_b200.editing.MaterialEdit) applied by tir_material_edit: scale 1, only probed vertices edited.
+    -> (albedo [V,3], roughness [V]).  Raises ValueError for a fresnel op: the asset has no fresnel column."""
+    from .editing import edit_materials
+    _check_asset_edits(edits)
+    V = v.shape[0]
+    maps = (None, None, p["albedo"], p["roughness"].reshape(V, 1), torch.zeros(V, 3, device=v.device),
+            p["probed"].float())
+    albedo, rough, _, _ = edit_materials(maps, edits, 1.0, 0.5, points=v)
+    return albedo, rough[:, 0]
+
+
 @torch.no_grad()
-def export_asset(tensoIR, ply_path, level=0.005, envmaps=True):
+def export_asset(tensoIR, ply_path, level=0.005, envmaps=True, edits=None):
     """A relightable asset of the model: ``ply_path`` holds export_mesh's geometry (byte-identical x y z and faces) with
     the probed albedo, roughness and predicted normal per vertex (``probe``), and, with ``envmaps``,
     ``{ply stem}_envmap_{k}.hdr`` the radiance of light k.  Pass envmaps=False when the model's lights were not
     learned, as for a general multi-light model loaded from a checkpoint (its lgtSGs_list is not in the state_dict).
-    Nothing on the model changes.  Returns the number of unprobed vertices."""
+    With ``edits`` (a list of tensoir_b200.editing.MaterialEdit without fresnel ops) the albedo, colour and roughness
+    columns hold the edited materials of the probed vertices (``edit_vertices``).  Nothing on the model changes.
+    Returns the number of unprobed vertices."""
     from .relight import write_hdr
+    if edits is not None:
+        _check_asset_edits(edits)
     pts, faces, v = asset_surface(tensoIR, level)
     p = probe(tensoIR, v, vertex_normals(tensoIR, v))
-    data = asset_ply_bytes(pts, faces, p["normal"], p["albedo"], p["roughness"], p["probed"])
+    albedo, rough = (p["albedo"], p["roughness"]) if edits is None else edit_vertices(p, v, edits)
+    data = asset_ply_bytes(pts, faces, p["normal"], albedo, rough, p["probed"])
     unprobed = int(pts.shape[0] - int(p["probed"].sum()))
     print(f"saving asset to {ply_path}: {pts.shape[0]} vertices, {faces.shape[0]} faces, {unprobed} unprobed")
     with open(ply_path, "wb") as f:

@@ -57,6 +57,21 @@ def env_tables(envir_light, light_names):
     return arr, keep
 
 
+def chunk_inputs(rays, maps):
+    """rays and maps = (depth, normal, albedo, roughness, fresnel, acc) of a chunk as the relighting kernels take them:
+    contiguous fp32, depth and acc [n], roughness [n, 1] or [n, 3]."""
+    depth, normal, albedo, rough, fresnel, acc = maps
+    f32 = lambda t: t.detach().float().contiguous()  # noqa: E731
+    rays, depth, normal, albedo, fresnel, acc = (f32(t) for t in (rays, depth.reshape(-1), normal, albedo, fresnel,
+                                                                   acc.reshape(-1)))
+    return rays, (depth, normal, albedo, f32(rough).reshape(rays.shape[0], -1), fresnel, acc)
+
+
+def env_group(envs, g):
+    """The TirEnvMap array ``envs`` from entry g on: the first map of a group of up to RELIGHT_MAX_LIGHTS."""
+    return C.cast(C.byref(envs, g * C.sizeof(_lib.TirEnvMap)), C.POINTER(_lib.TirEnvMap))
+
+
 @torch.no_grad()
 def relight_chunk_fused(tensoIR, envir_light, light_names, rays, maps, rescale_value, u, num_samples=NUM_SAMPLES,
                         acc_mask_threshold=0.5, vis_equation='nerv', out=None, row0=0, tables=None):
@@ -67,14 +82,9 @@ def relight_chunk_fused(tensoIR, envir_light, light_names, rays, maps, rescale_v
     out[:, row0:row0+n] and views of them are returned."""
     if vis_equation not in ('nerv', 'nerfactor'):
         raise ValueError(vis_equation)
-    lib = _lib.load()
-    depth, normal, albedo, rough, fresnel, acc = maps
     dev = rays.device
     L, n, S = len(light_names), int(rays.shape[0]), int(num_samples)
-    f32 = lambda t: t.detach().float().contiguous()  # noqa: E731
-    rays, depth, normal, albedo, fresnel, acc = (f32(t) for t in (rays, depth.reshape(-1), normal, albedo, fresnel,
-                                                                   acc.reshape(-1)))
-    rough = f32(rough).reshape(n, -1)
+    rays, (depth, normal, albedo, rough, fresnel, acc) = chunk_inputs(rays, maps)
     if tuple(u.shape) != (L, n, S) or u.dtype != torch.float64:
         raise ValueError(f"u must be float64 [{L}, {n}, {S}], got {u.dtype} {tuple(u.shape)}")
     u = u.to(dev).contiguous()
@@ -88,12 +98,27 @@ def relight_chunk_fused(tensoIR, envir_light, light_names, rays, maps, rescale_v
     G = _lib.RELIGHT_MAX_LIGHTS
     if L > G:                  # the kernels take up to TIR_RELIGHT_MAX_LIGHTS maps per call: groups of maps
         for g in range(0, L, G):
-            sub = (C.cast(C.byref(envs, g * C.sizeof(_lib.TirEnvMap)), C.POINTER(_lib.TirEnvMap)), keep)
+            sub = (env_group(envs, g), keep)
             relight_chunk_fused(tensoIR, envir_light, light_names[g:g + G], rays, maps, rescale_value, u[g:g + G],
                                 num_samples, acc_mask_threshold, vis_equation, out=(with_bg[g:g + G],
                                                                                     without_bg[g:g + G]),
                                 row0=row0, tables=sub)
         return with_bg[:, row0:row0 + n], without_bg[:, row0:row0 + n]
+    bins, pos, vis = relight_visibility(tensoIR, envs, L, rays, depth, normal, acc, u, S, acc_mask_threshold,
+                                        vis_equation)
+    relight_shade(envs, L, rays, normal, albedo, rough, fresnel, acc, S, acc_mask_threshold, rescale_value,
+                  (bins, pos, vis), vis_equation, out, row0)
+    del keep
+    return with_bg[:, row0:row0 + n], without_bg[:, row0:row0 + n]
+
+
+def relight_visibility(tensoIR, envs, L, rays, depth, normal, acc, u, num_samples, acc_mask_threshold, vis_equation):
+    """The material-independent half of relight_chunk_fused for up to RELIGHT_MAX_LIGHTS maps (``envs``, L entries):
+    tir_relight_sample, the read-back of the list length and the density march on the list.  Inputs are contiguous
+    fp32 (u fp64 [L, n, S]) device tensors.  -> (bins, pos, vis), what relight_shade reads."""
+    lib = _lib.load()
+    dev = rays.device
+    n, S = int(rays.shape[0]), int(num_samples)
     cap = L * n * S
     bins = torch.empty(L, n, S, dtype=torch.int32, device=dev)
     pos = torch.empty(L, n, S, dtype=torch.int32, device=dev)
@@ -115,16 +140,26 @@ def relight_chunk_fused(tensoIR, envir_light, light_names, rays, maps, rescale_v
         vis = (t_last if vis_equation == 'nerv' else acc_s).contiguous()
     else:
         vis = torch.zeros(1, device=dev)
+    return bins, pos, vis
+
+
+def relight_shade(envs, L, rays, normal, albedo, rough, fresnel, acc, num_samples, acc_mask_threshold, rescale_value,
+                  visibility, vis_equation, out, row0):
+    """The material half of relight_chunk_fused: tir_relight_shade of the chunk's rows into out = (with_bg, without_bg)
+    [L, R, 3] at rows row0.., with ``visibility`` = relight_visibility's (bins, pos, vis) for the same envs, rays and
+    maps.  rough is [n, 1] or [n, 3]; inputs are contiguous fp32 device tensors."""
+    lib = _lib.load()
+    bins, pos, vis = visibility
+    with_bg, without_bg = out
+    n, dev = int(rays.shape[0]), rays.device
     resc = torch.as_tensor(rescale_value, dtype=torch.float32).to(dev).reshape(-1).expand(3).contiguous()
     assert with_bg.is_contiguous() and without_bg.is_contiguous()
     _lib.check(lib.tir_relight_shade(envs, L, _lib.dptr(rays), _lib.dptr(normal), _lib.dptr(albedo), _lib.dptr(rough),
-                                     int(rough.shape[1]), _lib.dptr(fresnel), _lib.dptr(acc), n, S, thr,
-                                     _lib.dptr(resc), _lib.dptr(bins, torch.int32), _lib.dptr(pos, torch.int32),
-                                     _lib.dptr(vis), 0 if vis_equation == 'nerv' else 1, _lib.dptr(with_bg),
-                                     _lib.dptr(without_bg), int(with_bg.shape[1]), int(row0), _lib.stream_ptr()),
-               "tir_relight_shade")
-    del keep
-    return with_bg[:, row0:row0 + n], without_bg[:, row0:row0 + n]
+                                     int(rough.shape[1]), _lib.dptr(fresnel), _lib.dptr(acc), n, int(num_samples),
+                                     float(acc_mask_threshold), _lib.dptr(resc), _lib.dptr(bins, torch.int32),
+                                     _lib.dptr(pos, torch.int32), _lib.dptr(vis),
+                                     0 if vis_equation == 'nerv' else 1, _lib.dptr(with_bg), _lib.dptr(without_bg),
+                                     int(with_bg.shape[1]), int(row0), _lib.stream_ptr()), "tir_relight_shade")
 
 
 def pair_metrics(a, b, H, W):

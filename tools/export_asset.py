@@ -3,10 +3,12 @@ same seeds, the checkpoint loaded with tensoir_b200.relighting._load_model): ``{
 of tools/export_mesh.py with per-vertex albedo, roughness and predicted normal, and ``{ckpt[:-3]}_asset_envmap_{k}.hdr``
 the radiance of light k (tensoir_b200.mesh.export_asset, level 0.005).  A general multi-light checkpoint
 (``light_name_list``) gets no .hdr files: its SG lights (lgtSGs_list) are not in the state_dict, so the checkpoint does
-not hold them and the loaded model's lights are their random initialisation; the tool says so.  Run it with a TensoIR
-checkout on PYTHONPATH (for opt):
+not hold them and the loaded model's lights are their random initialisation; the tool says so.  With
+``--edits <json>`` (a list of material rules, the fields of tensoir_b200.editing.MaterialEdit, without fresnel ops)
+the albedo, colour and roughness columns hold the edited materials.  Run it with a TensoIR checkout on PYTHONPATH (for
+opt):
 
-    PYTHONPATH=<TensoIR checkout>:. python tools/export_asset.py --config <config> --ckpt <ckpt>
+    PYTHONPATH=<TensoIR checkout>:. python tools/export_asset.py --config <config> --ckpt <ckpt> [--edits <json>]
 """
 import os
 import sys
@@ -19,10 +21,31 @@ if ROOT not in sys.path:
     sys.path.append(ROOT)
 
 
+def pop_edits(argv):
+    """Remove ``--edits <json>`` from argv (opt.config_parser does not know it) -> the JSON path or None."""
+    if "--edits" not in argv:
+        return None
+    i = argv.index("--edits")
+    if i + 1 >= len(argv):
+        raise SystemExit("--edits needs a JSON file")
+    path = argv[i + 1]
+    del argv[i:i + 2]
+    return path
+
+
+def load_rules(path):
+    """The rule list of an --edits JSON file ([rule, ...]) as MaterialEdit, validated as load_edits validates a
+    variant."""
+    import json
+    from tensoir_b200.editing import load_edits
+    with open(path) as f:
+        return load_edits({"asset": json.load(f)})["asset"]
+
+
 @torch.no_grad()
-def main(args):
-    """export_asset on ``args.ckpt``, on ``cuda:{args.local_rank}`` (device 0 when args has no local_rank); returns the
-    PLY path written (None without a checkpoint)."""
+def main(args, edits=None):
+    """export_asset on ``args.ckpt`` with the material rules ``edits`` (None: unedited), on ``cuda:{args.local_rank}``
+    (device 0 when args has no local_rank); returns the PLY path written (None without a checkpoint)."""
     from tensoir_b200.mesh import export_asset
     from tensoir_b200.relighting import _load_model
     tensoIR = _load_model(args, torch.device(f"cuda:{getattr(args, 'local_rank', 0)}"))
@@ -30,7 +53,7 @@ def main(args):
         return None
     path = f'{args.ckpt[:-3]}_asset.ply'
     learned_lights = not tensoIR.general_lights
-    export_asset(tensoIR, path, level=0.005, envmaps=learned_lights)
+    export_asset(tensoIR, path, level=0.005, envmaps=learned_lights, edits=edits)
     if not learned_lights:
         print(f"{args.ckpt} is a general multi-light checkpoint: its lights (lgtSGs_list) are not saved in the "
               "checkpoint, so no environment map is written")
@@ -40,10 +63,12 @@ def main(args):
 if __name__ == "__main__":
     from opt import config_parser
 
+    edits_path = pop_edits(sys.argv)
+    edits = load_rules(edits_path) if edits_path else None
     args = config_parser()
     print(args)
     torch.set_default_dtype(torch.float32)
     torch.manual_seed(20211202)
     torch.cuda.manual_seed_all(20211202)
     np.random.seed(20211202)
-    main(args)
+    main(args, edits)
