@@ -3,6 +3,7 @@ tir_primary_radiance / tir_primary_radiance_backward against the oracle's autogr
 on the edge cases, and as the CUDA-graph step of phase 1 (StaticTrainStep(is_relight=False))."""
 import pytest
 import torch
+import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
 
@@ -44,9 +45,61 @@ def _fused_step(m, rays, li, seed, n_samples=N_SAMPLES):
     return out, loss
 
 
+def _kink_correction(m, fx, out):
+    """Gradient change of the renderModule head when its two ReLUs take the kernel's branches instead of the float64
+    ones -> {parameter name: delta (float64, CPU)}, empty when every branch agrees.
+
+    A pre-activation within the split-BF16 error of 0 can come out on either side of the ReLU kink in the kernel's
+    forward (tests/test_heads_kernels_fp64.py bounds that error), and the gradient of that sample then differs by its
+    whole d z entry.  The head is evaluated in float64 on the fused step's own appearance list (points, weights, ray
+    gradient), once with float64's branches and once with the kernel's dumped ones; every differing branch must lie
+    within twice the split-BF16 bound of its pre-activation."""
+    from test_heads_kernels_fp64 import gemm_bound, EPS32
+    ws = m.__dict__["_tir_radiance_ws"]
+    n = int(ws.t["a_offsets"][-1])
+    ray = ws.t["a_ray"][:n].long()
+    kmask = [ws.t["h1_0"][:n] > 0, ws.t["h2_0"][:n] > 0]
+    rgb = out[0].detach().requires_grad_(True)
+    (g_rgb,) = torch.autograd.grad(_loss(rgb, out[1].detach(), out[6].detach()), rgb)
+    rays, li = fx["rays"].to(DEV).double(), fx["light_idx"].reshape(-1).to(DEV)[ray].view(-1, 1).long()
+    grads = []
+    for use_kernel in (False, True):
+        old = torch.get_default_dtype()
+        torch.set_default_dtype(torch.float64)
+        try:
+            f = oracle_field(fx).to(DEV, torch.float64)
+            for p in f.parameters():
+                p.requires_grad_(True)
+            feat = O.app_feature(f, ws.t["a_xn"][:n].double(), li)
+            vd = rays[ray, 3:6]
+            x = torch.cat([feat, vd, O.positional_encoding(feat, f.fea_pe), O.positional_encoding(vd, f.view_pe)], -1)
+            mm = f.mlp_rgb
+            z1 = F.linear(x, mm.w0, mm.b0)
+            h1 = z1 * (kmask[0] if use_kernel else z1 > 0)
+            z2 = F.linear(h1, mm.w1, mm.b1)
+            h2 = z2 * (kmask[1] if use_kernel else z2 > 0)
+            o = torch.sigmoid(F.linear(h2, mm.w2, mm.b2))
+            aw = ws.t["a_w"][:n].double()[:, None]
+            rgb_map = torch.zeros(rays.shape[0], 3, device=DEV).index_add_(0, ray, aw * o)
+            if not use_kernel:
+                flips = [(kmask[0] != (z1 > 0)), (kmask[1] != (z2 > 0))]
+                if not any(bool(fl.any()) for fl in flips):
+                    return {}
+                for fl, z, a, w, b in ((flips[0], z1, x, mm.w0, mm.b0), (flips[1], z2, h1, mm.w1, mm.b1)):
+                    bnd = 2 * gemm_bound(a.detach().abs() @ w.detach().abs().t(), a.shape[1]) + EPS32 * b.detach().abs()
+                    assert bool((z.detach().abs() <= bnd)[fl].all()), "a ReLU branch differs outside the kernel's error"
+            (rgb_map * g_rgb.double()).sum().backward()
+        finally:
+            torch.set_default_dtype(old)
+        grads.append({k: p.grad for k, p in named_oracle_params(f).items() if p.grad is not None})
+    return {k: (grads[1][k] - grads[0][k]).cpu() for k in grads[0]}
+
+
 def _oracle_step(name, with_mask):
     """One phase-1 training step (recorded CPU jitter, white background) against the oracle differentiated by torch
-    autograd: lists bit-exact, maps and loss 1e-4 (1 + |x|) asserted here -> {parameter: max gradient error / max}."""
+    autograd: lists bit-exact, maps and loss 1e-4 (1 + |x|) asserted here -> {parameter: max gradient error / max}.
+    Where the fused head's forward took the other branch of a ReLU at a pre-activation within its arithmetic error of
+    0, the oracle's gradient is moved to that branch (``_kink_correction``)."""
     fx = _fixture(name)
     rays, li = fx["rays"], fx["light_idx"]
     m = model_from_fixture(fx, DEV, with_mask=with_mask)
@@ -75,6 +128,7 @@ def _oracle_step(name, with_mask):
     wl = _loss(want[0], want[1], want[6])
     close(loss, wl, TOL, "loss")
     wl.backward()
+    corr = _kink_correction(m, fx, out)
     worst, n = {}, 0
     named = named_oracle_params(f)
     for k, p in m.named_parameters():
@@ -82,8 +136,9 @@ def _oracle_step(name, with_mask):
         if w is None or w.grad is None:
             assert p.grad is None or float(p.grad.abs().max()) == 0.0, k
             continue
-        scale = float(w.grad.abs().max()) + 1e-12
-        worst[k] = float((p.grad.detach().cpu() - w.grad).abs().max()) / scale
+        want = w.grad.double() + corr[k] if k in corr else w.grad.double()
+        scale = float(want.abs().max()) + 1e-12
+        worst[k] = float((p.grad.detach().cpu().double() - want).abs().max()) / scale
         n += 1
     assert n >= 12 + 1 + 6, sorted(worst)           # VM factors, basis, renderModule (+ light_line)
     return worst
@@ -101,11 +156,12 @@ def test_radiance_step_matches_oracle_autograd(name, with_mask):
     assert not bad, (bad, max(worst.values()))
 
 
-@pytest.mark.xfail(strict=True, reason="appearance-side gradients on shrunk state A: cause not found, DESIGN.md §9")
 def test_shrunk_state_a_appearance_gradients_match_oracle():
-    """Appearance factors, basis and renderModule gradients on shrunk state A, within 5e-4 of their max.  They are up
-    to ~1e-2 away from the oracle (float32 and float64 oracles agree to 2.5e-5), for the modular path and the fused
-    node alike, while maps, lists and density gradients agree (DESIGN.md §9)."""
+    """Appearance factors, basis and renderModule gradients on shrunk state A, within 5e-4 of their max.  One
+    first-layer pre-activation of this step (sample 241, unit 45) is 1.6e-7 in float64, 0.0013 of the split-BF16
+    error bound of the head's forward: the kernel puts it on the other side of the ReLU, which alone moves these
+    gradients by up to 1.1e-2 of their max.  The oracle's gradient is taken on the kernel's branch there
+    (DESIGN.md §9)."""
     worst = {k: v for k, v in _oracle_step("shrunk_A", True).items() if k.startswith(APP_SIDE)}
     bad = {k: v for k, v in worst.items() if v > 5e-4}
     assert not bad, (bad, max(worst.values()))

@@ -107,13 +107,13 @@ def axis_taps(coord, size, clamped, unit):
     return out
 
 
-def tap_sums(planes, lines, x, clamped, unit):
+def tap_sums(planes, lines, x, clamped, unit, grid=GRID):
     """Per orientation k: the taps and the channel sums A_P = sum_t |w_t||P_t|, AX/AY = sum_t |dw_t/dx||P_t| (x / y of
     the plane), A_L = sum_u |w_u||L_u|, AZ = sum_u |dw_u/dz||L_u|, all [n, C]."""
     res = []
     for k in range(3):
         m0, m1, v = MAT[k][0], MAT[k][1], VEC[k]
-        W, H, D = GRID[m0], GRID[m1], GRID[v]
+        W, H, D = grid[m0], grid[m1], grid[v]
         P = planes[k][0].reshape(planes[k].shape[1], -1).t().abs()
         L = lines[k][0, :, :, 0].t().abs()
         tx, ty, tz = axis_taps(x[:, m0], W, clamped, unit), axis_taps(x[:, m1], H, clamped, unit), \
@@ -153,9 +153,9 @@ def scatter(ts, coef_p, coef_l, C_):
     return out
 
 
-def bound(mag, unit, n_add=None):
+def bound(mag, unit, n_add=None, grid=GRID):
     k = 16.0 if n_add is None else 16.0 + 4.0 * n_add.sqrt()
-    return EPS32 * (k * mag + 2.0 * (max(GRID) - 1) * unit)
+    return EPS32 * (k * mag + 2.0 * (max(grid) - 1) * unit)
 
 
 def check(got, want, bnd, what):
@@ -168,7 +168,7 @@ def check(got, want, bnd, what):
                                        float(want.reshape(-1)[worst]), float(bnd.reshape(-1)[worst]))
 
 
-def check_scatter(gp_got, gl_got, want_p, want_l, mags, units, what):
+def check_scatter(gp_got, gl_got, want_p, want_l, mags, units, what, grid=GRID):
     """Parameter gradients (channel-last [H,W,C] / [D,1,C] from the kernel) against the float64 NCHW gradients."""
     gp_n, gl_n = as_param_layout(gp_got, gl_got)
     for k in range(3):
@@ -177,8 +177,8 @@ def check_scatter(gp_got, gl_got, want_p, want_l, mags, units, what):
         C_ = mp.shape[1]
         H, W = want_p[k].shape[2], want_p[k].shape[3]
         D = want_l[k].shape[2]
-        bp = bound(mp, up, cp[:, None]).t().reshape(1, C_, H, W)
-        bl = bound(ml, ul, cl[:, None]).t().reshape(1, C_, D, 1)
+        bp = bound(mp, up, cp[:, None], grid).t().reshape(1, C_, H, W)
+        bl = bound(ml, ul, cl[:, None], grid).t().reshape(1, C_, D, 1)
         check(gp_n[k], want_p[k], bp, f"{what} plane {k}")
         check(gl_n[k], want_l[k], bl, f"{what} line {k}")
 
