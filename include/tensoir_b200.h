@@ -632,6 +632,57 @@ int tir_material_edit(const TirEditRule* rules /* host array [n_rules] */, int32
                       const float* acc, int64_t n, float acc_threshold, const float* scale /* [3] */,
                       float* albedo_out, float* rough_out, float* fresnel_out, int32_t* sel, void* stream);
 
+/* ---- relighting under analytic lights: directional, point and spot lights with marched shadows -----------------------
+ * One chunk of n primary rays under one setup of up to TIR_LIGHTS_MAX lights, light j with K_j area samples, in two
+ * calls around tir_march_density (as tir_relight_sample / tir_relight_shade are).  The slots of a chunk are laid out
+ * light-major: slot(j, i, s) = n * (K_0 + ... + K_{j-1}) + i * K_j + s, so lights of one setup may have different K.
+ *   tir_lights_sample  per slot of a hit ray (acc > acc_mask_threshold), from the surface point p = o + depth*d: the
+ *                      unit direction L towards the light sample and the falloff.  A light without extent, or with
+ *                      K = 1, is sampled at its centre and reads no uniform; otherwise (u[slot][0], u[slot][1]) is
+ *                      mapped to the unit disc (concentric map; the disc's axes are the orthonormal basis of Duff et
+ *                      al. 2017 around its normal) and the sample lies
+ *                        directional: at dir + extent * disc on the plane tangent to dir (extent = tan of the angular
+ *                                     radius), L its normalisation, falloff 1;
+ *                        point, spot: at pos + extent * disc on the disc of the sphere that faces p, L = (q - p)/d,
+ *                                     falloff = cone / d^2, cone = 1 for a point light and, for a spot, 1 where
+ *                                     c = -L . dir >= cos_inner, 0 where c <= cos_outer and smoothstep of
+ *                                     (c - cos_outer) / (cos_inner - cos_outer) between.
+ *                      The slot joins the shadow-ray list (origin p, direction L) when L . normal (raw normal) > 1e-6
+ *                      and falloff > 0.  L [slots,3], falloff [slots] and pos [slots] (list row, or -1) are written for
+ *                      every slot (zeros and -1 on non-hit rays); count and capacity as in tir_relight_sample.
+ *   tir_lights_shade   one warp per ray: linear = sum over lights, in order, of power_j * mean over the light's K slots
+ *                      of (albedo*rescale/pi + GGX) * vis * falloff * cosine, vis as in tir_relight_shade (0 where
+ *                      pos < 0).  without_bg = sRGB(clamp(linear)), white on non-hit rays; with_bg = acc_t*without_bg +
+ *                      (1-acc_t)*background with acc_t = acc > 0.9 ? acc : 0.  `linear` (may be NULL) gets the un-toned
+ *                      sum, 0 on non-hit rays.  Rows are written at [row0 + i] of [out_rows,3] maps.
+ * A point or spot light must lie outside the model's aabb: a shadow ray then leaves the box before it reaches the light,
+ * so tir_march_density, which has one far for all rays, is exact for it.  Every reduction is in a fixed order (no float
+ * atomics): repeated calls give identical bits.  TIR_ERR_SHAPE for n < 0, more than TIR_LIGHTS_MAX lights, K outside
+ * [1, TIR_LIGHT_SAMPLES_MAX], more than INT32_MAX slots, a stride other than 1 or 3 or rows out of range;
+ * TIR_ERR_CONFIG for an unknown type or vis_kind. */
+#define TIR_LIGHTS_MAX 16
+#define TIR_LIGHT_SAMPLES_MAX 1024
+enum { TIR_LIGHT_DIRECTIONAL = 0, TIR_LIGHT_POINT = 1, TIR_LIGHT_SPOT = 2 };
+typedef struct TirLight {
+  int32_t type, n_samples;
+  float dir[3];                /* unit; directional: towards the light; spot: axis, light -> target */
+  float pos[3];                /* point, spot */
+  float power[3];              /* irradiance facing the light (directional) or radiant intensity (point, spot) */
+  float extent;                /* directional: tan(angular radius); point, spot: sphere radius */
+  float cos_inner, cos_outer;  /* spot */
+} TirLight;
+int tir_lights_sample(const TirLight* lights /* host array [n_lights] */, int32_t n_lights, const float* rays,
+                      const float* depth, const float* normal, const float* acc, int64_t n,
+                      float acc_mask_threshold, const double* u /* [slots,2] */, float* L, float* falloff,
+                      int32_t* pos, float* list_o, float* list_d /* [capacity,3] */, int64_t capacity, int64_t* count,
+                      void* stream);
+int tir_lights_shade(const TirLight* lights, int32_t n_lights, const float* rays, const float* normal,
+                     const float* albedo, const float* rough, int32_t rough_stride /* 1: [n,1], 3: [n,3] */,
+                     const float* fresnel, const float* acc, int64_t n, float acc_mask_threshold,
+                     const float* rescale /* [3] */, const float* background /* [3] */, const float* L,
+                     const float* falloff, const int32_t* pos, const float* vis_list, int32_t vis_kind, float* with_bg,
+                     float* without_bg, float* linear /* or NULL */, int64_t out_rows, int64_t row0, void* stream);
+
 /* ---- mesh export: marching cubes over a dense volume (utils.py:165-225, skimage.measure.marching_cubes on
  * TensorBase.getDenseAlpha(), tensorBase_rotated_lights.py:737-753) ---------------------------------------------------
  * volume [X,Y,Z] fp32 C-contiguous, X, Y, Z >= 2 and X*Y*Z <= INT32_MAX (TIR_ERR_SHAPE otherwise).  A point is inside
