@@ -363,11 +363,32 @@ struct WgradSmem {
   __nv_bfloat16 bh[M * SB], bl[M * SB];     // activation tile [row][in]   (small role: products * light, 144 cols)
   __nv_bfloat16 ch[M * SA], cl[M * SA];     // small role: h2 tile
   float colsum[8 * HID];
+  float stage_gz[M * HID];                  // big roles: fp32 rows of the next tile, landing while this one multiplies
+  float stage_act[M * IN];
 };
 
-constexpr int P_W = 14;     // CTAs (row slices) per head for each of the two big weight gradients
-constexpr int P_S = 9;      // CTAs per head for the small ones (gW2, gb2, g basis_mat)
-constexpr int CTAS_PER_JOB = 2 * P_W + P_S;
+// Cost of one row of each weight-gradient role, relative to gW1 (= 1): gW0 loads 150 columns against 128 and runs
+// 10 n8-tiles per warp against 8; the small role (gW2, gb2, g basis_mat) loads ~310 floats per row, partly gathered
+// through the light index, with no prefetch.  Chosen by timing the kernel in the bench step on H100 (4 heads,
+// 33 CTAs each): small-role costs 1.0 / 1.5 / 2.0 / 2.5 / 3.0 / 3.5 gave 249 / 215 / 178 / 170 / 185 / 184 µs, and a
+// gW0 cost of 1.0 or 1.4 instead of 1.2 was slower.
+constexpr float kRowCostW0 = 1.2f;
+constexpr float kRowCostSmall = 2.5f;
+
+// Row slices (CTAs) per head for gW1, gW0 and the small role, from the CTAs a head may use: the split with the
+// smallest largest per-CTA cost, so that the roles of one head finish together.
+struct WgradSplit { int p1, p0, ps; };
+WgradSplit wgrad_split(int ctas) {
+  WgradSplit best{1, 1, 1};
+  float best_cost = 3.4e38f;
+  for (int p1 = 1; p1 <= ctas - 2; ++p1)
+    for (int p0 = 1; p1 + p0 <= ctas - 1; ++p0) {
+      const int ps = ctas - p1 - p0;
+      const float c = fmaxf(fmaxf(1.f / p1, kRowCostW0 / p0), kRowCostSmall / ps);
+      if (c < best_cost) { best_cost = c; best = WgradSplit{p1, p0, ps}; }
+    }
+  return best;
+}
 
 // acc[NT8][4] += A^T B over one 64-row tile: rows m0..m0+15 of the gradient (A columns), columns n0.. (B columns).
 // A stored [k][m] (stride sa), B stored [k][n] (stride sb): both read transposed with ldmatrix.trans.
@@ -398,8 +419,25 @@ __device__ __forceinline__ void wgrad_tile(float (&acc)[NT8][4], const __nv_bflo
   }
 }
 
+// Copy rows [base, min(base + M, r1)) of a row-major fp32 [*, ncol] array into dst ([M][ncol]) with 16-byte cp.async,
+// zero-filling the rest of the tile.  The tile's rows are contiguous, so it is copied as one flat range: with base a
+// multiple of 64 and a 16-byte aligned src, every chunk is aligned for ncol = 128 and 150.  Not waited for here.
+__device__ __forceinline__ void prefetch_tile(float* dst, const float* src, int ncol, int64_t base, int64_t r1) {
+  const int64_t rows = r1 - base < M ? r1 - base : M;
+  const int valid = (int)rows * ncol * 4;                // bytes
+  const float* s = src + base * ncol;
+  for (int c = threadIdx.x; c < M * ncol / 4; c += NT) {
+    const int left = valid - c * 16;
+    const int n = left < 0 ? 0 : (left > 16 ? 16 : left);
+    const uint32_t d = (uint32_t)__cvta_generic_to_shared(dst + c * 4);
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(d), "l"(n ? s + c * 4 : s), "r"(n) : "memory");
+  }
+  asm volatile("cp.async.commit_group;\n" ::: "memory");
+}
+
 // g_w[128][ld] += (d z)^T @ act  over rows [r0, r1);  g_b[128] += column sums of d z.
 // 16 warps: warp w owns gradient rows 16 (w % 8).. and the column half w / 8 (NT8H n8-tiles).
+// The fp32 rows of tile t + 1 are fetched into stage_* while tile t is multiplied.
 template <int NT8H>
 __device__ void wgrad_big(WgradSmem& s, const float* __restrict__ gz, const float* __restrict__ actv, int ncol, int ld,
                           int64_t r0, int64_t r1, float* g_w, float* g_b) {
@@ -408,26 +446,31 @@ __device__ void wgrad_big(WgradSmem& s, const float* __restrict__ gz, const floa
   const int mt = warp & 7, nh = warp >> 3;
   float acc[NT8H][4] = {};
   float cs0 = 0.f, cs1 = 0.f;                 // columns 2 (tid % 64), +1 of d z (512 % 64 == 0: fixed per thread)
+  prefetch_tile(s.stage_gz, gz, HID, r0, r1);
+  prefetch_tile(s.stage_act, actv, ncol, r0, r1);
   for (int i = tid; i < M * SB; i += NT) { s.bh[i] = __float2bfloat16_rn(0.f); s.bl[i] = __float2bfloat16_rn(0.f); }
-  __syncthreads();
   const int half_cols = ncol / 2;             // 64 or 75 float2 per row
   for (int64_t base = r0; base < r1; base += M) {
+    // the staged tile has landed, and every warp is done with the previous tile's MMAs
+    asm volatile("cp.async.wait_all;\n" ::: "memory");
+    __syncthreads();
     for (int idx = tid; idx < M * (HID / 2); idx += NT) {
       const int row = idx / (HID / 2), k = (idx % (HID / 2)) * 2;
-      float2 v = make_float2(0.f, 0.f);
-      if (base + row < r1) v = *reinterpret_cast<const float2*>(gz + (base + row) * HID + k);
+      const float2 v = *reinterpret_cast<const float2*>(s.stage_gz + row * HID + k);
       cs0 += v.x; cs1 += v.y;
       store_pair(s.ah, s.al, row * SA + k, v.x, v.y);
     }
     for (int idx = tid; idx < M * half_cols; idx += NT) {
       const int row = idx / half_cols, k = (idx % half_cols) * 2;
-      float2 v = make_float2(0.f, 0.f);
-      if (base + row < r1) v = *reinterpret_cast<const float2*>(actv + (base + row) * ncol + k);
+      const float2 v = *reinterpret_cast<const float2*>(s.stage_act + row * ncol + k);
       store_pair(s.bh, s.bl, row * SB + k, v.x, v.y);
     }
     __syncthreads();
+    if (base + M < r1) {
+      prefetch_tile(s.stage_gz, gz, HID, base + M, r1);
+      prefetch_tile(s.stage_act, actv, ncol, base + M, r1);
+    }
     wgrad_tile<NT8H>(acc, s.ah, s.al, SA, mt * 16, s.bh, s.bl, SB, nh * NT8H * 8, lane);
-    __syncthreads();
   }
 #pragma unroll
   for (int nt = 0; nt < NT8H; ++nt)
@@ -452,6 +495,7 @@ struct WgradParams {
   HeadBwdJob jobs[kMaxHeadJobs];
   HeadsBwdShared sh;
   int n_jobs;
+  WgradSplit split;
   int64_t n;
   const int64_t* n_dev;
 };
@@ -561,18 +605,21 @@ __device__ void wgrad_small(WgradSmem& s, const HeadBwdJob& J, const HeadsBwdSha
 __global__ void __launch_bounds__(NT, 1) heads_wgrad_kernel(const WgradParams p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   WgradSmem& s = *reinterpret_cast<WgradSmem*>(smem_raw);
-  const int job = (int)(blockIdx.x / CTAS_PER_JOB), role_id = (int)(blockIdx.x % CTAS_PER_JOB);
+  const WgradSplit sp = p.split;
+  const int per_job = sp.p1 + sp.p0 + sp.ps;
+  const int job = (int)(blockIdx.x / per_job), role_id = (int)(blockIdx.x % per_job);
   const HeadBwdJob& J = p.jobs[job];
   const int64_t total = list_rows(p.n, p.n_dev);
-  const int parts = role_id < 2 * P_W ? P_W : P_S;
-  const int part = role_id < P_W ? role_id : (role_id < 2 * P_W ? role_id - P_W : role_id - 2 * P_W);
+  const int role = role_id < sp.p1 ? 0 : (role_id < sp.p1 + sp.p0 ? 1 : 2);
+  const int parts = role == 0 ? sp.p1 : (role == 1 ? sp.p0 : sp.ps);
+  const int part = role == 0 ? role_id : (role == 1 ? role_id - sp.p1 : role_id - sp.p1 - sp.p0);
   int64_t chunk = (total + parts - 1) / parts;
   chunk = (chunk + M - 1) / M * M;
   const int64_t r0 = (int64_t)part * chunk;
   const int64_t r1 = r0 + chunk < total ? r0 + chunk : total;
   if (r0 >= r1) return;
-  if (role_id < P_W) wgrad_big<8>(s, J.gz2, J.h1, HID, HID, r0, r1, J.g_w1, J.g_b1);          // gW1 = dz2^T h1, gb1
-  else if (role_id < 2 * P_W) wgrad_big<10>(s, J.gz1, J.inp, IN, IN, r0, r1, J.g_w0, J.g_b0); // gW0 = dz1^T inp, gb0
+  if (role == 0) wgrad_big<8>(s, J.gz2, J.h1, HID, HID, r0, r1, J.g_w1, J.g_b1);          // gW1 = dz2^T h1, gb1
+  else if (role == 1) wgrad_big<10>(s, J.gz1, J.inp, IN, IN, r0, r1, J.g_w0, J.g_b0);     // gW0 = dz1^T inp, gb0
   else wgrad_small(s, J, p.sh, r0, r1);
 }
 
@@ -595,6 +642,10 @@ int launch_heads_backward(const TirField& f, const HeadBwdJob* jobs, int n_jobs,
       return TIR_ERR_NULL;
     if (J.light_mode != 0 && (!J.mlp.light_line || !sh.g_light || !sh.x0[J.point_set])) return TIR_ERR_NULL;
     if (J.point_set < 0 || J.point_set > 1) return TIR_ERR_CONFIG;
+    // the weight gradients copy 64-row tiles of these with 16-byte cp.async
+    if ((reinterpret_cast<uintptr_t>(J.gz1) | reinterpret_cast<uintptr_t>(J.gz2) | reinterpret_cast<uintptr_t>(J.h1) |
+         reinterpret_cast<uintptr_t>(J.inp)) & 15)
+      return TIR_ERR_CONFIG;
   }
   static bool configured = false;
   if (!configured) {
@@ -611,12 +662,14 @@ int launch_heads_backward(const TirField& f, const HeadBwdJob* jobs, int n_jobs,
   wp.sh = sh; wp.n_jobs = n_jobs; wp.n = n; wp.n_dev = n_dev;
   for (int j = 0; j < n_jobs; ++j) { dp.jobs[j] = jobs[j]; wp.jobs[j] = jobs[j]; }
   const int64_t tiles = (n + M - 1) / M;
-  int per_job = num_sms() / n_jobs;
+  int per_job = num_sms() / n_jobs;           // one wave: one CTA per SM (both kernels fit one CTA per SM)
+  if (per_job < 3) return TIR_ERR_CONFIG;     // the weight gradients need a CTA per role
+  wp.split = wgrad_split(per_job);
   if (tiles < per_job) per_job = (int)tiles;
   heads_dgrad_kernel<<<per_job * n_jobs, NT, sizeof(DgradSmem), stream>>>(dp);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return (int)e;
-  heads_wgrad_kernel<<<CTAS_PER_JOB * n_jobs, NT, sizeof(WgradSmem), stream>>>(wp);
+  heads_wgrad_kernel<<<(wp.split.p1 + wp.split.p0 + wp.split.ps) * n_jobs, NT, sizeof(WgradSmem), stream>>>(wp);
   return (int)cudaGetLastError();
 }
 
