@@ -4,12 +4,14 @@
 // (tensoRF_rotated_lights.py:167-224) + MLPRender_Fea / MLPBRDF_PEandFeature (tensorBase:122-146, :182-208).
 // The secondary sample list goes through the wgmma kernel of tir_mlp_wgmma.cu.
 //
-// The four contractions are genuine dense GEMMs over a tile of 64 samples and run on the tensor cores with
+// The four contractions are genuine dense GEMMs over a tile of 32 samples and run on the tensor cores with
 // error-compensated BF16: every fp32 operand x is split into hi = bf16(x), lo = bf16(x - hi) and the product is
 // accumulated in fp32 as A_hi*B_hi + A_hi*B_lo + A_lo*B_hi (the dropped lo*lo term is 2^-16 relative), which keeps
 // the 1e-4 parity bar that plain BF16/TF32 (~1e-3) would miss.  Persistent CTAs (one per SM) keep all weights
-// resident in shared memory as split BF16 (176 KB) and stream 64-sample tiles through one in-place activation
-// buffer; fragments are fetched with ldmatrix from rows padded to an odd multiple of 16 bytes (conflict free).
+// resident in shared memory as split BF16 (176 KB).  A CTA is two independent groups of 4 warps; each group streams
+// its own 32-sample tiles through its own in-place activation buffer and synchronises on its own named barrier, so
+// one group's gather and dumps overlap the other group's MMAs.  Fragments are fetched with ldmatrix from rows padded
+// to an odd multiple of 16 bytes (conflict free).
 #include <cuda_bf16.h>
 #include "tir_device.cuh"
 #include "tir_internal.h"
@@ -26,25 +28,31 @@ constexpr int HID = 128;
 constexpr int IN = 150;           // 27 + 3 + 54 + 54 + 6 + 6
 constexpr int K1 = 160;           // IN padded to k16
 constexpr int ON = 8;             // output N padded (<= 4 real)
-constexpr int M = 64;             // samples per tile
-constexpr int NT = 256;           // 8 warps
+constexpr int M = 32;             // samples per tile
+constexpr int NG = 2;             // warp groups per CTA, one tile in flight each
+constexpr int GT = 128;           // threads per group (4 warps)
+constexpr int NT = NG * GT;
 constexpr int SA = 168;           // activation row stride (bf16 elements); 336 B = odd multiple of 16 B
 constexpr int SW0 = 168;          // W0 rows [128][K1 -> 168]
 constexpr int SW1 = 136;          // W1 rows [128][128 -> 136]
 constexpr int SBS = 152;          // basis rows [32][144 -> 152]
 constexpr int SW2 = 136;          // W2 rows [8][128 -> 136]
 
+struct __align__(16) Tile {                  // one warp group's tile
+  __nv_bfloat16 ah[M * SA], al[M * SA];      // activations, in place across layers
+  float xn[M][3];
+  float xv[M][3];
+  int light[M];
+};
+
 struct Smem {
   __nv_bfloat16 w0h[HID * SW0], w0l[HID * SW0];
   __nv_bfloat16 w1h[HID * SW1], w1l[HID * SW1];
   __nv_bfloat16 bsh[FN * SBS], bsl[FN * SBS];
   __nv_bfloat16 w2h[ON * SW2], w2l[ON * SW2];
-  __nv_bfloat16 ah[M * SA], al[M * SA];      // activations, in place across layers
+  Tile t[NG];
   float b0[HID], b1[HID], b2[ON];
   float lmean[K0];                           // mean light row (light_mode 2, compute_intrinfeature)
-  float xn[M][3];
-  float xv[M][3];
-  int light[M];
 };
 
 struct MlpParams {
@@ -97,12 +105,19 @@ __device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], 
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
+// The named barrier of warp group `grp` (barrier 0 is __syncthreads).
+__device__ __forceinline__ void group_sync(int grp) {
+  asm volatile("bar.sync %0, %1;\n" ::"r"(grp + 1), "r"(GT) : "memory");
+}
+
 // One warp: acc[MT][NTL] (m16 x n8 tiles) += A[m0.., :K] * W[n0.., :K]^T with the 3-term split.
-// A row-major [M][SA] (hi/lo), W row-major [N][SWx] (hi/lo) == PyTorch [out,in].
+// A row-major [M][SA] (hi/lo), W row-major [N][SWx] (hi/lo) == PyTorch [out,in].  Every acc entry sees the same
+// k order whatever MT / NTL are, so the warp mapping does not change the sums.
 template <int MT, int NTL>
 __device__ __forceinline__ void warp_gemm(float (&acc)[MT][NTL][4], const __nv_bfloat16* ah, const __nv_bfloat16* al,
                                           int m0, const __nv_bfloat16* wh, const __nv_bfloat16* wl, int sw, int n0,
                                           int K, int lane) {
+  static_assert(NTL == 1 || NTL % 2 == 0, "n8 tiles are loaded in pairs");
   // ldmatrix source rows: A x4 = {(r0-7,k0-7),(r8-15,k0-7),(r0-7,k8-15),(r8-15,k8-15)}
   const int a_row = (lane & 7) + ((lane >> 3) & 1) * 8;
   const int a_col = (lane >> 4) * 8;
@@ -111,12 +126,15 @@ __device__ __forceinline__ void warp_gemm(float (&acc)[MT][NTL][4], const __nv_b
   const int b_col = ((lane >> 3) & 1) * 8;
   for (int k = 0; k < K; k += 16) {
     uint32_t bh[NTL][2], bl[NTL][2];
-    if (NTL == 2) {
-      uint32_t t[4];
-      ldsm_x4(t, wh + (n0 + b_row) * sw + k + b_col);
-      bh[0][0] = t[0]; bh[0][1] = t[1]; bh[NTL - 1][0] = t[2]; bh[NTL - 1][1] = t[3];
-      ldsm_x4(t, wl + (n0 + b_row) * sw + k + b_col);
-      bl[0][0] = t[0]; bl[0][1] = t[1]; bl[NTL - 1][0] = t[2]; bl[NTL - 1][1] = t[3];
+    if constexpr (NTL % 2 == 0) {
+#pragma unroll
+      for (int p = 0; p < NTL / 2; ++p) {
+        uint32_t t[4];
+        ldsm_x4(t, wh + (n0 + p * 16 + b_row) * sw + k + b_col);
+        bh[2 * p][0] = t[0]; bh[2 * p][1] = t[1]; bh[2 * p + 1][0] = t[2]; bh[2 * p + 1][1] = t[3];
+        ldsm_x4(t, wl + (n0 + p * 16 + b_row) * sw + k + b_col);
+        bl[2 * p][0] = t[0]; bl[2 * p][1] = t[1]; bl[2 * p + 1][0] = t[2]; bl[2 * p + 1][1] = t[3];
+      }
     } else {
       uint32_t t[2];
       ldsm_x2(t, wh + (n0 + (lane & 7)) * sw + k + b_col);
@@ -140,11 +158,11 @@ __device__ __forceinline__ void warp_gemm(float (&acc)[MT][NTL][4], const __nv_b
 }
 
 // Write columns [0, ncol) of the activation tile (hi + lo) to a row-major fp32 global array (ncol even): a warp writes
-// one row at a time as float2 (coalesced 256-byte segments, no integer division).
+// one row at a time as float2 (coalesced 256-byte segments, no integer division).  gtid: thread index in the group.
 __device__ __forceinline__ void dump_tile(const __nv_bfloat16* ah, const __nv_bfloat16* al, float* dst, int ncol,
-                                          int64_t base, int64_t total, int tid) {
-  const int lane = tid & 31, warp = tid >> 5;
-  for (int row = warp; row < M; row += NT / 32) {
+                                          int64_t base, int64_t total, int gtid) {
+  const int lane = gtid & 31, warp = gtid >> 5;
+  for (int row = warp; row < M; row += GT / 32) {
     if (base + row >= total) break;
     float* d = dst + (base + row) * ncol;
     for (int c = 2 * lane; c < ncol; c += 64) {
@@ -159,7 +177,7 @@ __device__ __forceinline__ void dump_tile(const __nv_bfloat16* ah, const __nv_bf
 __global__ void __launch_bounds__(NT, 1) app_mlp_kernel(const MlpParams p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   Smem& s = *reinterpret_cast<Smem*>(smem_raw);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x, lane = tid & 31;
   const int g = lane >> 2, t4 = lane & 3;
   const int n_jobs = p.n_jobs;
   const int job = (int)(blockIdx.x % n_jobs);
@@ -197,16 +215,19 @@ __global__ void __launch_bounds__(NT, 1) app_mlp_kernel(const MlpParams p) {
   }
   __syncthreads();
 
+  // ---- tiles: group grp of CTA c of this job takes tiles 2c + grp, +2 x (CTAs of the job), ...
+  const int grp = tid / GT, gtid = tid % GT, gw = gtid >> 5;
+  Tile& T = s.t[grp];
   const int64_t total = list_rows(p.n_points, p.n_dev);
   const int64_t n_tiles = (total + M - 1) / M;
-  const int64_t tile0 = (int64_t)(blockIdx.x / n_jobs);
-  const int64_t tstep = (int64_t)(gridDim.x / n_jobs);
+  const int64_t tile0 = (int64_t)(blockIdx.x / n_jobs) * NG + grp;
+  const int64_t tstep = (int64_t)(gridDim.x / n_jobs) * NG;
 
   for (int64_t tile = tile0; tile < n_tiles; tile += tstep) {
     const int64_t base = tile * M;
     // ---- point metadata
-    if (tid < M) {
-      const int64_t i = base + tid;
+    if (gtid < M) {
+      const int64_t i = base + gtid;
       float xn0 = 0.f, xn1 = 0.f, xn2 = 0.f, v0 = 0.f, v1 = 0.f, v2 = 0.f;
       int li = 0;
       if (i < total) {
@@ -216,17 +237,17 @@ __global__ void __launch_bounds__(NT, 1) app_mlp_kernel(const MlpParams p) {
         v0 = xi[0]; v1 = xi[1]; v2 = xi[2];
         li = J.light_idx ? J.light_idx[r] : 0;
       }
-      s.xn[tid][0] = xn0; s.xn[tid][1] = xn1; s.xn[tid][2] = xn2;
-      s.xv[tid][0] = v0; s.xv[tid][1] = v1; s.xv[tid][2] = v2;
-      s.light[tid] = li;
+      T.xn[gtid][0] = xn0; T.xn[gtid][1] = xn1; T.xn[gtid][2] = xn2;
+      T.xv[gtid][0] = v0; T.xv[gtid][1] = v1; T.xv[gtid][2] = v2;
+      T.light[gtid] = li;
     }
-    __syncthreads();
+    group_sync(grp);
 
     // ---- phase 1: gather.  4 threads per sample, 12 channels of each orientation per thread -> A[m][0..143]
     {
-      const int m = tid >> 2, qd = tid & 3;
-      const float xn[3] = {s.xn[m][0], s.xn[m][1], s.xn[m][2]};
-      const float* lrow = light_mode == 1 ? (mlp.light_line + (size_t)s.light[m] * K0)
+      const int m = gtid >> 2, qd = gtid & 3;
+      const float xn[3] = {T.xn[m][0], T.xn[m][1], T.xn[m][2]};
+      const float* lrow = light_mode == 1 ? (mlp.light_line + (size_t)T.light[m] * K0)
                                           : (light_mode == 2 ? s.lmean : nullptr);
       float* x0_dst = (J.save_x0 && base + m < total) ? J.save_x0 + (base + m) * K0 : nullptr;
 #pragma unroll
@@ -250,20 +271,20 @@ __global__ void __launch_bounds__(NT, 1) app_mlp_kernel(const MlpParams p) {
             x.x = __fmul_rn(x.x, lc.x); x.y = __fmul_rn(x.y, lc.y); x.z = __fmul_rn(x.z, lc.z); x.w = __fmul_rn(x.w, lc.w);
           }
           const int col = k * AC + c;
-          store_pair(s.ah, s.al, m * SA + col, x.x, x.y);
-          store_pair(s.ah, s.al, m * SA + col + 2, x.z, x.w);
+          store_pair(T.ah, T.al, m * SA + col, x.x, x.y);
+          store_pair(T.ah, T.al, m * SA + col + 2, x.z, x.w);
         }
       }
     }
-    __syncthreads();
-    if (p.save_xl && job == 0) dump_tile(s.ah, s.al, p.save_xl, K0, base, total, tid);
+    group_sync(grp);
+    if (p.save_xl && job == 0) dump_tile(T.ah, T.al, p.save_xl, K0, base, total, gtid);
 
     // ---- phase 2: basis_mat (144 -> 27, N padded to 32): warp w -> m-tile w/2, n-tiles 2*(w%2), +1
     {
       float acc[1][2][4] = {};
-      const int m0 = (warp >> 1) * 16, n0 = (warp & 1) * 16;
-      warp_gemm<1, 2>(acc, s.ah, s.al, m0, s.bsh, s.bsl, SBS, n0, K0, lane);
-      __syncthreads();   // every warp has finished reading the gathered products; A is rewritten in place
+      const int m0 = (gw >> 1) * 16, n0 = (gw & 1) * 16;
+      warp_gemm<1, 2>(acc, T.ah, T.al, m0, s.bsh, s.bsl, SBS, n0, K0, lane);
+      group_sync(grp);   // every warp has finished reading the gathered products; A is rewritten in place
       // MLP input [feat 27 | x 3 | sin PE(feat) 54 | cos 54 | sin PE(x) 6 | cos 6 | 0 pad 10]  (tensorBase:12-17,:136-142)
 #pragma unroll
       for (int nt = 0; nt < 2; ++nt)
@@ -273,9 +294,9 @@ __global__ void __launch_bounds__(NT, 1) app_mlp_kernel(const MlpParams p) {
           const int n = n0 + nt * 8 + 2 * t4;
           const float va = acc[0][nt][half * 2], vb = acc[0][nt][half * 2 + 1];
           if (n + 1 < F) {
-            store_pair(s.ah, s.al, row * SA + n, va, vb);
+            store_pair(T.ah, T.al, row * SA + n, va, vb);
           } else if (n < F) {
-            store_one(s.ah, s.al, row * SA + n, va);
+            store_one(T.ah, T.al, row * SA + n, va);
           }
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
@@ -285,59 +306,59 @@ __global__ void __launch_bounds__(NT, 1) app_mlp_kernel(const MlpParams p) {
               float s1, c1, s2, c2;
               sincosf(v, &s1, &c1);
               sincosf(__fmul_rn(v, 2.f), &s2, &c2);
-              store_pair(s.ah, s.al, row * SA + 30 + 2 * nn, s1, s2);
-              store_pair(s.ah, s.al, row * SA + 84 + 2 * nn, c1, c2);
+              store_pair(T.ah, T.al, row * SA + 30 + 2 * nn, s1, s2);
+              store_pair(T.ah, T.al, row * SA + 84 + 2 * nn, c1, c2);
             }
           }
         }
-      if (tid < M) {
-        const int row = tid;
+      if (gtid < M) {
+        const int row = gtid;
 #pragma unroll
         for (int d = 0; d < 3; ++d) {
-          const float v = s.xv[row][d];
-          store_one(s.ah, s.al, row * SA + 27 + d, v);
+          const float v = T.xv[row][d];
+          store_one(T.ah, T.al, row * SA + 27 + d, v);
           float s1, c1, s2, c2;
           sincosf(v, &s1, &c1);
           sincosf(__fmul_rn(v, 2.f), &s2, &c2);
-          store_pair(s.ah, s.al, row * SA + 138 + 2 * d, s1, s2);
-          store_pair(s.ah, s.al, row * SA + 144 + 2 * d, c1, c2);
+          store_pair(T.ah, T.al, row * SA + 138 + 2 * d, s1, s2);
+          store_pair(T.ah, T.al, row * SA + 144 + 2 * d, c1, c2);
         }
 #pragma unroll
-        for (int c = IN; c < K1; c += 2) store_pair(s.ah, s.al, row * SA + c, 0.f, 0.f);
+        for (int c = IN; c < K1; c += 2) store_pair(T.ah, T.al, row * SA + c, 0.f, 0.f);
       }
     }
-    __syncthreads();
-    if (J.save_in) dump_tile(s.ah, s.al, J.save_in, IN, base, total, tid);
+    group_sync(grp);
+    if (J.save_in) dump_tile(T.ah, T.al, J.save_in, IN, base, total, gtid);
 
-    // ---- phases 3/4: hidden layers.  warp w -> all 64 rows x units [16w, 16w+16)
+    // ---- phases 3/4: hidden layers.  warp w of the group -> all 32 rows x units [32w, 32w+32)
     auto hidden_layer = [&](const __nv_bfloat16* wh, const __nv_bfloat16* wl, int sw, const float* bias, int K) {
-      float acc[4][2][4] = {};
-      warp_gemm<4, 2>(acc, s.ah, s.al, 0, wh, wl, sw, warp * 16, K, lane);
-      __syncthreads();
+      float acc[2][4][4] = {};
+      warp_gemm<2, 4>(acc, T.ah, T.al, 0, wh, wl, sw, gw * 32, K, lane);
+      group_sync(grp);
 #pragma unroll
-      for (int mt = 0; mt < 4; ++mt)
+      for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
-        for (int nt = 0; nt < 2; ++nt) {
-          const int n = warp * 16 + nt * 8 + 2 * t4;
+        for (int nt = 0; nt < 4; ++nt) {
+          const int n = gw * 32 + nt * 8 + 2 * t4;
           const float ba = bias[n], bb = bias[n + 1];
-          store_pair(s.ah, s.al, (mt * 16 + g) * SA + n, fmaxf(acc[mt][nt][0] + ba, 0.f), fmaxf(acc[mt][nt][1] + bb, 0.f));
-          store_pair(s.ah, s.al, (mt * 16 + g + 8) * SA + n, fmaxf(acc[mt][nt][2] + ba, 0.f),
+          store_pair(T.ah, T.al, (mt * 16 + g) * SA + n, fmaxf(acc[mt][nt][0] + ba, 0.f), fmaxf(acc[mt][nt][1] + bb, 0.f));
+          store_pair(T.ah, T.al, (mt * 16 + g + 8) * SA + n, fmaxf(acc[mt][nt][2] + ba, 0.f),
                      fmaxf(acc[mt][nt][3] + bb, 0.f));
         }
-      __syncthreads();
+      group_sync(grp);
     };
     hidden_layer(s.w0h, s.w0l, SW0, s.b0, K1);
-    if (J.save_h1) dump_tile(s.ah, s.al, J.save_h1, HID, base, total, tid);
+    if (J.save_h1) dump_tile(T.ah, T.al, J.save_h1, HID, base, total, gtid);
     hidden_layer(s.w1h, s.w1l, SW1, s.b1, HID);
-    if (J.save_h2) dump_tile(s.ah, s.al, J.save_h2, HID, base, total, tid);
+    if (J.save_h2) dump_tile(T.ah, T.al, J.save_h2, HID, base, total, gtid);
 
-    // ---- phase 5: output layer (N padded to 8) on warps 0..3, activation
-    if (warp < 4) {
+    // ---- phase 5: output layer (N padded to 8) on warps 0..1 of the group, activation
+    if (gw < M / 16) {
       float acc[1][1][4] = {};
-      warp_gemm<1, 1>(acc, s.ah, s.al, warp * 16, s.w2h, s.w2l, SW2, 0, HID, lane);
+      warp_gemm<1, 1>(acc, T.ah, T.al, gw * 16, s.w2h, s.w2l, SW2, 0, HID, lane);
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const int row = warp * 16 + g + (e >> 1) * 8;
+        const int row = gw * 16 + g + (e >> 1) * 8;
         const int o = 2 * t4 + (e & 1);
         if (o < out_dim) {
           const float a = acc[0][0][e] + s.b2[o];
@@ -347,7 +368,7 @@ __global__ void __launch_bounds__(NT, 1) app_mlp_kernel(const MlpParams p) {
         }
       }
     }
-    __syncthreads();
+    group_sync(grp);
   }
 }
 
@@ -367,10 +388,10 @@ int launch(const MlpParams& p, int64_t n, cudaStream_t stream) {
     if (e != cudaSuccess) return (int)e;
     configured = true;
   }
-  int64_t tiles = (n + M - 1) / M;
+  const int64_t ctas = (n + NG * M - 1) / (NG * M);     // a CTA has NG tiles in flight
   const int nj = p.n_jobs;
   int per_job = num_sms() / nj;                            // CTAs per job: one wave, one CTA per SM
-  if (tiles < per_job) per_job = (int)(tiles > 0 ? tiles : 1);
+  if (ctas < per_job) per_job = (int)(ctas > 0 ? ctas : 1);
   app_mlp_kernel<<<per_job * nj, NT, smem, stream>>>(p);
   return (int)cudaGetLastError();
 }

@@ -4,8 +4,9 @@
 // and compute_{app,intrin}feature's tail (tensoRF_rotated_lights.py:155-224): in round 1 this was ~300 cuBLAS SIMT
 // sgemm / elementwise launches per step; here it is TWO launches for all heads of a step:
 //
-//   heads_dgrad_kernel   per 64-sample tile: d out -> d z3 -> (W2) -> ReLU' -> (W1^T GEMM) -> ReLU' -> (W0^T GEMM) ->
-//                        positional-encoding backward -> d feat -> (basis^T) -> d (plane*line*light) -> * light -> gx0,
+//   heads_dgrad_kernel   per 32-sample tile, two tiles in flight per CTA: d out -> d z3 -> (W2) -> ReLU' -> (W1^T GEMM)
+//                        -> ReLU' -> (W0^T GEMM) -> positional-encoding backward -> d feat -> (basis^T) ->
+//                        d (plane*line*light) -> * light -> gx0,
 //                        plus the light_line gradient; dumps d z1 / d z2 / d feat for the weight gradients.
 //   heads_wgrad_kernel   split-K weight gradients  gW1 = dz2^T h1,  gW0 = dz1^T inp  on the tensor cores (operands are
 //                        read "transposed" straight from the row-major tiles with ldmatrix.trans), bias column sums,
@@ -93,26 +94,54 @@ __device__ __forceinline__ void warp_gemm_nt(float (&acc)[MT][2][4], const __nv_
   }
 }
 
+// store(i, load(i)) for i = threadIdx.x, + blockDim.x, ... < n: a CTA-wide copy of read-only global data into shared
+// memory.  Each thread issues U loads before it stores any, so U loads are in flight per thread instead of one.
+template <int U, class Load, class Store>
+__device__ __forceinline__ void staged_fill(int n, Load load, Store store) {
+  const int step = (int)blockDim.x;
+  for (int i0 = (int)threadIdx.x; i0 < n; i0 += U * step) {
+    float v[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) v[u] = i0 + u * step < n ? load(i0 + u * step) : 0.f;
+#pragma unroll
+    for (int u = 0; u < U; ++u)
+      if (i0 + u * step < n) store(i0 + u * step, v[u]);
+  }
+}
+
 __device__ __forceinline__ float act_grad(int act, float y) { return act == 0 ? y * (1.f - y) : 1.f - y * y; }
 
 // ---------------------------------------------------------------------------------------------------------------------
 // data gradient
 // ---------------------------------------------------------------------------------------------------------------------
+constexpr int DM = 32;            // rows of a dgrad tile
+constexpr int DG = 2;             // dgrad warp groups per CTA, one tile in flight each
+constexpr int DGT = NT / DG;      // threads per dgrad group (8 warps)
+
+struct __align__(16) DgradTile {  // one warp group's tile
+  union {
+    struct { __nv_bfloat16 h[DM * SA], l[DM * SA]; } a;   // activation-gradient tile (A operand)
+    float gin[DM * GIN];                                  // d input of the MLP after the last GEMM
+  } u;
+  __nv_bfloat16 gfh[DM * SF], gfl[DM * SF];        // d feat tile (A operand of the basis GEMM)
+  float gz3[DM * 4];
+  int light[DM];
+};
+
 struct DgradSmem {
   __nv_bfloat16 w1h[HID * SA], w1l[HID * SA];     // W1^T: [in][out]
   __nv_bfloat16 w0h[GIN * SA], w0l[GIN * SA];     // W0^T: [in < 144][out]
-  union {
-    struct { __nv_bfloat16 h[M * SA], l[M * SA]; } a;   // activation-gradient tile (A operand)
-    float gin[M * GIN];                                 // d input of the MLP after the last GEMM
-  } u;
   __nv_bfloat16 bth[K0 * SF], btl[K0 * SF];        // basis^T: [c][f] (f padded to 32)
-  __nv_bfloat16 gfh[M * SF], gfl[M * SF];          // d feat tile (A operand of the basis GEMM)
+  DgradTile t[DG];
   float w2[4 * HID];
-  float gz3[M * 4];
   float glight[LMAX * K0];
   float lmean[K0];
-  int light[M];
 };
+
+// The named barrier of dgrad warp group `grp` (barrier 0 is __syncthreads).
+__device__ __forceinline__ void group_sync(int grp) {
+  asm volatile("bar.sync %0, %1;\n" ::"r"(grp + 1), "r"(DGT) : "memory");
+}
 
 struct DgradParams {
   TirField f;
@@ -124,10 +153,11 @@ struct DgradParams {
 };
 
 __global__ void __launch_bounds__(NT, 1) heads_dgrad_kernel(const DgradParams p) {
-  // warp w: column block w % 8 (16 columns), row half w / 8 (32 rows) of every 64 x 128 GEMM output
+  // two groups of 8 warps, each on its own 32-row tile; warp w of a group: column block w (16 columns) of every
+  // 32 x 128 GEMM output
   extern __shared__ __align__(128) unsigned char smem_raw[];
   DgradSmem& s = *reinterpret_cast<DgradSmem*>(smem_raw);
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x, lane = tid & 31;
   const int g = lane >> 2, t4 = lane & 3;
   const int job = (int)(blockIdx.x % p.n_jobs);
   const HeadBwdJob& J = p.jobs[job];
@@ -136,19 +166,24 @@ __global__ void __launch_bounds__(NT, 1) heads_dgrad_kernel(const DgradParams p)
   const int mode = J.light_mode;
 
   // ---- stage transposed split-BF16 weights (coalesced global reads; the one-off smem bank conflicts are irrelevant)
-  for (int i = tid; i < HID * HID; i += NT) {
+  constexpr int U = 8;   // staged loads in flight per thread
+  staged_fill<U>(HID * HID, [&](int i) { return __ldg(mlp.w1 + i); }, [&](int i, float v) {
     const int o = i / HID, k = i % HID;          // W1[o][k]  ->  w1T[k][o]
-    split_bf16(__ldg(mlp.w1 + i), s.w1h[k * SA + o], s.w1l[k * SA + o]);
-  }
-  for (int i = tid; i < HID * IN; i += NT) {
+    split_bf16(v, s.w1h[k * SA + o], s.w1l[k * SA + o]);
+  });
+  staged_fill<U>(HID * IN, [&](int i) { return __ldg(mlp.w0 + i); }, [&](int i, float v) {
     const int o = i / IN, k = i % IN;            // W0[o][k]  ->  w0T[k][o], k < 144 only
-    if (k < GIN) split_bf16(__ldg(mlp.w0 + i), s.w0h[k * SA + o], s.w0l[k * SA + o]);
+    if (k < GIN) split_bf16(v, s.w0h[k * SA + o], s.w0l[k * SA + o]);
+  });
+  staged_fill<U>(K0 * SF, [&](int i) {
+                   const int c = i / SF, f = i % SF;
+                   return f < F ? __ldg(mlp.basis + f * K0 + c) : 0.f;
+                 },
+                 [&](int i, float v) { split_bf16(v, s.bth[i], s.btl[i]); });   // basis[f][c] -> bT[c][f]
+  for (int i = tid; i < DG * DM * SF; i += NT) {
+    s.t[i / (DM * SF)].gfh[i % (DM * SF)] = __float2bfloat16_rn(0.f);
+    s.t[i / (DM * SF)].gfl[i % (DM * SF)] = __float2bfloat16_rn(0.f);
   }
-  for (int i = tid; i < K0 * SF; i += NT) {
-    const int c = i / SF, f = i % SF;            // basis[f][c] -> bT[c][f]
-    split_bf16(f < F ? __ldg(mlp.basis + f * K0 + c) : 0.f, s.bth[i], s.btl[i]);
-  }
-  for (int i = tid; i < M * SF; i += NT) { s.gfh[i] = __float2bfloat16_rn(0.f); s.gfl[i] = __float2bfloat16_rn(0.f); }
   for (int i = tid; i < 4 * HID; i += NT) s.w2[i] = (i / HID) < od ? __ldg(mlp.w2 + i) : 0.f;
   for (int i = tid; i < LMAX * K0; i += NT) s.glight[i] = 0.f;
   if (mode == 2)
@@ -159,145 +194,196 @@ __global__ void __launch_bounds__(NT, 1) heads_dgrad_kernel(const DgradParams p)
     }
   __syncthreads();
 
+  const int grp = tid / DGT, gtid = tid % DGT, gw = gtid >> 5;
+  DgradTile& T = s.t[grp];
   const int64_t total = list_rows(p.n, p.n_dev);
-  const int64_t n_tiles = (total + M - 1) / M;
+  const int64_t n_tiles = (total + DM - 1) / DM;
   const float* x0 = p.sh.x0[J.point_set];
 
-  for (int64_t tile = blockIdx.x / p.n_jobs; tile < n_tiles; tile += gridDim.x / p.n_jobs) {
-    const int64_t base = tile * M;
+  for (int64_t tile = (blockIdx.x / p.n_jobs) * DG + grp; tile < n_tiles; tile += (gridDim.x / p.n_jobs) * DG) {
+    const int64_t base = tile * DM;
     // ---- a. d z3 = d out * act'(out)
     {
-      const int row = tid >> 2, o = tid & 3;
+      const int row = gtid >> 2, o = gtid & 3;
       const int64_t i = base + row;
       float v = 0.f;
-      if (row < M && i < total && o < od)
+      if (row < DM && i < total && o < od)
         v = J.g_out[i * J.out_stride + o] * act_grad(J.act, J.out[i * J.out_stride + o]);
-      if (row < M) s.gz3[row * 4 + o] = v;
-      if (tid < M) {
-        const int64_t ii = base + tid;
+      if (row < DM) T.gz3[row * 4 + o] = v;
+      if (gtid < DM) {
+        const int64_t ii = base + gtid;
         int li = 0;
         if (ii < total && mode == 1 && J.light_idx) li = J.light_idx[J.x_index ? (int64_t)J.x_index[ii] : ii];
-        s.light[tid] = li;
+        T.light[gtid] = li;
       }
     }
-    __syncthreads();
-    // ---- b. d z2 = (d z3 @ W2) * [h2 > 0]   (K = out_dim <= 4: CUDA cores)
-    for (int idx = tid; idx < M * (HID / 2); idx += NT) {
+    group_sync(grp);
+    // ---- b. d z2 = (d z3 @ W2) * [h2 > 0]   (K = out_dim <= 4: CUDA cores).  A thread's h2 loads are issued
+    //         before its d z2 stores, which the compiler may not move them past.
+    constexpr int BN = DM * (HID / 2) / DGT;
+    float2 hb[BN];
+#pragma unroll
+    for (int u = 0; u < BN; ++u) {
+      const int idx = gtid + u * DGT, row = idx / (HID / 2), k = (idx % (HID / 2)) * 2;
+      hb[u] = base + row < total ? *reinterpret_cast<const float2*>(J.h2 + (base + row) * HID + k)
+                                 : make_float2(0.f, 0.f);
+    }
+#pragma unroll
+    for (int u = 0; u < BN; ++u) {
+      const int idx = gtid + u * DGT;
       const int row = idx / (HID / 2), k = (idx % (HID / 2)) * 2;
       const int64_t i = base + row;
       float va = 0.f, vb = 0.f;
       if (i < total) {
-        const float2 h = *reinterpret_cast<const float2*>(J.h2 + i * HID + k);
-        const float z0 = s.gz3[row * 4], z1 = s.gz3[row * 4 + 1], z2 = s.gz3[row * 4 + 2], z3 = s.gz3[row * 4 + 3];
+        const float2 h = hb[u];
+        const float z0 = T.gz3[row * 4], z1 = T.gz3[row * 4 + 1], z2 = T.gz3[row * 4 + 2], z3 = T.gz3[row * 4 + 3];
         va = z0 * s.w2[k] + z1 * s.w2[HID + k] + z2 * s.w2[2 * HID + k] + z3 * s.w2[3 * HID + k];
         vb = z0 * s.w2[k + 1] + z1 * s.w2[HID + k + 1] + z2 * s.w2[2 * HID + k + 1] + z3 * s.w2[3 * HID + k + 1];
         va = h.x > 0.f ? va : 0.f;
         vb = h.y > 0.f ? vb : 0.f;
         *reinterpret_cast<float2*>(J.gz2 + i * HID + k) = make_float2(va, vb);
       }
-      store_pair(s.u.a.h, s.u.a.l, row * SA + k, va, vb);
+      store_pair(T.u.a.h, T.u.a.l, row * SA + k, va, vb);
     }
-    __syncthreads();
+    group_sync(grp);
     // ---- c. d z1 = (d z2 @ W1) * [h1 > 0]
-    const int nb = warp & 7, mh = warp >> 3;
+    const int nb = gw;
     {
       float acc[2][2][4] = {};
-      warp_gemm_nt<2>(acc, s.u.a.h, s.u.a.l, mh * 32, s.w1h, s.w1l, SA, nb * 16, HID, lane);
-      __syncthreads();
+      warp_gemm_nt<2>(acc, T.u.a.h, T.u.a.l, 0, s.w1h, s.w1l, SA, nb * 16, HID, lane);
+      float2 h1v[2][2][2];      // the thread's h1 entries, loaded before its first d z1 store
 #pragma unroll
       for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
         for (int nt = 0; nt < 2; ++nt)
 #pragma unroll
           for (int half = 0; half < 2; ++half) {
-            const int row = mh * 32 + mt * 16 + g + half * 8;
+            const int64_t i = base + mt * 16 + g + half * 8;
+            h1v[mt][nt][half] = i < total ? *reinterpret_cast<const float2*>(J.h1 + i * HID + nb * 16 + nt * 8 + 2 * t4)
+                                          : make_float2(0.f, 0.f);
+          }
+      group_sync(grp);
+#pragma unroll
+      for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+        for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+          for (int half = 0; half < 2; ++half) {
+            const int row = mt * 16 + g + half * 8;
             const int col = nb * 16 + nt * 8 + 2 * t4;
             const int64_t i = base + row;
             float va = 0.f, vb = 0.f;
             if (i < total) {
-              const float2 h = *reinterpret_cast<const float2*>(J.h1 + i * HID + col);
+              const float2 h = h1v[mt][nt][half];
               va = h.x > 0.f ? acc[mt][nt][half * 2] : 0.f;
               vb = h.y > 0.f ? acc[mt][nt][half * 2 + 1] : 0.f;
               *reinterpret_cast<float2*>(J.gz1 + i * HID + col) = make_float2(va, vb);
             }
-            store_pair(s.u.a.h, s.u.a.l, row * SA + col, va, vb);
+            store_pair(T.u.a.h, T.u.a.l, row * SA + col, va, vb);
           }
     }
-    __syncthreads();
+    group_sync(grp);
     // ---- d. d input = d z1 @ W0   (columns [0,144) only: the 3-vector and its encoding carry no gradient)
     {
       float acc[2][2][4] = {};
       float acx[1][2][4] = {};
-      warp_gemm_nt<2>(acc, s.u.a.h, s.u.a.l, mh * 32, s.w0h, s.w0l, SA, nb * 16, HID, lane);
-      if (warp < 4) warp_gemm_nt<1>(acx, s.u.a.h, s.u.a.l, warp * 16, s.w0h, s.w0l, SA, HID, HID, lane);
-      __syncthreads();          // every warp is done reading the tile that `gin` aliases
+      warp_gemm_nt<2>(acc, T.u.a.h, T.u.a.l, 0, s.w0h, s.w0l, SA, nb * 16, HID, lane);
+      if (gw < DM / 16) warp_gemm_nt<1>(acx, T.u.a.h, T.u.a.l, gw * 16, s.w0h, s.w0l, SA, HID, HID, lane);
+      group_sync(grp);          // every warp of the group is done reading the tile that `gin` aliases
 #pragma unroll
       for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
         for (int nt = 0; nt < 2; ++nt)
 #pragma unroll
           for (int half = 0; half < 2; ++half) {
-            const int row = mh * 32 + mt * 16 + g + half * 8, col = nb * 16 + nt * 8 + 2 * t4;
-            *reinterpret_cast<float2*>(s.u.gin + row * GIN + col) =
+            const int row = mt * 16 + g + half * 8, col = nb * 16 + nt * 8 + 2 * t4;
+            *reinterpret_cast<float2*>(T.u.gin + row * GIN + col) =
                 make_float2(acc[mt][nt][half * 2], acc[mt][nt][half * 2 + 1]);
           }
-      if (warp < 4) {
+      if (gw < DM / 16) {
 #pragma unroll
         for (int nt = 0; nt < 2; ++nt)
 #pragma unroll
           for (int half = 0; half < 2; ++half) {
-            const int row = warp * 16 + g + half * 8, col = HID + nt * 8 + 2 * t4;
-            *reinterpret_cast<float2*>(s.u.gin + row * GIN + col) =
+            const int row = gw * 16 + g + half * 8, col = HID + nt * 8 + 2 * t4;
+            *reinterpret_cast<float2*>(T.u.gin + row * GIN + col) =
                 make_float2(acx[0][nt][half * 2], acx[0][nt][half * 2 + 1]);
           }
       }
     }
-    __syncthreads();
-    // ---- e. positional-encoding backward: d feat_f = d in_f + sum_p 2^p (d sin_fp * cos_fp - d cos_fp * sin_fp)
-    for (int idx = tid; idx < M * F; idx += NT) {
+    group_sync(grp);
+    // ---- e. positional-encoding backward: d feat_f = d in_f + sum_p 2^p (d sin_fp * cos_fp - d cos_fp * sin_fp);
+    //         the dumped sin / cos of all a thread's entries are loaded before its d feat stores
+    constexpr int EN = (DM * F + DGT - 1) / DGT;
+    float4 sc[EN];            // sin 2^0, sin 2^1, cos 2^0, cos 2^1 of feature f
+#pragma unroll
+    for (int u = 0; u < EN; ++u) {
+      const int idx = gtid + u * DGT, row = idx / F, f = idx % F;
+      sc[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (idx < DM * F && base + row < total) {
+        const float* in = J.inp + (base + row) * IN;
+        sc[u] = make_float4(in[30 + 2 * f], in[31 + 2 * f], in[84 + 2 * f], in[85 + 2 * f]);
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < EN; ++u) {
+      const int idx = gtid + u * DGT;
+      if (idx >= DM * F) break;
       const int row = idx / F, f = idx % F;
       const int64_t i = base + row;
       float v = 0.f;
       if (i < total) {
-        const float* in = J.inp + i * IN;
-        const float* gi = s.u.gin + row * GIN;
-        v = gi[f] + (gi[30 + 2 * f] * in[84 + 2 * f] - gi[84 + 2 * f] * in[30 + 2 * f]) +
-            2.f * (gi[31 + 2 * f] * in[85 + 2 * f] - gi[85 + 2 * f] * in[31 + 2 * f]);
+        const float* gi = T.u.gin + row * GIN;
+        v = gi[f] + (gi[30 + 2 * f] * sc[u].z - gi[84 + 2 * f] * sc[u].x) +
+            2.f * (gi[31 + 2 * f] * sc[u].w - gi[85 + 2 * f] * sc[u].y);
         J.gfeat[i * GF + f] = v;
       }
-      split_bf16(v, s.gfh[row * SF + f], s.gfl[row * SF + f]);
+      split_bf16(v, T.gfh[row * SF + f], T.gfl[row * SF + f]);
     }
-    __syncthreads();
+    group_sync(grp);
     // ---- f. d (products * light) = d feat @ basis (tensor cores: K = 32, N = 144);  gx0 = that * light row;
     //         light_line gradient = sum over samples of d(...) * raw products
     {
-      // 9 column blocks of 16 x 2 row halves = 18 warp tasks; warps 0..15 take one, warps 0..1 a second one
-      for (int task = warp; task < 18; task += NT / 32) {
-        const int cb = task % 9, rh = task / 9;
+      // 9 column blocks of 16 over the tile's 32 rows: warps 0..7 of the group take one, warp 0 the ninth
+      for (int cb = gw; cb < 9; cb += DGT / 32) {
         float acc[2][2][4] = {};
-        warp_gemm_nt<2>(acc, s.gfh, s.gfl, rh * 32, s.bth, s.btl, SF, cb * 16, 32, lane, SF);
+        warp_gemm_nt<2>(acc, T.gfh, T.gfl, 0, s.bth, s.btl, SF, cb * 16, 32, lane, SF);
         float gl[2][2][4];            // d(...) * raw products: the light_line gradient contributions
+        // the light factors and raw products of the thread's entries, loaded before its first gx0 store
+        float2 lf[2][2][2], xr[2][2][2];
 #pragma unroll
         for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
           for (int nt = 0; nt < 2; ++nt)
 #pragma unroll
             for (int half = 0; half < 2; ++half) {
-              const int row = rh * 32 + mt * 16 + g + half * 8, c = cb * 16 + nt * 8 + 2 * t4;
+              const int row = mt * 16 + g + half * 8, c = cb * 16 + nt * 8 + 2 * t4;
+              const int64_t i = base + row;
+              lf[mt][nt][half] = make_float2(1.f, 1.f);
+              xr[mt][nt][half] = make_float2(0.f, 0.f);
+              if (i >= total) continue;
+              if (mode == 1)
+                lf[mt][nt][half] =
+                    __ldg(reinterpret_cast<const float2*>(mlp.light_line + (size_t)T.light[row] * K0 + c));
+              else if (mode == 2)
+                lf[mt][nt][half] = make_float2(s.lmean[c], s.lmean[c + 1]);
+              if (mode != 0) xr[mt][nt][half] = __ldg(reinterpret_cast<const float2*>(x0 + i * K0 + c));
+            }
+#pragma unroll
+        for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+          for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+            for (int half = 0; half < 2; ++half) {
+              const int row = mt * 16 + g + half * 8, c = cb * 16 + nt * 8 + 2 * t4;
               const int64_t i = base + row;
               gl[mt][nt][half * 2] = 0.f; gl[mt][nt][half * 2 + 1] = 0.f;
               if (i >= total) continue;
               const float a0 = acc[mt][nt][half * 2], a1 = acc[mt][nt][half * 2 + 1];
-              float l0 = 1.f, l1 = 1.f;
-              if (mode == 1) {
-                const float2 lv = __ldg(reinterpret_cast<const float2*>(mlp.light_line + (size_t)s.light[row] * K0 + c));
-                l0 = lv.x; l1 = lv.y;
-              } else if (mode == 2) {
-                l0 = s.lmean[c]; l1 = s.lmean[c + 1];
-              }
-              *reinterpret_cast<float2*>(J.gx0 + i * K0 + c) = make_float2(a0 * l0, a1 * l1);
+              const float2 lv = lf[mt][nt][half];
+              *reinterpret_cast<float2*>(J.gx0 + i * K0 + c) = make_float2(a0 * lv.x, a1 * lv.y);
               if (mode != 0) {
-                const float2 xv = __ldg(reinterpret_cast<const float2*>(x0 + i * K0 + c));
+                const float2 xv = xr[mt][nt][half];
                 gl[mt][nt][half * 2] = a0 * xv.x; gl[mt][nt][half * 2 + 1] = a1 * xv.y;
               }
             }
@@ -315,8 +401,8 @@ __global__ void __launch_bounds__(NT, 1) heads_dgrad_kernel(const DgradParams p)
                 for (int mt = 0; mt < 2; ++mt)
 #pragma unroll
                   for (int half = 0; half < 2; ++half) {
-                    const int row = rh * 32 + mt * 16 + g + half * 8;
-                    if (mode == 2 || s.light[row] == l) v += gl[mt][nt][half * 2 + e];
+                    const int row = mt * 16 + g + half * 8;
+                    if (mode == 2 || T.light[row] == l) v += gl[mt][nt][half * 2 + e];
                   }
                 v += __shfl_xor_sync(0xffffffffu, v, 4);
                 v += __shfl_xor_sync(0xffffffffu, v, 8);
@@ -331,7 +417,7 @@ __global__ void __launch_bounds__(NT, 1) heads_dgrad_kernel(const DgradParams p)
               for (int nt = 0; nt < 2; ++nt)
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
-                  const int row = rh * 32 + mt * 16 + g + (e >> 1) * 8, lr = s.light[row];
+                  const int row = mt * 16 + g + (e >> 1) * 8, lr = T.light[row];
                   if (lr >= LMAX && gl[mt][nt][e] != 0.f)
                     atomicAdd(p.sh.g_light + (size_t)lr * K0 + cb * 16 + nt * 8 + 2 * t4 + (e & 1), gl[mt][nt][e]);
                 }
@@ -339,8 +425,9 @@ __global__ void __launch_bounds__(NT, 1) heads_dgrad_kernel(const DgradParams p)
         }
       }
     }
-    __syncthreads();
+    group_sync(grp);
   }
+  __syncthreads();            // both groups have added their light_line sums
   // ---- flush the light_line gradient
   if (mode == 1) {
     const int rows = L < LMAX ? L : LMAX;
@@ -661,11 +748,11 @@ int launch_heads_backward(const TirField& f, const HeadBwdJob* jobs, int n_jobs,
   WgradParams wp{};
   wp.sh = sh; wp.n_jobs = n_jobs; wp.n = n; wp.n_dev = n_dev;
   for (int j = 0; j < n_jobs; ++j) { dp.jobs[j] = jobs[j]; wp.jobs[j] = jobs[j]; }
-  const int64_t tiles = (n + M - 1) / M;
+  const int64_t ctas = (n + DG * DM - 1) / (DG * DM);   // dgrad: DG tiles of DM rows in flight per CTA
   int per_job = num_sms() / n_jobs;           // one wave: one CTA per SM (both kernels fit one CTA per SM)
   if (per_job < 3) return TIR_ERR_CONFIG;     // the weight gradients need a CTA per role
   wp.split = wgrad_split(per_job);
-  if (tiles < per_job) per_job = (int)tiles;
+  if (ctas < per_job) per_job = (int)ctas;
   heads_dgrad_kernel<<<per_job * n_jobs, NT, sizeof(DgradSmem), stream>>>(dp);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return (int)e;
