@@ -65,6 +65,18 @@ def test_null_arguments_are_rejected(lib):
     assert lib.tir_epilogue_fwd(5, None, None, None, None, 0.04, 1, None, None, None, None) == -1
     assert lib.tir_tail_fwd(0, None, None, None, None, None, None, None, None, None, None) == 0      # empty: no-op
     assert lib.tir_density_points(None, None, 0, None, None, None) == 0      # empty input is a no-op, not an error
+    # the four shading entry points: NULL inputs, an empty batch, and a direct-light gradient table larger than the
+    # 200 KB of shared memory the backward may use (34 lights x 512 directions x 12 B), refused before any launch
+    p = ctypes.c_void_p(16)
+    for n in (5, 0, -1):
+        want = -1 if n > 0 else 0
+        assert lib.tir_shade_fwd(*[None] * 6, n, None, None, 512, None, 3, *[None] * 4) == want
+        assert lib.tir_shade_bwd(*[None] * 6, n, None, None, 512, None, 3, *[None] * 9) == want
+        assert lib.tir_shade_hits_fwd(*[None] * 7, n, None, None, 512, None, 3, None, None, 1, None, None, None) == want
+        assert lib.tir_shade_hits_bwd(*[None] * 7, n, None, None, 512, None, 3, None, None, 1, *[None] * 8) == want
+    assert lib.tir_shade_bwd(*[p] * 6, 5, p, p, 512, p, 34, *[p] * 8, None) == -2
+    assert lib.tir_shade_hits_bwd(*[p] * 7, 5, p, p, 512, p, 34, p, p, 1, *[p] * 7, None) == -2
+    assert lib.tir_shade_hits_bwd(*[p] * 7, 5, p, p, 512, p, 33, p, p, 1, *[p] * 6, None, None) == -1
 
 
 def test_no_cpu_fallback():
