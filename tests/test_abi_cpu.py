@@ -77,6 +77,64 @@ def test_null_arguments_are_rejected(lib):
     assert lib.tir_shade_bwd(*[p] * 6, 5, p, p, 512, p, 34, *[p] * 8, None) == -2
     assert lib.tir_shade_hits_bwd(*[p] * 7, 5, p, p, 512, p, 34, p, p, 1, *[p] * 7, None) == -2
     assert lib.tir_shade_hits_bwd(*[p] * 7, 5, p, p, 512, p, 33, p, p, 1, *[p] * 6, None, None) == -1
+    # the march entry points: NULL inputs, empty inputs, and the shape / capacity / config checks, all before any
+    # launch.  The checks that read the structs get a real TirField (dC = 16), TirMarchCfg and TirDensityVolume.
+    from tensoir_b200 import _lib
+    fld = _lib.TirField()
+    fld.dC, fld.aC, fld.grid[:] = 16, 48, [8, 8, 8]
+    cfg = _lib.TirMarchCfg()
+    cfg.sampling, cfg.n_samples, cfg.z_table = _lib.SAMPLE_TABLE, 96, 16
+    vol = _lib.TirDensityVolume()                                   # an empty box: no volume data needed
+    mlp = _lib.TirMlp()
+    F_, G_, V_, M_ = ctypes.byref(fld), ctypes.byref(cfg), ctypes.byref(vol), ctypes.byref(mlp)
+
+    # every call below is refused, so the stand-in pointers are never dereferenced
+    def radiance(n, f=F_, g=G_, cap=64, null=False):
+        q = None if null else p
+        return lib.tir_march_radiance(f, None if null else M_, q, q, None, n, g, q, q, q, q, q, q, cap, None, None)
+
+    def march(n, f=F_, g=G_, null=False):
+        q = None if null else p
+        return lib.tir_march_density(f, q, q, n, g, q, q, q, None, None), radiance(n, f, g, null=null)
+
+    def secondary_vol(n_pts, n_dirs=512, f=F_, g=G_, cap=64, null=False, v=V_):
+        q, m = (None, None) if null else (p, M_)
+        return (lib.tir_secondary_march_vol(f, q, q, n_pts, q, n_dirs, g, v, q, q, q, cap, None, None),
+                lib.tir_secondary_radiance_vol(f, m, q, q, None, n_pts, q, n_dirs, g, v, q, q, q, q, cap, None, None))
+
+    def secondary(n_pts, n_dirs=512, f=F_, g=G_, cap=64, null=False):
+        q, m = (None, None) if null else (p, M_)
+        return (lib.tir_secondary_march(f, q, q, n_pts, q, n_dirs, g, q, q, q, cap, None, None),
+                lib.tir_secondary_radiance(f, m, q, q, None, n_pts, q, n_dirs, g, q, q, q, q, cap, None, None)) \
+            + secondary_vol(n_pts, n_dirs, f, g, cap, null)
+    assert march(5, null=True) == (-1, -1) and march(5, f=None, g=None) == (-1, -1)
+    assert secondary(5, null=True) == (-1,) * 4 and secondary(5, f=None, g=None) == (-1,) * 4
+    for n in (0, -1):                                               # empty inputs: no-ops, whatever the pointers
+        assert march(n, null=True) == (0, 0) and secondary(n, null=True) == (0,) * 4
+    assert secondary_vol(5, v=None) == (-1, -1)                   # the volume entry points without a volume
+    for n_dirs in (0, -3):
+        assert secondary(5, n_dirs=n_dirs) == (-2,) * 4
+    for cap in (0, -1):
+        assert radiance(5, cap=cap) == -4 and secondary(5, cap=cap) == (-4,) * 4
+    for n_samples in (0, -2):
+        cfg.n_samples = n_samples
+        assert march(5) == (-3, -3) and secondary(5) == (-3,) * 4
+    cfg.n_samples = 96
+    fld.dC = 8
+    assert march(5) == (-2, -2) and secondary(5) == (-2,) * 4
+    fld.dC = 16
+    cfg.sampling = 7
+    assert march(5) == (-3, -3) and secondary(5) == (-3,) * 4
+    cfg.sampling = _lib.SAMPLE_TABLE
+    cfg.z_table = None
+    assert march(5) == (-1, -1) and secondary(5) == (-1,) * 4
+    cfg.z_table = 16
+    vol.n[:] = [9, 1, 1]                                            # a box that leaves the 8^3 grid
+    assert secondary_vol(5) == (-2, -2)
+    vol.n[:] = [0, 0, 0]
+    # the 3-CTA volume instance keeps 32-bit per-lane counts: n_pts * n_dirs * ceil(n_samples / 32) * 2 must stay
+    # below 2^32 (here 2^21 * 512 * 3 * 2 = 6.4e9)
+    assert secondary_vol(1 << 21) == (-2, -2)
 
 
 def test_no_cpu_fallback():
