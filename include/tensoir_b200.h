@@ -683,6 +683,33 @@ int tir_lights_shade(const TirLight* lights, int32_t n_lights, const float* rays
                      const float* falloff, const int32_t* pos, const float* vis_list, int32_t vis_kind, float* with_bg,
                      float* without_bg, float* linear /* or NULL */, int64_t out_rows, int64_t row0, void* stream);
 
+/* ---- light transport to the texels of an environment map (inverse lighting) -----------------------------------------
+ * With geometry and materials fixed, relight()'s shading is linear in the environment map: for one surface hit its
+ * estimator has expectation sum_k f_k * vis_k * cos_k * L_k * dOmega_k over the map's K = H*W texels, with
+ * dOmega_k = pdf / pdf_return = 2 pi^2 sin(theta_k) / (H W).  These two calls write that linear map, the transport
+ * T[c, i, k], around tir_march_density (relight()'s 96-sample equal-z table over [0.05, 1.5]):
+ *   tir_transport_sample  per (ray, texel) of a hit ray (acc > acc_mask_threshold): the texel's direction dirs[k] joins
+ *                         the visibility list (origin o + depth*d, direction dirs[k]) when dirs[k] . normal (raw normal)
+ *                         > 1e-6, as a sample of tir_relight_sample does.  pos[n,K] (list row, or -1) is written for
+ *                         every (ray, texel), -1 on non-hit rays; count and capacity as in tir_relight_sample.
+ *   tir_transport_build   one warp per ray, lanes over the texels: T[c, i, k] = (albedo*rescale/pi + GGX)_c * vis *
+ *                         cosine * dOmega[k], the per-sample term of tir_relight_shade with unit radiance and the solid
+ *                         angle in place of 1 / pdf_return; vis as in tir_relight_shade; 0 where pos < 0 and on rows
+ *                         with acc <= acc_mask_threshold.  T is [3, n, K] fp32: one contiguous [n, K] matrix per channel.
+ * No reduction, no float atomics: repeated calls on the same list give identical bits.  TIR_ERR_SHAPE for K outside
+ * [1, TIR_TRANSPORT_MAX_TEXELS], n < 0, n*K > INT32_MAX, capacity outside [0, INT32_MAX] or a stride other than 1 or 3;
+ * TIR_ERR_CONFIG for an unknown vis_kind. */
+#define TIR_TRANSPORT_MAX_TEXELS 2048
+int tir_transport_sample(const float* dirs /* [K,3] */, int32_t K, const float* rays, const float* depth,
+                         const float* normal, const float* acc, int64_t n, float acc_mask_threshold, int32_t* pos,
+                         float* list_o, float* list_d /* [capacity,3] */, int64_t capacity, int64_t* count,
+                         void* stream);
+int tir_transport_build(const float* dirs, const float* domega /* [K] */, int32_t K, const float* rays,
+                        const float* normal, const float* albedo, const float* rough,
+                        int32_t rough_stride /* 1: [n,1], 3: [n,3] */, const float* fresnel, const float* acc,
+                        int64_t n, float acc_mask_threshold, const float* rescale /* [3] */, const int32_t* pos,
+                        const float* vis_list, int32_t vis_kind, float* T /* [3,n,K] */, void* stream);
+
 /* ---- mesh export: marching cubes over a dense volume (utils.py:165-225, skimage.measure.marching_cubes on
  * TensorBase.getDenseAlpha(), tensorBase_rotated_lights.py:737-753) ---------------------------------------------------
  * volume [X,Y,Z] fp32 C-contiguous, X, Y, Z >= 2 and X*Y*Z <= INT32_MAX (TIR_ERR_SHAPE otherwise).  A point is inside

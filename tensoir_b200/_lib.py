@@ -148,6 +148,8 @@ LIGHTS_MAX = 16           # TIR_LIGHTS_MAX
 LIGHT_SAMPLES_MAX = 1024  # TIR_LIGHT_SAMPLES_MAX
 LIGHT_DIRECTIONAL, LIGHT_POINT, LIGHT_SPOT = 0, 1, 2
 
+TRANSPORT_MAX_TEXELS = 2048  # TIR_TRANSPORT_MAX_TEXELS (csrc/tir_transport.cu)
+
 EXPORTS = {
     "tir_abi_version": (C.c_int, []),
     "tir_pack_channels_last": (C.c_int, [f32p, f32p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
@@ -254,6 +256,10 @@ EXPORTS = {
     "tir_lights_shade": (C.c_int, [C.POINTER(TirLight), C.c_int32, f32p, f32p, f32p, f32p, C.c_int32, f32p, f32p,
                                    C.c_int64, C.c_float, f32p, f32p, f32p, f32p, C.c_void_p, f32p, C.c_int32, f32p,
                                    f32p, f32p, C.c_int64, C.c_int64, C.c_void_p]),
+    "tir_transport_sample": (C.c_int, [f32p, C.c_int32, f32p, f32p, f32p, f32p, C.c_int64, C.c_float, C.c_void_p,
+                                       f32p, f32p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "tir_transport_build": (C.c_int, [f32p, f32p, C.c_int32, f32p, f32p, f32p, f32p, C.c_int32, f32p, f32p, C.c_int64,
+                                      C.c_float, f32p, C.c_void_p, f32p, C.c_int32, f32p, C.c_void_p]),
     "tir_marching_cubes_work_size": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int64)]),
     "tir_marching_cubes_count": (C.c_int, [f32p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_int64,
                                            C.c_void_p, C.c_void_p]),
@@ -275,7 +281,8 @@ KERNELS_PER_CALL = {"tir_pack_channels_last": 1, "tir_unpack_channels_last_add":
                     "tir_primary_backward": 9, "tir_primary_radiance": 2, "tir_primary_radiance_backward": 6,
                     "tir_composite_bwd": 1, "tir_tail_fwd": 1, "tir_tail_bwd": 1, "tir_epilogue_fwd": 1,
                     "tir_epilogue_bwd": 1, "tir_eval_view": 3, "tir_relight_sample": 1, "tir_relight_shade": 1,
-                    "tir_material_edit": 1, "tir_lights_sample": 1, "tir_lights_shade": 1, "tir_marching_cubes_count": 7, "tir_marching_cubes_emit": 2}
+                    "tir_material_edit": 1, "tir_lights_sample": 1, "tir_lights_shade": 1,
+                    "tir_transport_sample": 1, "tir_transport_build": 1, "tir_marching_cubes_count": 7, "tir_marching_cubes_emit": 2}
 launch_count = 0
 
 _lib = None

@@ -33,6 +33,18 @@ def write_hdr(path, rgb):
         raise OSError(f"could not write {path}")
 
 
+def latlong_tables(H, W):
+    """The texel tables of an H x W lat-long map as Environment_Light builds them, fp32 on the CPU: sin of the row
+    centres' polar angle [H] and the unit direction of every texel [H, W, 3] (row 0 looks up, column 0 along -x)."""
+    sin_t = torch.sin(torch.linspace(0 + 0.5 / H, np.pi - 0.5 / H, H))
+    lat, lng = np.pi / H, 2 * np.pi / W
+    phi, theta = torch.meshgrid([torch.linspace(np.pi / 2 - 0.5 * lat, -np.pi / 2 + 0.5 * lat, H),
+                                 torch.linspace(np.pi - 0.5 * lng, -np.pi + 0.5 * lng, W)], indexing='ij')
+    dirs = torch.stack([torch.cos(theta) * torch.cos(phi), torch.sin(theta) * torch.cos(phi),
+                        torch.sin(phi)], dim=-1).view(H, W, 3)
+    return sin_t, dirs
+
+
 class Environment_Light:
     """Same tables as the reference class (hdr_rgbs / hdr_pdf_sample / hdr_pdf_return / hdr_dir per light name);
     ``hdr_path`` may be a directory of .hdr files (reference behaviour) or a dict {name: [H,W,3] array}."""
@@ -49,15 +61,10 @@ class Environment_Light:
             rgb = torch.as_tensor(np.asarray(arr)).float()
             inten = torch.sum(rgb, dim=2, keepdim=True)
             H, W, _ = inten.shape
-            sin_t = torch.sin(torch.linspace(0 + 0.5 / H, np.pi - 0.5 / H, H))
+            sin_t, dirs = latlong_tables(H, W)
             pdf = inten * sin_t.view(-1, 1, 1)
             pdf = pdf / torch.sum(pdf)
             pdf_ret = pdf * H * W / (2 * np.pi * np.pi * sin_t.view(-1, 1, 1))
-            lat, lng = np.pi / H, 2 * np.pi / W
-            phi, theta = torch.meshgrid([torch.linspace(np.pi / 2 - 0.5 * lat, -np.pi / 2 + 0.5 * lat, H),
-                                         torch.linspace(np.pi - 0.5 * lng, -np.pi + 0.5 * lng, W)], indexing='ij')
-            dirs = torch.stack([torch.cos(theta) * torch.cos(phi), torch.sin(theta) * torch.cos(phi),
-                                torch.sin(phi)], dim=-1).view(H, W, 3)
             self.hdr_rgbs[name] = rgb.to(device)
             self.hdr_pdf_sample[name] = pdf.to(device)
             self.hdr_pdf_return[name] = pdf_ret.to(device)

@@ -222,10 +222,12 @@ def _load_model(args, device):
 
 
 @torch.no_grad()
-def relight(dataset, args, tensoIR=None):
+def relight(dataset, args, tensoIR=None, *, rescale_value=None):
     """relight_importance.py:30-340.  ``dataset`` follows the reference relighting test set's item contract
     (rays, rgbs [L, H*W, 3], rgbs_mask, albedo, ...) with ``split`` and ``light_names``; ``args`` needs ckpt (when
-    ``tensoIR`` is None), hdrdir, geo_buffer_path and batch_size; the script-only flags default to SCRIPT_DEFAULTS."""
+    ``tensoIR`` is None), hdrdir, geo_buffer_path and batch_size; the script-only flags default to SCRIPT_DEFAULTS.
+    ``rescale_value``: the albedo rescale ratio [3] to shade with; None computes it from ``dataset``
+    (compute_rescale_ratio), as the reference does."""
     from .relight import Environment_Light
     opt = {k: getattr(args, k, v) for k, v in SCRIPT_DEFAULTS.items()}
     device = torch.device("cuda")
@@ -243,8 +245,9 @@ def relight(dataset, args, tensoIR=None):
     thr = float(opt["acc_mask_threshold"])
     envir_light = Environment_Light(args.hdrdir, device=device)
     tables = env_tables(envir_light, names)
-    _, rescale_value = compute_rescale_ratio(tensoIR, dataset)
-    rescale_value = rescale_value.to(device)
+    if rescale_value is None:
+        _, rescale_value = compute_rescale_ratio(tensoIR, dataset)
+    rescale_value = torch.as_tensor(rescale_value, dtype=torch.float32).to(device)
 
     psnr, ssim, l_alex, l_vgg = ({n: [] for n in names} for _ in range(4))
     rgb_frames, aligned_albedo_list, roughness_list = [], [], []
