@@ -478,7 +478,6 @@ extern "C" int tir_primary_heads(const TirField* field, const TirHeadJob* jobs, 
   cudaStream_t stream = (cudaStream_t)stream_;
   const int64_t cap = w->cap_app;
   const int64_t* n_app = w->a_offsets + n_rays;
-  jitter_points_kernel<<<blocks_for(cap * 3, 256), 256, 0, stream>>>(w->a_xn, w->noise, cap, n_app, w->a_xj);
   HeadJobDev dev[kMaxHeadJobs];
   for (int j = 0; j < n_jobs; ++j) {
     if (!w->out[j]) return TIR_ERR_NULL;
@@ -502,6 +501,8 @@ extern "C" int tir_primary_heads(const TirField* field, const TirHeadJob* jobs, 
     if (ps < 0 || ps > 1) return TIR_ERR_CONFIG;
     if (!saved[ps] && w->x0[ps]) { dev[j].save_x0 = w->x0[ps]; saved[ps] = true; }
   }
+  // every job is validated above, before the first launch: a refused call leaves the workspace untouched
+  jitter_points_kernel<<<blocks_for(cap * 3, 256), 256, 0, stream>>>(w->a_xn, w->noise, cap, n_app, w->a_xj);
   rc = launch_heads_forward(*field, dev, n_jobs, cap, n_app, stream);
   if (rc) return rc;
   if (normals_kind != TIR_NORMALS_PREDICTED) {

@@ -135,6 +135,71 @@ def test_null_arguments_are_rejected(lib):
     # the 3-CTA volume instance keeps 32-bit per-lane counts: n_pts * n_dirs * ceil(n_samples / 32) * 2 must stay
     # below 2^32 (here 2^21 * 512 * 3 * 2 = 6.4e9)
     assert secondary_vol(1 << 21) == (-2, -2)
+    # the four fused primary entry points (tir_primary_march / _app_list / _heads / _backward): NULL and empty calls,
+    # a capacity of 0, a density field that is not 16 channels, a job table with fewer than 3 jobs or without a role,
+    # an indexed light on a job that does not read the ray table, and a backward without the x0 dumps; all before any
+    # launch
+    w = _lib.TirPrimaryWork()
+    for k, _ in w._fields_:
+        if k not in ("cap_valid", "cap_app", "x0", "inp", "h1", "h2", "out"):
+            setattr(w, k, 16)
+    w.cap_valid, w.cap_app = 64, 64
+    for j in range(_lib.MAX_HEADS):
+        w.out[j] = w.inp[j] = w.h1[j] = w.h2[j] = 16
+    w.x0[0] = w.x0[1] = 16
+    bw = _lib.TirPrimaryBwdWork()
+    for k, _ in bw._fields_:
+        if k in ("g_out", "gz1", "gz2", "gfeat", "gx0"):
+            getattr(bw, k)[:] = [16] * _lib.MAX_HEADS
+        else:
+            setattr(bw, k, 16)
+    grs = _lib.TirPrimaryGrads()
+    maps = _lib.TirRayMaps()
+    jobs = (_lib.TirHeadJob * 4)()
+    for j, (role, ps, x_in, lm) in enumerate(((0, 0, 0, 1), (1, 0, 1, 2), (2, 1, 1, 2), (3, 0, 1, 2))):
+        jobs[j].role, jobs[j].point_set, jobs[j].x_in, jobs[j].light_mode = role, ps, x_in, lm
+        jobs[j].mlp.light_line = 16
+    W_, B_, J_, R_ = ctypes.byref(w), ctypes.byref(bw), ctypes.byref(grs), ctypes.byref(maps)
+    # every call below is refused before any launch (or is empty), so the stand-in pointers are never dereferenced
+    def pmarch(n, f=F_, null=False):
+        return lib.tir_primary_march(f, None if null else p, n, None if null else G_, None if null else W_, None, None)
+
+    def pheads(n, f=F_, nj=4, kind=0, null=False):
+        q = None if null else p
+        return lib.tir_primary_heads(f, None if null else jobs, nj, kind, q, q, n, None if null else W_, 0.04, 1,
+                                     None if null else R_, q, q, None, None)
+
+    def pbackward(n, f=F_, nj=4, kind=0, null=False):
+        q = None if null else p
+        return lib.tir_primary_backward(f, None if null else jobs, nj, kind, q, q, n, None if null else W_,
+                                        None if null else B_, 0.04, 1, None if null else R_, None, None, None,
+                                        None if null else J_, None)
+
+    def primary(n, f=F_, null=False):
+        return (pmarch(n, f, null), lib.tir_primary_app_list(f, n, None if null else W_, None),
+                pheads(n, f, null=null), pbackward(n, f, null=null))
+    assert primary(5, null=True) == (-1,) * 4 and primary(5, f=None) == (-1,) * 4
+    for n in (0, -1):
+        assert primary(n, null=True) == (0,) * 4
+    for cap in ("cap_valid", "cap_app"):
+        setattr(w, cap, 0)
+        assert pmarch(5) == -4
+        setattr(w, cap, 64)
+    fld.dC = 8
+    assert pmarch(5) == -2
+    fld.dC = 16
+    assert (pheads(5, nj=2), pbackward(5, nj=2)) == (-3, -3)      # fewer than 3 jobs
+    for j, role in ((0, 0), (1, 1), (2, 2)):                         # without the rgb / brdf / brdf-jitter role
+        jobs[j].role = 3
+        assert (pheads(5, nj=3, kind=2), pbackward(5, nj=3, kind=2)) == (-3, -3)
+        jobs[j].role = role
+    assert (pheads(5, nj=3, kind=0), pbackward(5, nj=3, kind=0)) == (-3, -3)   # predicted normals, no normal head
+    jobs[1].light_mode = 1                                          # an indexed light without the ray table
+    assert pheads(5) == -3
+    jobs[1].light_mode = 2
+    w.x0[1] = None                                                  # the backward needs both x0 dumps
+    assert pbackward(5) == -1
+    w.x0[1] = 16
 
 
 def test_no_cpu_fallback():

@@ -27,7 +27,8 @@ Tolerances follow from the arithmetic, per entry, in float64:
 The reference functions themselves are pinned by ``test_stage_references_match_autograd_cpu``: chained, they equal
 torch autograd of the same head as an nn.Sequential in float64.
 
-The four-job backward is not checked here: its g_out comes from the tail kernels."""
+The four-job backward, whose g_out comes from the tail kernels, is checked by test_primary_kernels_fp64.py with
+Stages.data_grads and Stages.param_grads."""
 import ctypes as C
 import math
 
@@ -331,9 +332,19 @@ class Stages:
 
     def backward(self, what, g_outd, gz2, gz1, gfeat, gx0, grads, g_light_got=None, n_add_w=P_W):
         """grads: dict w0, b0, w1, b1, w2, b2, basis of the kernel (only this head's contributions)."""
-        n, act, W = self.n, self.act, self.W
+        a = self.data_grads(what, g_outd, gz2, gz1, gfeat, gx0)
+        want, bnds = self.param_grads(g_outd, gz2, gz1, gfeat, a, n_add_w)
+        if self.mode:
+            check(g_light_got, want["light"], bnds["light"] + 1e-30, f"{what}: d light_line")
+        for k in ("w0", "b0", "w1", "b1", "w2", "b2", "basis"):
+            check(grads[k], want[k], bnds[k] + 1e-30, f"{what}: d {k}")
+        return a
+
+    def data_grads(self, what, g_outd, gz2, gz1, gfeat, gx0):
+        """d z2, d z1, d feat and d x0 of the kernel against float64 from its own upstream dumps -> d (x0 * light)"""
+        act, W = self.act, self.W
         od = W[2].shape[0]
-        inp, h1, h2, x0, out = self.inp, self.h1, self.h2, self.x0, self.out[:, :od]
+        inp, h1, h2, out = self.inp, self.h1, self.h2, self.out[:, :od]
         gz3 = g_z3(g_outd[:, :od], out, act)
         gz3_mag = g_outd[:, :od].abs() * act_grad(out, act).abs()
         check(gz2, g_z2(gz3, W[2], h2), 8 * EPS32 * (gz3_mag @ W[2].abs()) * (h2 > 0) + 1e-30, f"{what}: d z2")
@@ -347,19 +358,16 @@ class Stages:
         e_a = gemm_bound(a_mag, 32)
         check(gx0, a * self.lrow, e_a * self.lrow_abs + EPS32 * (self.c_l + 1) * a_mag * self.lrow_abs + 1e-30,
               f"{what}: d x0")
-        if self.mode:
-            t_mag = a_mag * x0.abs()
-            want = g_light(a, x0, self.mode, self.light, self.L)
-            if self.mode == 1:
-                cnt = torch.bincount(self.light.long(), minlength=self.L).double()[:, None]
-                mag = torch.zeros(self.L, K0, dtype=torch.float64, device=DEV).index_add_(0, self.light.long(), t_mag)
-                emag = torch.zeros_like(mag).index_add_(0, self.light.long(), e_a * x0.abs())
-            else:
-                cnt = torch.full((self.L, 1), float(n), dtype=torch.float64, device=DEV)
-                mag = (t_mag.sum(0, keepdim=True) / self.L).expand(self.L, K0)
-                emag = ((e_a * x0.abs()).sum(0, keepdim=True) / self.L).expand(self.L, K0)
-            bnd = emag + mag * EPS32 * (18.0 + 4.0 * cnt.sqrt())
-            check(g_light_got, want, bnd + 1e-30, f"{what}: d light_line")
+        return a
+
+    def param_grads(self, g_outd, gz2, gz1, gfeat, a, n_add_w=P_W):
+        """float64 weight, bias, basis_mat and (light modes 1, 2) light_line gradients of this head and their bounds:
+        (want, bounds), two dicts, so the contributions of heads that share a parameter can be summed."""
+        n, act, W = self.n, self.act, self.W
+        od = W[2].shape[0]
+        inp, h1, h2, x0, out = self.inp, self.h1, self.h2, self.x0, self.out[:, :od]
+        gz3 = g_z3(g_outd[:, :od], out, act)
+        gz3_mag = g_outd[:, :od].abs() * act_grad(out, act).abs()
         xl = x0 * self.lrow
         xl_mag = x0.abs() * self.lrow_abs
         want = weight_grads(gz1, gz2, gz3, inp, h1, h2, gfeat, xl)
@@ -372,13 +380,27 @@ class Stages:
                     b2=sum_bound(sl(gz3_mag), n + n_add_w) + 4 * EPS32 * sl(gz3_mag),
                     basis=gemm_bound(gfeat.abs().t() @ xl_mag, n, n_add_w)
                     + EPS32 * self.c_l * (gfeat.abs().t() @ xl_mag))
-        for k in ("w0", "b0", "w1", "b1", "w2", "b2", "basis"):
-            check(grads[k], want[k], bnds[k] + 1e-30, f"{what}: d {k}")
-        return a
+        if self.mode:
+            a_mag = gfeat.abs() @ self.basis.abs()
+            e_a = gemm_bound(a_mag, 32)
+            t_mag = a_mag * x0.abs()
+            want["light"] = g_light(a, x0, self.mode, self.light, self.L)
+            if self.mode == 1:
+                cnt = torch.bincount(self.light.long(), minlength=self.L).double()[:, None]
+                mag = torch.zeros(self.L, K0, dtype=torch.float64, device=DEV).index_add_(0, self.light.long(), t_mag)
+                emag = torch.zeros_like(mag).index_add_(0, self.light.long(), e_a * x0.abs())
+            else:
+                cnt = torch.full((self.L, 1), float(n), dtype=torch.float64, device=DEV)
+                mag = (t_mag.sum(0, keepdim=True) / self.L).expand(self.L, K0)
+                emag = ((e_a * x0.abs()).sum(0, keepdim=True) / self.L).expand(self.L, K0)
+            bnds["light"] = emag + mag * EPS32 * (18.0 + 4.0 * cnt.sqrt())
+        return want, bnds
 
 
-def check_factor_grads(planes, lines, grid, xn, gx0, gp, gl, what):
-    """Appearance-factor gradients (channel-last, from the kernel) against a float64 scatter of the kernel's d x0."""
+def check_factor_grads(planes, lines, grid, xn, gx0, gp, gl, what, prefill=0.0):
+    """Appearance-factor gradients (channel-last, from the kernel) against a float64 scatter of the kernel's d x0.
+    ``prefill``: the value every gradient entry held before the kernel accumulated into it; its modulus joins the
+    magnitude of every entry, for the roundings of adding to it."""
     import test_vm_kernels_fp64 as V
     with V.f64():
         ps_ = [p.detach().double().clone().requires_grad_(True) for p in planes]
@@ -394,7 +416,9 @@ def check_factor_grads(planes, lines, grid, xn, gx0, gp, gl, what):
                       lambda k, t, j: ga[:, k] * t["ltaps"][j][1][:, None] * t["AP"], 48)
         u = V.scatter(tu, lambda k, t, j: ga[:, k] * t["ptaps"][j][1][:, None] * t["AL"],
                       lambda k, t, j: ga[:, k] * t["ltaps"][j][1][:, None] * t["AP"], 48)
-        V.check_scatter(gp, gl, [p.grad for p in ps_], [p.grad for p in ls_], m, u, what, grid)
+        m = [(mp + abs(prefill), ml + abs(prefill), cp, cl) for mp, ml, cp, cl in m]
+        V.check_scatter([g - prefill for g in gp], [g - prefill for g in gl], [p.grad for p in ps_],
+                        [p.grad for p in ls_], m, u, what, grid)
 
 
 def check_gather(planes, lines, grid, xn, x0, what):

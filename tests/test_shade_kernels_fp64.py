@@ -178,6 +178,7 @@ class Gates:
         amb = (v - lo).abs() <= x.e
         if hi != math.inf:
             amb |= (v - hi).abs() <= x.e
+        amb &= x.e > 0                          # an exact value takes the kernel's branch
         self.n[name] = self.n.get(name, 0) + int(amb.sum())
         while dec.dim() < _d(term.v).dim():
             dec, amb = dec[..., None], amb[..., None]
