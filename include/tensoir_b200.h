@@ -710,6 +710,60 @@ int tir_transport_build(const float* dirs, const float* domega /* [K] */, int32_
                         int64_t n, float acc_mask_threshold, const float* rescale /* [3] */, const int32_t* pos,
                         const float* vis_list, int32_t vis_kind, float* T /* [3,n,K] */, void* stream);
 
+/* ---- one bounce of indirect light for relighting under environment maps ----------------------------------------------
+ * For a hit primary ray i (acc > acc_mask_threshold) and map l:
+ *
+ *   linear[l,i] = (1/S)  * sum_s direct_s                  (exactly tir_relight_shade's sum, same order, same bits)
+ *               + (1/K)  * sum_k T[i,k] * w[i,k] * Lo[l, h(i,k)]
+ *   without_bg  = tone(linear),  with_bg = rl_composite(...)  (as tir_relight_shade)
+ *
+ * with K cosine-weighted directions per hit (Malley's method on lt_disc and lt_frame of the normalised normal), their
+ * throughput T = (albedo*rescale/pi + GGX) * cosine / pdf, the secondary march's occlusion weight w = 1 - vis, and Lo
+ * the un-toned direct light of map l at the secondary hit x = p + (depth / acc) * omega seen from -omega (definitions
+ * in csrc/tir_indirect_body.h).  One bounce only; cosine sampling only.  Around the existing calls:
+ *   tir_indirect_sample   per (ray, slot), u [n,K,2] fp64: dir [n,K,3], T [n,K,3] and pos [n,K] (secondary-list row or
+ *                         -1) for every slot (zeros and -1 on non-hit rays and on slots with cosine or z <= 1e-6); the
+ *                         marched slots' (surface point, direction) are appended to list_o / list_d; count and
+ *                         capacity as in tir_relight_sample.
+ *   tir_march_density     on the list, with relight()'s table: t_last, acc, depth per list row.
+ *   tir_indirect_hits     per slot, through pos: a secondary hit when w > 1e-3 and acc > 0, with w = 1 - t_last
+ *                         (vis_kind 0, nerv) or 1 - (1 - acc) (vis_kind 1, nerfactor).  The hits are compacted in slot
+ *                         order (a scan, not an append): hit_rays [m_h,6] = (x, omega), xn [m_h,3] = (x - aabb[0:3]) *
+ *                         aabb[3:6] - 1 (aabb: host [6] = lo, inverse half extent), w [m_h], hit [n,K] (row or -1).
+ *                         *count (device) is set to m_h; rows past capacity are not written (hit -1) but counted.
+ *                         work: tir_indirect_hits_work_size bytes of device scratch (TIR_ERR_CAPACITY when smaller).
+ *   tir_relight_sample    + tir_march_density on the hits (rays = hit_rays, depth 0), S2 samples per hit.
+ *   tir_indirect_radiance one warp per (map, hit): Lo[l, row0 + h] of [L, out_rows, 3] = mean over S2 of rl_contrib
+ *                         with the view direction -omega, un-toned; vis as in tir_relight_shade.
+ *   tir_indirect_shade    one warp per (map, ray): tir_relight_shade's outputs with the indirect sum added before the
+ *                         tone map on rays with at least one hit slot (other rows have tir_relight_shade's bits).
+ *                         Lo [L, m_h, 3]; indirect (NULL allowed) [L, out_rows, 3] receives the un-toned indirect term.
+ * Fixed-order sums and a stable hit list: repeated calls give identical bits.  TIR_ERR_SHAPE for n < 0, K outside
+ * [1, 1024], S2 outside [1, 1024], n*K > INT32_MAX, more than TIR_RELIGHT_MAX_LIGHTS maps, capacity outside
+ * [0, INT32_MAX], a stride other than 1 or 3 or output rows out of range; TIR_ERR_CONFIG for an unknown vis_kind. */
+int tir_indirect_sample(const float* rays, const float* depth, const float* normal, const float* albedo,
+                        const float* rough, int32_t rough_stride, const float* fresnel, const float* acc, int64_t n,
+                        int32_t K, float acc_mask_threshold, const float* rescale /* [3] */, const double* u,
+                        float* dir, float* T, int32_t* pos, float* list_o, float* list_d /* [capacity,3] */,
+                        int64_t capacity, int64_t* count, void* stream);
+int tir_indirect_hits_work_size(int64_t n, int32_t K, int64_t* bytes);
+int tir_indirect_hits(int64_t n, int32_t K, const int32_t* pos, const float* list_o, const float* list_d,
+                      const float* t_last, const float* acc, const float* depth, int32_t vis_kind,
+                      const float* aabb /* host [6] */, float* hit_rays, float* xn, float* w, int32_t* hit,
+                      int64_t capacity, int64_t* count, void* work, int64_t work_bytes, void* stream);
+int tir_indirect_radiance(const TirEnvMap* envs, int32_t n_lights, const float* hit_rays, const float* normal,
+                          const float* albedo, const float* rough, int32_t rough_stride, const float* fresnel,
+                          int64_t m, int32_t n_samples, const float* rescale, const int32_t* bin, const int32_t* pos,
+                          const float* vis_list, int32_t vis_kind, float* Lo, int64_t out_rows, int64_t row0,
+                          void* stream);
+int tir_indirect_shade(const TirEnvMap* envs, int32_t n_lights, const float* rays, const float* normal,
+                       const float* albedo, const float* rough, int32_t rough_stride, const float* fresnel,
+                       const float* acc, int64_t n, int32_t n_samples, float acc_mask_threshold,
+                       const float* rescale, const int32_t* bin, const int32_t* pos, const float* vis_list,
+                       int32_t vis_kind, int32_t K, const float* T, const int32_t* hit, const float* w,
+                       const float* Lo, int64_t m_h, float* with_bg, float* without_bg, float* indirect,
+                       int64_t out_rows, int64_t row0, void* stream);
+
 /* ---- mesh export: marching cubes over a dense volume (utils.py:165-225, skimage.measure.marching_cubes on
  * TensorBase.getDenseAlpha(), tensorBase_rotated_lights.py:737-753) ---------------------------------------------------
  * volume [X,Y,Z] fp32 C-contiguous, X, Y, Z >= 2 and X*Y*Z <= INT32_MAX (TIR_ERR_SHAPE otherwise).  A point is inside

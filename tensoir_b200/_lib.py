@@ -260,6 +260,20 @@ EXPORTS = {
                                        f32p, f32p, C.c_int64, C.c_void_p, C.c_void_p]),
     "tir_transport_build": (C.c_int, [f32p, f32p, C.c_int32, f32p, f32p, f32p, f32p, C.c_int32, f32p, f32p, C.c_int64,
                                       C.c_float, f32p, C.c_void_p, f32p, C.c_int32, f32p, C.c_void_p]),
+    "tir_indirect_sample": (C.c_int, [f32p, f32p, f32p, f32p, f32p, C.c_int32, f32p, f32p, C.c_int64, C.c_int32,
+                                      C.c_float, f32p, C.c_void_p, f32p, f32p, C.c_void_p, f32p, f32p, C.c_int64,
+                                      C.c_void_p, C.c_void_p]),
+    "tir_indirect_hits_work_size": (C.c_int, [C.c_int64, C.c_int32, C.POINTER(C.c_int64)]),
+    "tir_indirect_hits": (C.c_int, [C.c_int64, C.c_int32, C.c_void_p, f32p, f32p, f32p, f32p, f32p, C.c_int32,
+                                    C.POINTER(C.c_float), f32p, f32p, f32p, C.c_void_p, C.c_int64, C.c_void_p,
+                                    C.c_void_p, C.c_int64, C.c_void_p]),
+    "tir_indirect_radiance": (C.c_int, [C.POINTER(TirEnvMap), C.c_int32, f32p, f32p, f32p, f32p, C.c_int32, f32p,
+                                        C.c_int64, C.c_int32, f32p, C.c_void_p, C.c_void_p, f32p, C.c_int32, f32p,
+                                        C.c_int64, C.c_int64, C.c_void_p]),
+    "tir_indirect_shade": (C.c_int, [C.POINTER(TirEnvMap), C.c_int32, f32p, f32p, f32p, f32p, C.c_int32, f32p, f32p,
+                                     C.c_int64, C.c_int32, C.c_float, f32p, C.c_void_p, C.c_void_p, f32p, C.c_int32,
+                                     C.c_int32, f32p, C.c_void_p, f32p, f32p, C.c_int64, f32p, f32p, f32p, C.c_int64,
+                                     C.c_int64, C.c_void_p]),
     "tir_marching_cubes_work_size": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int64)]),
     "tir_marching_cubes_count": (C.c_int, [f32p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_int64,
                                            C.c_void_p, C.c_void_p]),
@@ -282,7 +296,9 @@ KERNELS_PER_CALL = {"tir_pack_channels_last": 1, "tir_unpack_channels_last_add":
                     "tir_composite_bwd": 1, "tir_tail_fwd": 1, "tir_tail_bwd": 1, "tir_epilogue_fwd": 1,
                     "tir_epilogue_bwd": 1, "tir_eval_view": 3, "tir_relight_sample": 1, "tir_relight_shade": 1,
                     "tir_material_edit": 1, "tir_lights_sample": 1, "tir_lights_shade": 1,
-                    "tir_transport_sample": 1, "tir_transport_build": 1, "tir_marching_cubes_count": 7, "tir_marching_cubes_emit": 2}
+                    "tir_transport_sample": 1, "tir_transport_build": 1,
+                    "tir_indirect_sample": 1, "tir_indirect_hits": 3, "tir_indirect_radiance": 1,
+                    "tir_indirect_shade": 1, "tir_marching_cubes_count": 7, "tir_marching_cubes_emit": 2}
 launch_count = 0
 
 _lib = None

@@ -106,16 +106,7 @@ __global__ void __launch_bounds__(kWarps * 32) relight_shade_kernel(const ShadeP
              p.fresnel + i * 3, resc, c);
     float acc[3] = {0.f, 0.f, 0.f};
     const int64_t k0 = w * p.S;
-    for (int s = lane; s < p.S; s += 32) {
-      const int b = p.bin[k0 + s];
-      const int q = p.pos[k0 + s];
-      float vis = 0.f;
-      if (q >= 0) vis = p.vis_kind ? 1.f - p.vis[q] : p.vis[q];
-      float Ld[3], rgb[3];
-#pragma unroll
-      for (int ch = 0; ch < 3; ++ch) { Ld[ch] = __ldg(e.dir + (int64_t)b * 3 + ch); rgb[ch] = __ldg(e.rgb + (int64_t)b * 3 + ch); }
-      rl_contrib(c, Ld, rgb, __ldg(e.pdf_return + b), vis, acc);
-    }
+    rl_direct_lane(e, c, p.bin + k0, p.pos + k0, p.vis, p.vis_kind, p.S, lane, 32, acc);
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) wo[ch] = tone(warp_sum(acc[ch]) / (float)p.S, 1);
   }

@@ -86,6 +86,29 @@ RL_HD void rl_contrib(const tir::PointCtx& c, const float L[3], const float rgb[
   }
 }
 
+#if defined(__CUDA_ARCH__)
+#define RL_LDG(p) __ldg(p)
+#else
+#define RL_LDG(p) (*(p))
+#endif
+
+// The direct per-sample loop of one (map, point): lane `lane` of `lanes` adds rl_contrib of samples lane, lane + lanes,
+// ... (bin and list row from bin[] / pos[], vis as relight() reads it from the march) to acc[3].  The kernels run it on
+// the 32 lanes of a warp and reduce with warp_sum; the host builds run the 32 lanes in turn and reduce with the same
+// xor butterfly.
+RL_HD void rl_direct_lane(const TirEnvMap& e, const tir::PointCtx& c, const int32_t* bin, const int32_t* pos,
+                          const float* vis_list, int vis_kind, int S, int lane, int lanes, float acc[3]) {
+  for (int s = lane; s < S; s += lanes) {
+    const int b = bin[s];
+    const int q = pos[s];
+    float vis = 0.f;
+    if (q >= 0) vis = vis_kind ? 1.f - vis_list[q] : vis_list[q];
+    float Ld[3], rgb[3];
+    for (int ch = 0; ch < 3; ++ch) { Ld[ch] = RL_LDG(e.dir + (int64_t)b * 3 + ch); rgb[ch] = RL_LDG(e.rgb + (int64_t)b * 3 + ch); }
+    rl_contrib(c, Ld, rgb, RL_LDG(e.pdf_return + b), vis, acc);
+  }
+}
+
 // Composite of one output row (:167-181): without_bg (already toned, or white), background, acc threshold 0.9
 RL_HD void rl_composite(const TirEnvMap& e, const float* ray, float acc, const float wo[3], float with_bg[3]) {
   float bg[3];

@@ -112,10 +112,22 @@ def relight_chunk_fused(tensoIR, envir_light, light_names, rays, maps, rescale_v
     return with_bg[:, row0:row0 + n], without_bg[:, row0:row0 + n]
 
 
-def relight_visibility(tensoIR, envs, L, rays, depth, normal, acc, u, num_samples, acc_mask_threshold, vis_equation):
+def slot_order(pos, list_o, list_d):
+    """Rewrite a list appended in warp-scheduling order into slot order, in place of pos: the density march's result
+    for a ray can change in its last bits with the rays next to it in the list, so this makes the march, and what
+    reads it, reproducible.  -> (list_o, list_d) of the marched rows."""
+    sel = pos >= 0
+    rows = pos[sel].long()
+    pos[sel] = torch.arange(rows.numel(), dtype=pos.dtype, device=pos.device)
+    return list_o[rows], list_d[rows]
+
+
+def relight_visibility(tensoIR, envs, L, rays, depth, normal, acc, u, num_samples, acc_mask_threshold, vis_equation,
+                       ordered=False):
     """The material-independent half of relight_chunk_fused for up to RELIGHT_MAX_LIGHTS maps (``envs``, L entries):
     tir_relight_sample, the read-back of the list length and the density march on the list.  Inputs are contiguous
-    fp32 (u fp64 [L, n, S]) device tensors.  -> (bins, pos, vis), what relight_shade reads."""
+    fp32 (u fp64 [L, n, S]) device tensors.  ``ordered``: march the list in slot order (slot_order).
+    -> (bins, pos, vis), what relight_shade reads."""
     lib = _lib.load()
     dev = rays.device
     n, S = int(rays.shape[0]), int(num_samples)
@@ -134,6 +146,8 @@ def relight_visibility(tensoIR, envs, L, rays, depth, normal, acc, u, num_sample
     if m > cap:
         raise _lib.TirError(f"relight visibility list overflow: {m} > {cap}")
     if m > 0:
+        if ordered:
+            list_o, list_d = slot_order(pos, list_o[:m], list_d[:m])
         table = ops.equal_z_table(96, 0.05, 1.5, dev)
         t_last, acc_s, _ = ops.march_density(tensoIR, list_o[:m], list_d[:m], table=table,
                                              counters=tensoIR.__dict__.get("_tir_counters"))
@@ -227,7 +241,10 @@ def relight(dataset, args, tensoIR=None, *, rescale_value=None):
     (rays, rgbs [L, H*W, 3], rgbs_mask, albedo, ...) with ``split`` and ``light_names``; ``args`` needs ckpt (when
     ``tensoIR`` is None), hdrdir, geo_buffer_path and batch_size; the script-only flags default to SCRIPT_DEFAULTS.
     ``rescale_value``: the albedo rescale ratio [3] to shade with; None computes it from ``dataset``
-    (compute_rescale_ratio), as the reference does."""
+    (compute_rescale_ratio), as the reference does.
+    Indirect light (indirect.py) is read from ``args`` too: ``indirect_samples`` K (0, the default, shades direct light
+    only), ``indirect_light_samples`` S2 (32), ``indirect_seed`` (lighting.SEED) and ``save_indirect``, which also
+    writes the linear indirect-only image of every map as {view}/relighting_indirect/{light}.hdr."""
     from .relight import Environment_Light
     opt = {k: getattr(args, k, v) for k, v in SCRIPT_DEFAULTS.items()}
     device = torch.device("cuda")
@@ -249,6 +266,17 @@ def relight(dataset, args, tensoIR=None, *, rescale_value=None):
         _, rescale_value = compute_rescale_ratio(tensoIR, dataset)
     rescale_value = torch.as_tensor(rescale_value, dtype=torch.float32).to(device)
 
+    # one bounce of indirect light (indirect.py): off unless indirect_samples > 0
+    n_ind = int(getattr(args, "indirect_samples", 0) or 0)
+    save_ind = n_ind > 0 and bool(getattr(args, "save_indirect", False))
+    if n_ind > 0:
+        from .indirect import relight_chunk_indirect
+        from .lighting import SEED
+        seed = getattr(args, "indirect_seed", None)
+        gen = torch.Generator(device).manual_seed(SEED if seed is None else int(seed))
+        ind_kw = dict(indirect_samples=n_ind, indirect_light_samples=int(getattr(args, "indirect_light_samples", 32)
+                                                                           or 32))
+
     psnr, ssim, l_alex, l_vgg = ({n: [] for n in names} for _ in range(4))
     rgb_frames, aligned_albedo_list, roughness_list = [], [], []
     gp = args.geo_buffer_path
@@ -265,6 +293,7 @@ def relight(dataset, args, tensoIR=None, *, rescale_value=None):
 
         with_map = torch.empty(L, n_pix, 3, device=device)
         without_map = torch.empty(L, n_pix, 3, device=device)
+        ind_map = torch.empty(L, n_pix, 3, device=device) if save_ind else None
         prim = {}
         for s in range(0, n_pix, args.batch_size):
             e = min(s + args.batch_size, n_pix)
@@ -278,9 +307,15 @@ def relight(dataset, args, tensoIR=None, *, rescale_value=None):
                     prim[k] = torch.empty((n_pix,) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
                 prim[k][s:e] = t
             u = _uniforms(L, e - s, NUM_SAMPLES, device)
-            relight_chunk_fused(tensoIR, envir_light, names, rays, (depth, normal, albedo, rough, fresnel, acc),
-                                rescale_value, u, NUM_SAMPLES, thr, opt["vis_equation"], out=(with_map, without_map),
-                                row0=s, tables=tables)
+            if n_ind > 0:
+                relight_chunk_indirect(tensoIR, envir_light, names, rays, (depth, normal, albedo, rough, fresnel, acc),
+                                       rescale_value, u, gen, **ind_kw, acc_mask_threshold=thr,
+                                       vis_equation=opt["vis_equation"], out=(with_map, without_map), row0=s,
+                                       tables=tables, indirect_out=ind_map)
+            else:
+                relight_chunk_fused(tensoIR, envir_light, names, rays, (depth, normal, albedo, rough, fresnel, acc),
+                                    rescale_value, u, NUM_SAMPLES, thr, opt["vis_equation"],
+                                    out=(with_map, without_map), row0=s, tables=tables)
 
         # metrics of every map against its ground truth (:212-226): the image without background
         met = pair_metrics(without_map, gt_rgb, H, W).cpu().numpy()
@@ -299,6 +334,12 @@ def relight(dataset, args, tensoIR=None, *, rescale_value=None):
             for k, name in enumerate(names):
                 _imwrite(os.path.join(cur_dir_path, 'relighting_with_bg', f'{name}.png'), u8w[k])
                 _imwrite(os.path.join(cur_dir_path, 'relighting_without_bg', f'{name}.png'), u8o[k])
+        if save_ind:
+            from .relight import write_hdr
+            os.makedirs(os.path.join(cur_dir_path, 'relighting_indirect'), exist_ok=True)
+            ind_np = ind_map.reshape(L, H, W, 3).cpu().numpy()
+            for k, name in enumerate(names):
+                write_hdr(os.path.join(cur_dir_path, 'relighting_indirect', f'{name}.hdr'), ind_np[k])
         with open(os.path.join(cur_dir_path, 'relighting_without_bg', 'relight_psnr.txt'), 'w') as f:
             for name in names:
                 f.write(f'{name}: PNSR {psnr[name][-1]}; SSIM {ssim[name][-1]}; L_Alex {l_alex[name][-1]}; '

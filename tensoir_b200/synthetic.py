@@ -45,9 +45,10 @@ def _lego_boxes():
 
 
 def box_density_factors(grid_size: Sequence[int], aabb: torch.Tensor, n_comp: Sequence[int] = (16, 16, 16),
-                        amplitude: float = 30.0, noise: float = 1e-3, generator=None):
+                        amplitude: float = 30.0, noise: float = 1e-3, generator=None, boxes=None):
     """Return (planes, lines) in the reference layout: plane k [1,C,G[m1],G[m0]], line k
-    [1,C,G[v],1] (tensoRF_rotated_lights.py:19-29)."""
+    [1,C,G[v],1] (tensoRF_rotated_lights.py:19-29).  ``boxes``: (lo_xyz, hi_xyz, orientation) list, default the lego
+    scene's."""
     g = torch.Generator().manual_seed(SEED + 7) if generator is None else generator
     lo, hi = aabb[0].tolist(), aabb[1].tolist()
     coords = [torch.linspace(lo[a], hi[a], int(grid_size[a])) for a in range(3)]
@@ -58,7 +59,7 @@ def box_density_factors(grid_size: Sequence[int], aabb: torch.Tensor, n_comp: Se
         v = VEC_MODE[k]
         planes.append(noise * torch.randn((1, n_comp[k], int(grid_size[m1]), int(grid_size[m0])), generator=g))
         lines.append(noise * torch.randn((1, n_comp[k], int(grid_size[v]), 1), generator=g))
-    for (blo, bhi, k) in _lego_boxes():
+    for (blo, bhi, k) in (_lego_boxes() if boxes is None else boxes):
         c = used[k]
         if c >= n_comp[k]:
             continue

@@ -5,6 +5,10 @@ tools/dropin_train_check.py:
 
     PYTHONPATH=<TensoIR checkout>:. python tools/relight_importance.py --config <config> --ckpt <ckpt> \\
         --hdrdir <dir of .hdr maps> --geo_buffer_path <out dir>
+
+``--indirect_samples K`` adds one bounce of indirect light with K directions per surface hit (default 0: direct light
+only, the reference's estimator), ``--indirect_light_samples S2`` sets the light samples per secondary hit (default 32)
+and ``--save_indirect 1`` also writes the linear indirect-only images.
 """
 import os
 import sys
@@ -15,8 +19,24 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.append(ROOT)
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from relight_lights import pop_option  # noqa: E402
+
+
+def indirect_options(argv):
+    """Remove the indirect-light flags from argv (opt.config_parser does not know them) -> dict of the args
+    attributes relight() reads: --indirect_samples K (0: direct light only), --indirect_light_samples S2 (32),
+    --save_indirect 1 (also write relighting_indirect/{light}.hdr)."""
+    k = pop_option(argv, "--indirect_samples", int)
+    s2 = pop_option(argv, "--indirect_light_samples", int)
+    save = pop_option(argv, "--save_indirect", int)
+    return dict(indirect_samples=k or 0, indirect_light_samples=32 if s2 is None else s2,
+                save_indirect=bool(save))
+
 
 if __name__ == "__main__":
+    indirect = indirect_options(sys.argv)
+
     from dataLoader import dataset_dict
     from opt import config_parser
 
@@ -44,6 +64,8 @@ if __name__ == "__main__":
     args.if_render_normal = True
     args.vis_equation = 'nerv'
     args.render_video = True
+    for k, v in indirect.items():
+        setattr(args, k, v)
 
     dataset = dataset_dict[args.dataset_name]
     # names of the environment maps used for relighting
