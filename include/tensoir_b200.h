@@ -782,6 +782,28 @@ int tir_marching_cubes_emit(const float* volume, int32_t X, int32_t Y, int32_t Z
                             double sz, const void* work, int64_t work_bytes, int64_t n_verts, int64_t n_faces,
                             float* verts, int32_t* faces, void* stream);
 
+/* ---- textured glTF export: the texture atlas of a marching-cubes mesh (tensoir_b200/gltf.py) -----------------------
+ * faces [F,3] int32 in marching_cubes' winding (reversed here, as the PLY writes them), v [V,3] fp32 the field
+ * positions of the vertices, a T x T atlas (T a power of two in [256, 8192]) of s x s cells (s in [6, 64],
+ * floor(T/s)^2 >= ceil(F/2)); the layout, the no-bleed guarantee, the probe points, the tangent frames and the
+ * encoding are documented in csrc/tir_atlas_body.h.  Texels are numbered face-major, F * s(s-1)/2 in all (int64).
+ *   tir_atlas_texels   texels [first, first+n): pix [n] int32 = row * T + column, pos [n,3] fp32 the texel's point on
+ *                      its face (clamped barycentrics of its corners' v);
+ *   tir_atlas_encode   the same texels with their probe results (albedo [n,3], rough [n], normal [n,3], probed [n]
+ *                      uint8): one RGBA8 word per texel into base_color, metallic_roughness and normal_map [T,T,4];
+ *                      other texels are not written;
+ *   tir_atlas_corners  per face corner, unwelded (row 3f+k = corner k of face f): position [3F,3] = v, normal [3F,3]
+ *                      and tangent [3F,4] the face's frame, texcoord [3F,2] its UV.
+ * One thread per texel / face, no atomics: repeated calls give identical bits.  n = 0 (F = 0 for the corners) is a
+ * no-op; TIR_ERR_SHAPE for a negative size, a layout outside the ranges above or a texel range past the last texel. */
+int tir_atlas_texels(const int32_t* faces, int64_t n_faces, const float* v, int32_t T, int32_t s, int64_t first,
+                     int64_t n, int32_t* pix, float* pos, void* stream);
+int tir_atlas_encode(const int32_t* faces, int64_t n_faces, const float* v, int32_t T, int32_t s, int64_t first,
+                     int64_t n, const float* albedo, const float* rough, const float* normal, const uint8_t* probed,
+                     uint8_t* base_color, uint8_t* metallic_roughness, uint8_t* normal_map, void* stream);
+int tir_atlas_corners(const int32_t* faces, int64_t n_faces, const float* v, int32_t T, int32_t s, float* position,
+                      float* normal, float* tangent, float* texcoord, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -280,6 +280,12 @@ EXPORTS = {
     "tir_marching_cubes_emit": (C.c_int, [f32p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_double, C.c_double,
                                           C.c_double, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, f32p, C.c_void_p,
                                           C.c_void_p]),
+    "tir_atlas_texels": (C.c_int, [C.c_void_p, C.c_int64, f32p, C.c_int32, C.c_int32, C.c_int64, C.c_int64, C.c_void_p,
+                                   f32p, C.c_void_p]),
+    "tir_atlas_encode": (C.c_int, [C.c_void_p, C.c_int64, f32p, C.c_int32, C.c_int32, C.c_int64, C.c_int64, f32p, f32p,
+                                   f32p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "tir_atlas_corners": (C.c_int, [C.c_void_p, C.c_int64, f32p, C.c_int32, C.c_int32, f32p, f32p, f32p, f32p,
+                                    C.c_void_p]),
 }
 
 # kernels launched per entry point (for bench.py's gpu_launches claim)
@@ -298,7 +304,8 @@ KERNELS_PER_CALL = {"tir_pack_channels_last": 1, "tir_unpack_channels_last_add":
                     "tir_material_edit": 1, "tir_lights_sample": 1, "tir_lights_shade": 1,
                     "tir_transport_sample": 1, "tir_transport_build": 1,
                     "tir_indirect_sample": 1, "tir_indirect_hits": 3, "tir_indirect_radiance": 1,
-                    "tir_indirect_shade": 1, "tir_marching_cubes_count": 7, "tir_marching_cubes_emit": 2}
+                    "tir_indirect_shade": 1, "tir_marching_cubes_count": 7, "tir_marching_cubes_emit": 2,
+                    "tir_atlas_texels": 1, "tir_atlas_encode": 1, "tir_atlas_corners": 1}
 launch_count = 0
 
 _lib = None

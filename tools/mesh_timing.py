@@ -1,6 +1,6 @@
 """Time the native mesh export on the 300^3 synthetic lego scene and print one JSON line.
 
-    python tools/mesh_timing.py [--grid 300] [--reps 20] [--host] [--asset]
+    python tools/mesh_timing.py [--grid 300] [--reps 20] [--host] [--asset] [--glb]
 
 Reports getDenseAlpha, the marching-cubes calls (tir_marching_cubes_count + _emit, CUDA events over repeated
 launches after warm-up, outputs preallocated: the calls are issued back to back, so host launch overhead can show in
@@ -12,7 +12,10 @@ CPU build, not the reference (whose skimage path is not measured here).  --asset
 mesh.export_asset on the same model, three runs after a warm-up, each step synchronised, wall clock, with each run's
 total: the surface (getDenseAlpha and the two marching-cubes calls), the derived normals at the vertices, the probe
 forward, the record packing with its device-to-host copy, the PLY write, the environment maps with their .hdr writes;
-plus V and the unprobed count.  Compiled artefacts and written files go to a temporary directory.
+plus V and the unprobed count.  --glb times gltf.export_asset_glb's steps the same way (T = 4096, one warm-up and
+three timed runs): the surface, then summed over the texel chunks the texels, their derived normals, the probe forward
+and the encode, then the corners, the device-to-host copy, the PNG encode and the .glb write; plus F, the texel count,
+the unprobed count and the file size.  Compiled artefacts and written files go to a temporary directory.
 """
 import argparse
 import ctypes as C
@@ -110,12 +113,58 @@ def _asset_timing(model, tmp, runs=3):
                 probe_offset=mesh.probe_offset(model))
 
 
+def _glb_timing(model, tmp, T=4096, runs=3):
+    """gltf.export_asset_glb's steps in its order (the .glb written without fsync, no .hdr files: --asset times
+    those), after one warm-up run: per timed run the wall time of each step, each synchronised before and after, the
+    per-chunk steps summed over the chunks, and of the whole run"""
+    from tensoir_b200 import gltf, mesh
+    path = os.path.join(tmp, "lego_asset.glb")
+    out = []
+    for _ in range(runs + 1):
+        t = dict.fromkeys(("texels_ms", "texel_normals_ms", "probe_forward_ms", "encode_ms"), 0.0)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        (_, faces, v), t["surface_ms"] = _wall(lambda: mesh.asset_surface(model))
+        F = int(faces.shape[0])
+        s = gltf.atlas_cell_size(F, T)
+        total, unprobed = gltf.texel_count(F, s), 0
+        images = gltf.new_images(T, v.device)
+        for first in range(0, total, gltf.TEXEL_CHUNK):
+            n = min(gltf.TEXEL_CHUNK, total - first)
+            (_, pos), dt = _wall(lambda: gltf.atlas_texels(faces, v, T, s, first, n))
+            t["texels_ms"] += dt
+            nrm, dt = _wall(lambda: mesh.vertex_normals(model, pos))
+            t["texel_normals_ms"] += dt
+            p, dt = _wall(lambda: mesh.probe(model, pos, nrm))
+            t["probe_forward_ms"] += dt
+            _, dt = _wall(lambda: gltf.atlas_encode(faces, v, T, s, first, p["albedo"], p["roughness"], p["normal"],
+                                                    p["probed"], images))
+            t["encode_ms"] += dt
+            unprobed += n - int(p["probed"].sum())
+        corners, t["corners_ms"] = _wall(lambda: gltf.atlas_corners(faces, v, T, s))
+        (host, imgs), t["d2h_ms"] = _wall(lambda: ({k: c.cpu().numpy() for k, c in corners.items()},
+                                                   images.cpu().numpy()))
+        pngs, t["png_encode_ms"] = _wall(lambda: [gltf.png_bytes(im) for im in imgs])
+
+        def write():
+            with open(path, "wb") as f:
+                f.write(gltf.glb_bytes(host, pngs))
+        _, t["glb_write_ms"] = _wall(write)
+        for k in ("texels_ms", "texel_normals_ms", "probe_forward_ms", "encode_ms"):
+            t[k] = round(t[k], 3)
+        t["total_ms"] = round((time.perf_counter() - t0) * 1e3, 3)
+        out.append(t)
+    return dict(runs=out[1:], texture_size=T, cell=s, F=F, texels=total, unprobed=unprobed,
+                glb_bytes=os.path.getsize(path), png_bytes=[len(q) for q in pngs])
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--grid", type=int, default=300)
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--host", action="store_true")
     ap.add_argument("--asset", action="store_true")
+    ap.add_argument("--glb", action="store_true")
     a = ap.parse_args()
     from tensoir_b200 import _lib, mesh
     from tensoir_b200.synthetic import make_lego_model
@@ -182,6 +231,7 @@ def main():
             host_ms = (time.perf_counter() - t0) * 1e3
             assert torch.equal(torch.from_numpy(hv), verts.cpu()) and torch.equal(torch.from_numpy(hf), faces.cpu())
         asset = _asset_timing(model, tmp) if a.asset else None
+        glb = _glb_timing(model, tmp) if a.glb else None
     name, power = _card()
     vol_bytes = X * Y * Z * 4
     print(json.dumps(dict(
@@ -191,7 +241,7 @@ def main():
         ply_bytes=len(body_dev), volume_bytes=vol_bytes,
         mc_volume_read_GBps=round(vol_bytes / (t_both * 1e-3) / 1e9, 1),
         mc_kernels_ms=kernels, mc_kernels_total_ms=round(sum(kernels.values()), 4),
-        host_build_ms=None if host_ms is None else round(host_ms, 1), asset=asset)))
+        host_build_ms=None if host_ms is None else round(host_ms, 1), asset=asset, glb=glb)))
 
 
 if __name__ == "__main__":
