@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define TIR_ABI_VERSION 3
+#define TIR_ABI_VERSION 4
 
 typedef enum TirStatus {
   TIR_OK = 0,
@@ -481,19 +481,21 @@ int tir_primary_radiance_backward(const TirField* field, const TirHeadJob* job, 
 /* ---- optimiser pass (SURVEY.md 8 f3): torch.optim.Adam's update for a list of dense fp32 tensors in ONE launch, with
  * the L1 regulariser's gradient (l1 * sign(param), density_L1 of tensoRF_rotated_lights.py:74-78) folded in, the
  * gradient cleared for the next accumulation, and a device-side skip flag (found_inf != 0: parameters, moments and the
- * step counter stay untouched, gradients are still cleared).  table / chunk_prefix / state live in device memory:
- * chunk_prefix[k] = first chunk (of tir_adam_chunk_elems() elements) of tensor k, state = {step, 1-beta1^t,
- * sqrt(1-beta2^t), skipped}. */
+ * step counts stay untouched, gradients are still cleared).  Every tensor has its own step count (torch.optim.Adam's
+ * per-parameter state["step"]), advanced by one per call.  table / chunk_prefix / bias live in device memory:
+ * chunk_prefix[k] = first chunk (of tir_adam_chunk_elems() elements) of tensor k; bias: 2 * n_tensors floats of scratch
+ * (tensor k's 1-beta1^t and sqrt(1-beta2^t)). */
 typedef struct TirAdamTensor {
   float* p; float* g; float* m; float* v;   /* parameter, gradient, exp_avg, exp_avg_sq: same dense layout, n elements */
   int64_t n;
   const float* lr_dev;                      /* learning rate in device memory (CUDA-graph replay), or NULL -> lr */
   float lr;
   float l1;                                 /* coefficient of sign(param) added to the gradient (0: none) */
+  float* step;                              /* this tensor's step count: one float in device memory */
 } TirAdamTensor;
 int tir_adam_chunk_elems(void);
 int tir_adam_step(const TirAdamTensor* table_dev, int32_t n_tensors, const int64_t* chunk_prefix_dev,
-                  int64_t total_chunks, float* state_dev, float beta1, float beta2, float eps,
+                  int64_t total_chunks, float* bias_dev, float beta1, float beta2, float eps,
                   const float* found_inf_dev, int32_t clear_grad, void* stream);
 
 /* Total-variation regulariser of up to TIR_TV_MAX_PLANES VM planes in one launch (SURVEY.md 8 f3): TVLoss (utils.py:143-162)

@@ -14,7 +14,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("TIR_LIB") or os.path.join(_HERE, "lib", "libtensoir_b200.so")   # TIR_LIB: A/B builds
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 CNT_MASK, CNT_DENSITY, CNT_APP, CNT_RAYS, CNT_OVERFLOW, CNT_SLOTS = 0, 1, 2, 3, 4, 8
 SAMPLE_STEP, SAMPLE_TABLE = 0, 1
 
@@ -60,7 +60,7 @@ MARCH_CELL_BRICKS = 4
 
 class TirAdamTensor(C.Structure):
     _fields_ = [("p", C.c_void_p), ("g", C.c_void_p), ("m", C.c_void_p), ("v", C.c_void_p), ("n", C.c_int64),
-                ("lr_dev", C.c_void_p), ("lr", C.c_float), ("l1", C.c_float)]
+                ("lr_dev", C.c_void_p), ("lr", C.c_float), ("l1", C.c_float), ("step", C.c_void_p)]
 
 
 class TirTvPlane(C.Structure):

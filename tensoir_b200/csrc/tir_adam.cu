@@ -13,22 +13,23 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kChunk = kThreads * 16;      // elements per CTA
 
-__global__ void adam_prologue_kernel(float* state, float beta1, float beta2, const float* found_inf) {
-  // state: [0] step, [1] 1 - beta1^step, [2] sqrt(1 - beta2^step), [3] skip flag
-  const bool skip = found_inf && found_inf[0] != 0.f;
-  if (!skip) {
-    const float step = state[0] + 1.f;
-    state[0] = step;
-    state[1] = 1.f - powf(beta1, step);
-    state[2] = sqrtf(1.f - powf(beta2, step));
-  }
-  state[3] = skip ? 1.f : 0.f;
+// Per-tensor step counts, as torch.optim.Adam keeps them (state["step"] of each parameter): every table entry's counter
+// advances by one unless found_inf is set, and its bias corrections go to bias[k] = {1 - beta1^t, sqrt(1 - beta2^t)}.
+__global__ void adam_prologue_kernel(const TirAdamTensor* __restrict__ table, int n_tensors, float2* __restrict__ bias,
+                                     float beta1, float beta2, const float* __restrict__ found_inf) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n_tensors || (found_inf && found_inf[0] != 0.f)) return;
+  float* counter = table[k].step;
+  const float step = counter[0] + 1.f;
+  counter[0] = step;
+  bias[k] = make_float2(1.f - powf(beta1, step), sqrtf(1.f - powf(beta2, step)));
 }
 
 __global__ void __launch_bounds__(kThreads) adam_main_kernel(const TirAdamTensor* __restrict__ table, int n_tensors,
                                                              const int64_t* __restrict__ chunk_prefix,
-                                                             const float* __restrict__ state, float beta1, float beta2,
-                                                             float eps, int clear_grad) {
+                                                             const float2* __restrict__ bias,
+                                                             const float* __restrict__ found_inf, float beta1,
+                                                             float beta2, float eps, int clear_grad) {
   // which tensor does this chunk belong to
   const int64_t chunk = blockIdx.x;
   int lo = 0, hi = n_tensors - 1;
@@ -38,8 +39,9 @@ __global__ void __launch_bounds__(kThreads) adam_main_kernel(const TirAdamTensor
   }
   const TirAdamTensor t = table[lo];
   const int64_t base = (chunk - chunk_prefix[lo]) * kChunk;
-  const bool skip = state[3] != 0.f;
-  const float bc1 = state[1], bc2s = state[2];
+  const bool skip = found_inf && found_inf[0] != 0.f;
+  const float2 bc = skip ? make_float2(1.f, 1.f) : bias[lo];
+  const float bc1 = bc.x, bc2s = bc.y;
   const float lr = t.lr_dev ? t.lr_dev[0] : t.lr;
   const float step_size = lr / bc1;
   const bool vec = ((reinterpret_cast<uintptr_t>(t.p) | reinterpret_cast<uintptr_t>(t.g) | reinterpret_cast<uintptr_t>(t.m) |
@@ -98,13 +100,18 @@ __global__ void __launch_bounds__(kThreads) adam_main_kernel(const TirAdamTensor
 extern "C" int tir_adam_chunk_elems(void) { return kChunk; }
 
 extern "C" int tir_adam_step(const TirAdamTensor* table_dev, int32_t n_tensors, const int64_t* chunk_prefix_dev,
-                             int64_t total_chunks, float* state_dev, float beta1, float beta2, float eps,
+                             int64_t total_chunks, float* bias_dev, float beta1, float beta2, float eps,
                              const float* found_inf_dev, int32_t clear_grad, void* stream_) {
-  if (n_tensors <= 0 || total_chunks <= 0) return TIR_OK;
-  if (!table_dev || !chunk_prefix_dev || !state_dev) return TIR_ERR_NULL;
+  if (n_tensors <= 0) return TIR_OK;
+  if (!table_dev || !chunk_prefix_dev || !bias_dev) return TIR_ERR_NULL;
   cudaStream_t stream = (cudaStream_t)stream_;
-  adam_prologue_kernel<<<1, 1, 0, stream>>>(state_dev, beta1, beta2, found_inf_dev);
-  adam_main_kernel<<<(unsigned)total_chunks, kThreads, 0, stream>>>(table_dev, n_tensors, chunk_prefix_dev, state_dev,
-                                                                   beta1, beta2, eps, clear_grad);
+  constexpr int kPrologueThreads = 128;
+  // tensors with no elements still count a step, like torch.optim.Adam's
+  adam_prologue_kernel<<<(n_tensors + kPrologueThreads - 1) / kPrologueThreads, kPrologueThreads, 0, stream>>>(
+      table_dev, n_tensors, reinterpret_cast<float2*>(bias_dev), beta1, beta2, found_inf_dev);
+  if (total_chunks > 0)
+    adam_main_kernel<<<(unsigned)total_chunks, kThreads, 0, stream>>>(table_dev, n_tensors, chunk_prefix_dev,
+                                                                     reinterpret_cast<const float2*>(bias_dev),
+                                                                     found_inf_dev, beta1, beta2, eps, clear_grad);
   return (int)cudaGetLastError();
 }

@@ -2,8 +2,10 @@
 (csrc/tir_adam.cu), with the density L1 regulariser's gradient folded in, the gradients cleared in the same pass (the
 backward kernels accumulate into persistent buffers) and a device-side ``found_inf`` skip flag — SURVEY.md §8 f3.
 
-State layout follows torch.optim.Adam (``state[p] = {'step', 'exp_avg', 'exp_avg_sq'}``), so optimizer checkpoints are
-interchangeable; learning rates may be floats or 0-dim device tensors (CUDA-graph replay, static_step.lr_tensors).
+State layout follows torch.optim.Adam (``state[p] = {'step', 'exp_avg', 'exp_avg_sq'}``, ``step`` a 0-dim fp32 device
+tensor as with ``capturable=True``), so optimizer checkpoints are interchangeable.  Like torch, every parameter counts its
+own steps: one that gets no gradient is skipped and its count stays put, so a parameter that joins late starts its bias
+corrections at step 1.  Learning rates may be floats or 0-dim device tensors (CUDA-graph replay, static_step.lr_tensors).
 """
 from __future__ import annotations
 
@@ -14,15 +16,36 @@ import torch
 from . import _lib
 
 
+def _same_layout(a, b):
+    return a.shape == b.shape and all(sa == sb for sa, sb, n in zip(a.stride(), b.stride(), a.shape) if n > 1)
+
+
+def _moment(t, p):
+    """A loaded exp_avg / exp_avg_sq laid out like its parameter: the kernel walks all four tensors in p's memory order."""
+    if t.device == p.device and t.dtype == torch.float32 and _same_layout(t, p):
+        return t
+    return torch.empty_like(p, memory_format=torch.preserve_format).copy_(t)
+
+
+def _own_step(step, dev):
+    """``state["step"]`` as the parameter's own 0-dim fp32 tensor on ``dev``.  A loaded checkpoint may hold it as a
+    number or a CPU tensor (torch.optim.Adam without capturable), or as a view that other parameters share."""
+    if (torch.is_tensor(step) and step.device == dev and step.dtype == torch.float32 and step.dim() == 0
+            and step.untyped_storage().nbytes() == 4):
+        return step
+    return torch.as_tensor(step).to(device=dev, dtype=torch.float32).reshape(()).clone()
+
+
 class FusedAdam(torch.optim.Optimizer):
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, l1=None, clear_grad=True):
         """``l1``: {parameter: coefficient} — adds coefficient * sign(parameter) to that parameter's gradient, i.e. the
         gradient of ``coefficient * parameter.abs().sum()`` (for ``w * mean|x|`` pass ``w / x.numel()``)."""
-        super().__init__(params, dict(lr=lr, betas=betas, eps=eps))
+        # weight_decay / amsgrad / maximize: torch.optim.Adam's options at the values this update implements, so that a
+        # state_dict of this optimizer loads into torch's
+        super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=0.0, amsgrad=False, maximize=False))
         self.l1 = {id(p): float(c) for p, c in (l1 or {}).items()}
         self.clear_grad = bool(clear_grad)
         self._key = None
-        self._state_dev = None
         self._keep = None
 
     def density_l1(self, model, weight):
@@ -42,12 +65,12 @@ class FusedAdam(torch.optim.Optimizer):
         prefix = [0]
         keep = []
         for k, (p, g, st, grp) in enumerate(entries):
-            same = all(sg == sp for sg, sp, n in zip(g.stride(), p.stride(), p.shape) if n > 1) and g.shape == p.shape
-            if not same or not self._dense(p):
+            if not _same_layout(g, p) or not self._dense(p):
                 raise _lib.TirError("FusedAdam needs dense parameters whose gradients share their layout "
                                     f"(got strides {tuple(p.stride())} / {tuple(g.stride())})")
             t = table[k]
             t.p, t.g, t.m, t.v, t.n = p.data_ptr(), g.data_ptr(), st["exp_avg"].data_ptr(), st["exp_avg_sq"].data_ptr(), p.numel()
+            t.step = st["step"].data_ptr()
             lr = grp["lr"]
             if isinstance(lr, torch.Tensor):
                 t.lr_dev, t.lr = lr.data_ptr(), 0.0
@@ -59,6 +82,7 @@ class FusedAdam(torch.optim.Optimizer):
         raw = torch.frombuffer(bytearray(bytes(table)), dtype=torch.uint8).clone()
         self._table = raw.to(dev)
         self._prefix = torch.tensor(prefix, dtype=torch.int64).to(dev)
+        self._bias = torch.empty(2 * len(entries), device=dev)       # per entry: 1 - beta1^t, sqrt(1 - beta2^t)
         self._n, self._chunks = len(entries), prefix[-1]
         self._keep = keep
 
@@ -76,31 +100,35 @@ class FusedAdam(torch.optim.Optimizer):
                 beta1, beta2, eps = float(b1), float(b2), float(grp["eps"])
             elif (beta1, beta2, eps) != (float(b1), float(b2), float(grp["eps"])):
                 raise _lib.TirError("FusedAdam: betas / eps must be the same for every parameter group")
+            if grp.get("weight_decay", 0.0) or grp.get("amsgrad", False) or grp.get("maximize", False):
+                raise _lib.TirError("FusedAdam implements Adam without weight_decay, amsgrad or maximize")
             for p in grp["params"]:
                 if p.grad is None:
                     continue
                 st = self.state[p]
                 if not st:
+                    st["step"] = torch.zeros((), dtype=torch.float32, device=p.device)
                     st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
                     st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                else:
+                    st["step"] = _own_step(st["step"], p.device)
+                    st["exp_avg"] = _moment(st["exp_avg"], p)
+                    st["exp_avg_sq"] = _moment(st["exp_avg_sq"], p)
                 dev = p.device
                 entries.append((p, p.grad, st, grp))
         if not entries:
             return loss
-        if self._state_dev is None or self._state_dev.device != dev:
-            self._state_dev = torch.zeros(4, device=dev)
-        key = tuple((p.data_ptr(), g.data_ptr(), st["exp_avg"].data_ptr(),
+        key = tuple((p.data_ptr(), g.data_ptr(), st["exp_avg"].data_ptr(), st["exp_avg_sq"].data_ptr(),
+                     st["step"].data_ptr(),
                      grp["lr"].data_ptr() if isinstance(grp["lr"], torch.Tensor) else float(grp["lr"]),
                      self.l1.get(id(p), 0.0)) for p, g, st, grp in entries)
         if key != self._key:
             self._build(entries, dev)
             self._key = key
-        for p, _, st, _ in entries:
-            st["step"] = self._state_dev[0]            # one shared counter (every parameter steps together)
         lib = _lib.load()
         fi = getattr(self, "found_inf", None)
         _lib.check(lib.tir_adam_step(C.c_void_p(self._table.data_ptr()), self._n, C.c_void_p(self._prefix.data_ptr()),
-                                     self._chunks, C.c_void_p(self._state_dev.data_ptr()), beta1, beta2, eps,
+                                     self._chunks, C.c_void_p(self._bias.data_ptr()), beta1, beta2, eps,
                                      None if fi is None else C.c_void_p(fi.data_ptr()), int(self.clear_grad),
                                      _lib.stream_ptr()), "tir_adam_step")
         return loss

@@ -26,7 +26,7 @@ def test_header_symbols_exported(lib):
     for n in names:
         assert hasattr(lib, n), f"{n} declared in the header but not exported"
         assert n in _lib.EXPORTS, f"{n} has no ctypes binding"
-    assert lib.tir_abi_version() == 3
+    assert lib.tir_abi_version() == 4
 
 
 def test_struct_sizes_match_header(lib):
@@ -34,6 +34,7 @@ def test_struct_sizes_match_header(lib):
     assert (ctypes.sizeof(_lib.TirField), ctypes.sizeof(_lib.TirMlp), ctypes.sizeof(_lib.TirMarchCfg)) == (248, 88, 48)
     assert _lib.APP_SAMPLE_BYTES == 24
     assert ctypes.sizeof(_lib.TirRayMaps) == 64
+    assert ctypes.sizeof(_lib.TirAdamTensor) == 64        # p g m v, n, lr_dev, lr + l1, step
 
 
 def test_primary_struct_sizes_match_the_c_compiler(lib, tmp_path):

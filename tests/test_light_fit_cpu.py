@@ -193,7 +193,7 @@ def test_max_texels_constant(tmp_path):
     exe = tmp_path / "k"
     subprocess.run(["gcc", "-I", os.path.join(REPO, "include"), str(src), "-o", str(exe)], check=True)
     out = subprocess.run([str(exe)], check=True, capture_output=True, text=True).stdout.split()
-    assert [int(v) for v in out] == [_lib.TRANSPORT_MAX_TEXELS, 3] == [2048, _lib.ABI_VERSION]
+    assert [int(v) for v in out] == [_lib.TRANSPORT_MAX_TEXELS, 4] == [2048, _lib.ABI_VERSION]
 
 
 # ---- 2. the texel tables ----------------------------------------------------------------------------------------------
