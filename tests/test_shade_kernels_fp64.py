@@ -15,7 +15,7 @@ roundoff, so one correctly rounded op is covered with a factor 2 to spare) the r
   * a + b:  e_a + e_b + u (|a + b| + e_a + e_b)              (the fp32 result is rounded once)
   * a * b:  |a| e_b + |b| e_a + e_a e_b + u (|ab| + that)     (exact in the inputs' errors, not first order)
   * a / b:  (e_a + |a/b| e_b) / (|b| - e_b) + u (...)           (infinite when e_b >= |b|)
-  * sqrt:   e / sqrt(x) + u (...);  exp2f: 2^x (2^e - 1) + 2u 2^x (the CUDA Math API's 2 ulp);
+  * sqrt:   min(e / sqrt(x), sqrt(e)) + u (...);  exp2f: 2^x (2^e - 1) + 2u 2^x (the CUDA Math API's 2 ulp);
     powf(x, y): |y| max((x - e)^(y - 1), (x + e)^(y - 1)) e + 4u x^y (its 4 ulp); mean-value bounds at the worst
     end of [x - e, x + e], so not first order
   * clamp / fmaxf: 1-Lipschitz, so e passes through; where the value is clamped by more than e, the result is exact
@@ -140,7 +140,8 @@ class R:
 
     def sqrt(self):
         s = self.v.sqrt()
-        return R.rnd(s, self.e / _d(s))
+        # |sqrt(x + e) - sqrt(x)| <= min(e / sqrt(x), sqrt(e)); an exact input adds only the rounding
+        return R.rnd(s, torch.where(self.e > 0, torch.minimum(self.e / _d(s), self.e.sqrt()), 0.0))
 
     def exp2(self):
         p = torch.exp2(self.v)
@@ -190,14 +191,17 @@ class Gates:
 # the kernel's shading, forward and explicit backward, in float64
 # ------------------------------------------------------------------------------------------------------------------
 def tone(lin, srgb):
-    """tone() of tir_ggx.h on a value (the kernel's saved lin); returns R."""
-    t = R(lin).clamp(0.0, 1.0)
+    """tone() of tir_ggx.h on a value (the kernel's saved lin) or on an R; returns R.  Where an R lies within its
+    bound of the sRGB threshold, the jump between the two branches is added to the bound."""
+    t = (lin if isinstance(lin, R) else R(lin)).clamp(0.0, 1.0)
     if not srgb:
         return t
     lo = t * SRGB_S
     hi = (t + LO).pow(SRGB_E) * SRGB_A - SRGB_B
     sel = _d(t.v) <= SRGB_T
-    return R(torch.where(sel, lo.v, hi.v), torch.where(sel, lo.e, hi.e))
+    amb = ((_d(t.v) - SRGB_T).abs() <= t.e) & (t.e > 0)
+    jump = torch.where(amb, (lo.v - hi.v).abs() + torch.maximum(lo.e, hi.e), torch.zeros_like(t.e))
+    return R(torch.where(sel, lo.v, hi.v), torch.where(sel, lo.e, hi.e) + jump)
 
 
 def tone_grad(lin, srgb):
@@ -211,16 +215,10 @@ def tone_grad(lin, srgb):
     return R(v, e)
 
 
-def shade_ref(n, V, a, F0, r, dirs, w, D, vis, ind, go=None, sgn=None, gates=None):
-    """One row block: n, V, a, F0, r [m,3] (V as loaded: the list form's view or minus the ray direction; r broadcast
-    over the channels in the hits form), dirs [nl,3], w [nl], D = direct[light] [m,nl,3], vis [m,nl], ind [m,nl,3],
-    go [m,3] (R) the gradient reaching the linear value.  Returns a dict of R: lin [m,3]; with go also g_normal,
-    g_albedo, g_fresnel, g_rough [m,3] (per channel, before any channel sum) and gd [m,nl,3], each row's term of the
-    direct-light gradient; plus nov, the value whose sign picks the normal's side."""
-    gates = gates if gates is not None else Gates()
-    nl = dirs.shape[0]
-    c_lane = math.ceil(nl / 32) + 5
-    N, Vr, A, F0r, Rr = R(n), R(V), R(a), R(F0), R(r)
+def ggx_ref(N, Vr, F0r, Rr, L, sgn=None):
+    """ggx_point, ggx_dir and ggx_terms of tir_ggx.h in float64 (R): N, Vr, F0r, Rr [m,3] as the kernel loads them,
+    L [nl,3] directions shared by every row or [m,nl,3] per row, both as stored; sgn [m] replaces sign(nov).  Returns
+    a namespace of the intermediates the shading forward and backward read; spec is GGX_specular [m,nl,3]."""
     # ggx_point
     inv_nn = 1.0 / dot3(N, N).sqrt().clamp(TINY)
     inv_vn = 1.0 / dot3(Vr, Vr).sqrt().clamp(TINY)
@@ -234,15 +232,15 @@ def shade_ref(n, V, a, F0, r, dirs, w, D, vis, ind, go=None, sgn=None, gates=Non
     alpha2 = al * al
     k = (al + Rr * 2.0 + 1.0) / 8.0
     nom1 = NoV[:, None] * (1.0 - k) + k
-    # ggx_dir
-    L = R(dirs)
-    cosr = dot3(L[None], N[:, None])                                     # [m,nl] raw L . n
+    # ggx_dir, [m|1,nl]
+    L = L if L.v.dim() == 3 else L[None]
+    cosr = dot3(L, N[:, None])                                          # [m,nl] raw L . n
     cosv = cosr.clamp(0.0)
     inv_ln = 1.0 / dot3(L, L).sqrt().clamp(TINY)
-    Ln = L * inv_ln[:, None]
-    H = (Ln[None] + Vn[:, None]) * 0.5
+    Ln = L * inv_ln[..., None]
+    H = (Ln + Vn[:, None]) * 0.5
     Hn = H * (1.0 / dot3(H, H).sqrt().clamp(TINY))[..., None]
-    NoL_raw, NoH_raw, VoH_raw = dot3(Np[:, None], Ln[None]), dot3(Np[:, None], Hn), dot3(Vn[:, None], Hn)
+    NoL_raw, NoH_raw, VoH_raw = dot3(Np[:, None], Ln), dot3(Np[:, None], Hn), dot3(Vn[:, None], Hn)
     NoL, NoH, VoH = NoL_raw.clamp(LO, 1.0), NoH_raw.clamp(LO, 1.0), VoH_raw.clamp(LO, 1.0)
     p2 = ((VoH * FM_A - FM_B) * VoH).exp2()
     # ggx_terms, [m,nl,3]
@@ -255,6 +253,27 @@ def shade_ref(n, V, a, F0, r, dirs, w, D, vis, ind, go=None, sgn=None, gates=Non
     nomr = FOUR_PI * nom0 * nom0 * n1 * nom2
     nom = nomr.clamp(LO, FOUR_PI)
     spec = frac / nom
+    return types.SimpleNamespace(inv_nn=inv_nn, Vn=Vn, nov=nov, s=s, Np=Np, nov2=nov2, NoV=NoV, k=k, cosr=cosr,
+                                 cosv=cosv, Ln=Ln, Hn=Hn, NoL_raw=NoL_raw, NoH_raw=NoH_raw, F0c=F0c, al2=al2, kc=kc,
+                                 n1=n1, NoHc=NoHc, NoLc=NoLc, p2c=p2c, frac0=frac0, nom0=nom0, nom2=nom2, nomr=nomr,
+                                 nom=nom, spec=spec)
+
+
+def shade_ref(n, V, a, F0, r, dirs, w, D, vis, ind, go=None, sgn=None, gates=None):
+    """One row block: n, V, a, F0, r [m,3] (V as loaded: the list form's view or minus the ray direction; r broadcast
+    over the channels in the hits form), dirs [nl,3], w [nl], D = direct[light] [m,nl,3], vis [m,nl], ind [m,nl,3],
+    go [m,3] (R) the gradient reaching the linear value.  Returns a dict of R: lin [m,3]; with go also g_normal,
+    g_albedo, g_fresnel, g_rough [m,3] (per channel, before any channel sum) and gd [m,nl,3], each row's term of the
+    direct-light gradient; plus nov, the value whose sign picks the normal's side."""
+    gates = gates if gates is not None else Gates()
+    nl = dirs.shape[0]
+    c_lane = math.ceil(nl / 32) + 5
+    N, Vr, A, F0r, Rr = R(n), R(V), R(a), R(F0), R(r)
+    g = ggx_ref(N, Vr, F0r, Rr, R(dirs), sgn)
+    inv_nn, Vn, nov, s, Np, nov2, NoV, k = g.inv_nn, g.Vn, g.nov, g.s, g.Np, g.nov2, g.NoV, g.k
+    cosr, cosv, Ln, Hn, NoL_raw, NoH_raw = g.cosr, g.cosv, g.Ln, g.Hn, g.NoL_raw, g.NoH_raw
+    F0c, al2, kc, n1, NoHc, NoLc, p2c = g.F0c, g.al2, g.kc, g.n1, g.NoHc, g.NoLc, g.p2c
+    frac0, nom0, nom2, nomr, nom, spec = g.frac0, g.nom0, g.nom2, g.nomr, g.nom, g.spec
     brdf = A[:, None] / PI + spec
     light = R(vis)[..., None] * R(D) + R(ind)
     cw = cosv * R(w)[None]
@@ -282,7 +301,7 @@ def shade_ref(n, V, a, F0, r, dirs, w, D, vis, ind, go=None, sgn=None, gates=Non
     gNoV_t = g_nom1 * (1.0 - kc)
     g_NoL = gates.gate(g_NoL, NoL_raw, LO, 1.0, "NoL")
     g_NoH = gates.gate(g_NoH, NoH_raw, LO, 1.0, "NoH")
-    gNp_t = g_NoL[..., None] * Ln[None] + g_NoH[..., None] * Hn
+    gNp_t = g_NoL[..., None] * Ln + g_NoH[..., None] * Hn
     gn_t = gates.gate(g_cos[..., None] * R(dirs)[None], cosr, 0.0, math.inf, "cos", strict=True)
     gNp, gn, ga, gF0, gal2, gk = (t.sum(1, c_lane) for t in (gNp_t, gn_t, ga_t, gF0_t, gal2_t, gk_t))
     m = n.shape[0]
