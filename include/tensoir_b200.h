@@ -598,6 +598,47 @@ int tir_relight_shade(const TirEnvMap* envs, int32_t n_lights, const float* rays
                       int32_t vis_kind, float* with_bg, float* without_bg, int64_t out_rows, int64_t row0,
                       void* stream);
 
+/* ---- relighting with multiple importance sampling: GGX-lobe samples combined with environment-map samples ----------
+ * An opt-in estimator of the same chunk (tir_relight_shade's is the default).  For a hit ray i and map l:
+ *
+ *   linear[l,i] = sum over the S_l light samples of map l and the S_b BRDF samples of ray i of
+ *                 f(w) * V(w) * E_l(w) * cos(w) / (S_l * p_light_l(w) + S_b * p_brdf(w))
+ *
+ * an unbiased estimate of the integral of f V E cos over the sphere, with f tir_relight_shade's BRDF, cos the raw-normal
+ * cosine (a sample with cos <= 1e-6 contributes 0 and is not marched), V the march's visibility as tir_relight_shade
+ * reads it, and E_l map l taken as piecewise constant over its lat-long texels.  Light samples: a texel from the fp64
+ * CDF, then a point uniform in its solid angle, p_light = P_texel / dOmega_texel (exact solid angle).  BRDF samples,
+ * one set per ray shared by every map: with probability 1/2 a GGX visible-normal half vector (alpha = mean(r)^2, about
+ * the view-side normal) reflected, else a cosine-weighted direction; p_brdf = 1/2 G1(V) D(h) / (4 NoV) + 1/2 max(Np.w,
+ * 0) / pi.  E and p_light of every sample come from the texel of its direction as rounded.  Definitions in
+ * csrc/tir_mis_body.h.  Slots: the L*n*S_l light slots (map, ray, sample) first, then the n*S_b BRDF slots (ray,
+ * sample).
+ *   tir_relight_mis_sample  one thread per slot of a hit ray (acc > acc_mask_threshold), u_light [L,n,S_l,3] and
+ *                           u_brdf [n,S_b,3] fp64 (u_brdf may be NULL when S_b = 0): dir [slots,3] and pos [slots]
+ *                           (list row, or -1) for every slot (zeros and -1 on non-hit rays); the marched slots'
+ *                           (surface point, direction) are appended to list_o / list_d; count and capacity as in
+ *                           tir_relight_sample.
+ *   tir_march_density       on the list, by the caller, with relight()'s table.
+ *   tir_relight_mis_shade   one warp per (map, ray), lanes over the map's light slots and then the ray's BRDF slots:
+ *                           linear as above in a fixed order, without_bg = sRGB(clamp(linear)), white on non-hit rays;
+ *                           with_bg as tir_relight_shade.  linear_out (NULL allowed) [L,out_rows,3] gets the un-toned
+ *                           sum, 0 on non-hit rays.  Rows are written at [l, row0 + i] of [L, out_rows, 3] maps.
+ * Repeated calls on the same list give identical bits.  TIR_ERR_SHAPE for n < 0, S_l < 1, S_b < 0, a stride other than
+ * 1 or 3, more than TIR_RELIGHT_MAX_LIGHTS maps, capacity outside [0, INT32_MAX] or output rows out of range;
+ * TIR_ERR_CONFIG for an unknown vis_kind; TIR_ERR_NULL for a missing input. */
+int tir_relight_mis_sample(const TirEnvMap* envs /* host array [n_lights] */, int32_t n_lights, const float* rays,
+                           const float* depth, const float* normal, const float* albedo, const float* rough,
+                           int32_t rough_stride /* 1: [n,1], 3: [n,3] */, const float* fresnel, const float* acc,
+                           int64_t n, int32_t S_l, int32_t S_b, float acc_mask_threshold, const double* u_light,
+                           const double* u_brdf, float* dir, int32_t* pos, float* list_o,
+                           float* list_d /* [capacity,3] */, int64_t capacity, int64_t* count, void* stream);
+int tir_relight_mis_shade(const TirEnvMap* envs, int32_t n_lights, const float* rays, const float* normal,
+                          const float* albedo, const float* rough, int32_t rough_stride, const float* fresnel,
+                          const float* acc, int64_t n, int32_t S_l, int32_t S_b, float acc_mask_threshold,
+                          const float* rescale /* [3] */, const float* dir, const int32_t* pos, const float* vis_list,
+                          int32_t vis_kind, float* with_bg, float* without_bg, float* linear_out /* or NULL */,
+                          int64_t out_rows, int64_t row0, void* stream);
+
 /* ---- material editing: the BRDF parameters of n surface points, edited by a table of rules, for tir_relight_shade
  * (or any other consumer) ----------------------------------------------------------------------------------------------
  * The point of row i is points[i] when `points` is given, else rays[i].o + depth[i] * rays[i].d rounded as

@@ -249,6 +249,12 @@ EXPORTS = {
     "tir_relight_shade": (C.c_int, [C.POINTER(TirEnvMap), C.c_int32, f32p, f32p, f32p, f32p, C.c_int32, f32p, f32p,
                                     C.c_int64, C.c_int32, C.c_float, f32p, C.c_void_p, C.c_void_p, f32p, C.c_int32,
                                     f32p, f32p, C.c_int64, C.c_int64, C.c_void_p]),
+    "tir_relight_mis_sample": (C.c_int, [C.POINTER(TirEnvMap), C.c_int32, f32p, f32p, f32p, f32p, f32p, C.c_int32,
+                                         f32p, f32p, C.c_int64, C.c_int32, C.c_int32, C.c_float, C.c_void_p,
+                                         C.c_void_p, f32p, C.c_void_p, f32p, f32p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "tir_relight_mis_shade": (C.c_int, [C.POINTER(TirEnvMap), C.c_int32, f32p, f32p, f32p, f32p, C.c_int32, f32p,
+                                        f32p, C.c_int64, C.c_int32, C.c_int32, C.c_float, f32p, f32p, C.c_void_p, f32p,
+                                        C.c_int32, f32p, f32p, f32p, C.c_int64, C.c_int64, C.c_void_p]),
     "tir_material_edit": (C.c_int, [C.POINTER(TirEditRule), C.c_int32, f32p, f32p, f32p, f32p, f32p, C.c_int32, f32p,
                                     f32p, C.c_int64, C.c_float, f32p, f32p, f32p, f32p, C.c_void_p, C.c_void_p]),
     "tir_lights_sample": (C.c_int, [C.POINTER(TirLight), C.c_int32, f32p, f32p, f32p, f32p, C.c_int64, C.c_float,
@@ -301,7 +307,7 @@ KERNELS_PER_CALL = {"tir_pack_channels_last": 1, "tir_unpack_channels_last_add":
                     "tir_primary_backward": 9, "tir_primary_radiance": 2, "tir_primary_radiance_backward": 6,
                     "tir_composite_bwd": 1, "tir_tail_fwd": 1, "tir_tail_bwd": 1, "tir_epilogue_fwd": 1,
                     "tir_epilogue_bwd": 1, "tir_eval_view": 3, "tir_relight_sample": 1, "tir_relight_shade": 1,
-                    "tir_material_edit": 1, "tir_lights_sample": 1, "tir_lights_shade": 1,
+                    "tir_relight_mis_sample": 1, "tir_relight_mis_shade": 1, "tir_material_edit": 1, "tir_lights_sample": 1, "tir_lights_shade": 1,
                     "tir_transport_sample": 1, "tir_transport_build": 1,
                     "tir_indirect_sample": 1, "tir_indirect_hits": 3, "tir_indirect_radiance": 1,
                     "tir_indirect_shade": 1, "tir_marching_cubes_count": 7, "tir_marching_cubes_emit": 2,

@@ -142,19 +142,25 @@ def relight_visibility(tensoIR, envs, L, rays, depth, normal, acc, u, num_sample
                                       n, S, thr, _lib.dptr(u, dtype=torch.float64), _lib.dptr(bins, torch.int32),
                                       _lib.dptr(pos, torch.int32), _lib.dptr(list_o), _lib.dptr(list_d), cap,
                                       _lib.dptr(count, torch.int64), _lib.stream_ptr()), "tir_relight_sample")
-    m = int(count.item())                          # the one host sync of the chunk: sizes the visibility march
+    return bins, pos, march_list(tensoIR, pos, list_o, list_d, count, vis_equation, ordered)
+
+
+def march_list(tensoIR, pos, list_o, list_d, count, vis_equation, ordered=False):
+    """The density march of an appended visibility list: reads back its length (``count``, the one host sync of the
+    chunk) and marches its rows with relight()'s 96-sample table over [0.05, 1.5].  ``ordered``: put the list in slot
+    order first (slot_order, rewriting pos).  -> vis per list row (t_last for nerv, acc for nerfactor)."""
+    cap = int(list_o.shape[0])
+    m = int(count.item())
     if m > cap:
         raise _lib.TirError(f"relight visibility list overflow: {m} > {cap}")
-    if m > 0:
-        if ordered:
-            list_o, list_d = slot_order(pos, list_o[:m], list_d[:m])
-        table = ops.equal_z_table(96, 0.05, 1.5, dev)
-        t_last, acc_s, _ = ops.march_density(tensoIR, list_o[:m], list_d[:m], table=table,
-                                             counters=tensoIR.__dict__.get("_tir_counters"))
-        vis = (t_last if vis_equation == 'nerv' else acc_s).contiguous()
-    else:
-        vis = torch.zeros(1, device=dev)
-    return bins, pos, vis
+    if m == 0:
+        return torch.zeros(1, device=list_o.device)
+    if ordered:
+        list_o, list_d = slot_order(pos, list_o[:m], list_d[:m])
+    table = ops.equal_z_table(96, 0.05, 1.5, list_o.device)
+    t_last, acc_s, _ = ops.march_density(tensoIR, list_o[:m], list_d[:m], table=table,
+                                         counters=tensoIR.__dict__.get("_tir_counters"))
+    return (t_last if vis_equation == 'nerv' else acc_s).contiguous()
 
 
 def relight_shade(envs, L, rays, normal, albedo, rough, fresnel, acc, num_samples, acc_mask_threshold, rescale_value,
@@ -235,6 +241,23 @@ def _load_model(args, device):
     return model
 
 
+def mis_options(args):
+    """relight()'s estimator options from ``args``: -> (sampling, brdf_samples).  ValueError for an unknown sampling,
+    brdf_samples outside [0, NUM_SAMPLES - 1], or sampling 'mis' with indirect light."""
+    sampling = getattr(args, "sampling", None) or "light"
+    n_brdf = getattr(args, "brdf_samples", None)
+    given = n_brdf is not None
+    n_brdf = 128 if n_brdf is None else n_brdf
+    if sampling not in ("light", "mis"):
+        raise ValueError(f"sampling must be 'light' or 'mis', got {sampling!r}")
+    if (given or sampling == "mis") and (isinstance(n_brdf, bool) or int(n_brdf) != n_brdf
+                                         or not 0 <= n_brdf <= NUM_SAMPLES - 1):
+        raise ValueError(f"brdf_samples must be an integer in [0, {NUM_SAMPLES - 1}], got {n_brdf!r}")
+    if sampling == "mis" and int(getattr(args, "indirect_samples", 0) or 0) > 0:
+        raise ValueError("sampling='mis' does not combine with indirect_samples > 0")
+    return sampling, int(n_brdf)
+
+
 @torch.no_grad()
 def relight(dataset, args, tensoIR=None, *, rescale_value=None):
     """relight_importance.py:30-340.  ``dataset`` follows the reference relighting test set's item contract
@@ -244,8 +267,12 @@ def relight(dataset, args, tensoIR=None, *, rescale_value=None):
     (compute_rescale_ratio), as the reference does.
     Indirect light (indirect.py) is read from ``args`` too: ``indirect_samples`` K (0, the default, shades direct light
     only), ``indirect_light_samples`` S2 (32), ``indirect_seed`` (lighting.SEED) and ``save_indirect``, which also
-    writes the linear indirect-only image of every map as {view}/relighting_indirect/{light}.hdr."""
+    writes the linear indirect-only image of every map as {view}/relighting_indirect/{light}.hdr.
+    ``sampling``: 'light' (the default, the reference's estimator) or 'mis' (mis.relight_chunk_mis: S_b =
+    ``brdf_samples`` (128) BRDF samples per hit and S_l = NUM_SAMPLES - S_b light samples per (map, hit), combined by
+    multiple importance sampling; not with indirect light)."""
     from .relight import Environment_Light
+    sampling, n_brdf = mis_options(args)
     opt = {k: getattr(args, k, v) for k, v in SCRIPT_DEFAULTS.items()}
     device = torch.device("cuda")
     if tensoIR is None:
@@ -265,6 +292,9 @@ def relight(dataset, args, tensoIR=None, *, rescale_value=None):
     if rescale_value is None:
         _, rescale_value = compute_rescale_ratio(tensoIR, dataset)
     rescale_value = torch.as_tensor(rescale_value, dtype=torch.float32).to(device)
+
+    if sampling == 'mis':
+        from .mis import mis_uniforms, relight_chunk_mis
 
     # one bounce of indirect light (indirect.py): off unless indirect_samples > 0
     n_ind = int(getattr(args, "indirect_samples", 0) or 0)
@@ -306,6 +336,12 @@ def relight(dataset, args, tensoIR=None, *, rescale_value=None):
                 if k not in prim:
                     prim[k] = torch.empty((n_pix,) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)
                 prim[k][s:e] = t
+            if sampling == 'mis':
+                u_light, u_brdf = mis_uniforms(L, e - s, NUM_SAMPLES - n_brdf, n_brdf, device)
+                relight_chunk_mis(tensoIR, envir_light, names, rays, (depth, normal, albedo, rough, fresnel, acc),
+                                  rescale_value, u_light, u_brdf, acc_mask_threshold=thr,
+                                  vis_equation=opt["vis_equation"], out=(with_map, without_map), row0=s, tables=tables)
+                continue
             u = _uniforms(L, e - s, NUM_SAMPLES, device)
             if n_ind > 0:
                 relight_chunk_indirect(tensoIR, envir_light, names, rays, (depth, normal, albedo, rough, fresnel, acc),

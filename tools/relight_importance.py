@@ -8,7 +8,10 @@ tools/dropin_train_check.py:
 
 ``--indirect_samples K`` adds one bounce of indirect light with K directions per surface hit (default 0: direct light
 only, the reference's estimator), ``--indirect_light_samples S2`` sets the light samples per secondary hit (default 32)
-and ``--save_indirect 1`` also writes the linear indirect-only images.
+and ``--save_indirect 1`` also writes the linear indirect-only images.  ``--sampling mis`` shades with multiple
+importance sampling (GGX-lobe samples combined with environment-map samples, tensoir_b200/mis.py) instead of the
+reference's texel-centre estimator, with ``--brdf_samples N`` of the 512 samples per surface hit drawn from the BRDF
+(default 128).
 """
 import os
 import sys
@@ -34,8 +37,17 @@ def indirect_options(argv):
                 save_indirect=bool(save))
 
 
+def sampling_options(argv):
+    """Remove the estimator flags from argv -> dict of the args attributes relight() reads: --sampling light|mis
+    (light), --brdf_samples N (128)."""
+    sampling = pop_option(argv, "--sampling", str)
+    n_brdf = pop_option(argv, "--brdf_samples", int)
+    return dict(sampling=sampling or "light", brdf_samples=128 if n_brdf is None else n_brdf)
+
+
 if __name__ == "__main__":
     indirect = indirect_options(sys.argv)
+    indirect.update(sampling_options(sys.argv))
 
     from dataLoader import dataset_dict
     from opt import config_parser

@@ -1,9 +1,14 @@
 """Time the relighting evaluation on N synthetic views of the lego scene under five environment maps and print one JSON
 line: seconds per view by phase (primary render, sample + visibility list, visibility march, shade, metrics, PNG
 writing), and on the same chunks and the same sample indices the eager relight_chunk (tensoir_b200/relight.py) with the
-largest difference between the two.
+largest difference between the two.  With ``--sampling mis`` the chunks go through mis.relight_chunk_mis (S_b =
+``--brdf_samples`` BRDF samples and 512 - S_b light samples per (map, hit)) and the eager comparison is skipped.  Both
+modes report the shadow rays marched per view and a noise figure: on the middle chunk of every view, the RMSE of the
+linear estimate against the mean of 16 MIS passes (S_b = 128), over the hit pixels of every map whose reference is
+below 0.98 (the default estimator's linear value is its sRGB output inverted, on pixels below the clamp).
 
-    python tools/relight_views.py [--views 2] [--grid 300] [--size 800] [--batch 4096]
+    python tools/relight_views.py [--views 2] [--grid 300] [--size 800] [--batch 4096] [--sampling light|mis]
+                                  [--brdf_samples 128]
 """
 import argparse
 import json
@@ -25,10 +30,13 @@ def main():
     ap.add_argument("--grid", type=int, default=300)
     ap.add_argument("--size", type=int, default=800)
     ap.add_argument("--batch", type=int, default=4096)
+    ap.add_argument("--sampling", choices=("light", "mis"), default="light")
+    ap.add_argument("--brdf_samples", type=int, default=128)
     a = ap.parse_args()
     import __graft_entry__ as g
     g.build()
     import bench
+    import tensoir_b200.mis as MIS
     import tensoir_b200.relighting as R
     from eval_views import gpu_info
     from tensoir_b200 import ops
@@ -52,7 +60,8 @@ def main():
     # phase timing: the two relighting kernels and the march are timed through the same wrappers relight() calls
     lib = R._lib.load()
     timers = {}
-    for key, fn_name in (("sample", "tir_relight_sample"), ("shade", "tir_relight_shade")):
+    for key, fn_name in (("sample", "tir_relight_sample"), ("shade", "tir_relight_shade"),
+                         ("sample", "tir_relight_mis_sample"), ("shade", "tir_relight_mis_shade")):
         fn = getattr(lib, fn_name)
 
         def timed(*x, _fn=fn, _key=key):
@@ -66,11 +75,14 @@ def main():
     # "eager_march" inside the eager one, so that the two shading figures can be compared on their own
     march = ops.march_density
     march_key = [None]
+    shadow_rays = [0]
 
     def timed_march(*x, **k):
         t0 = tick()
         r = march(*x, **k)
         timers[march_key[0]] = timers.get(march_key[0], 0.0) + tick() - t0
+        if march_key[0] == "march":
+            shadow_rays[0] += int(x[1].shape[0])
         return r
     ops.march_density = timed_march
 
@@ -83,12 +95,15 @@ def main():
                 march_key[0] = None
         return run
     relight_chunk_fused = with_march_key("march", R.relight_chunk_fused)
+    relight_chunk_mis = with_march_key("march", MIS.relight_chunk_mis)
+    S_b = a.brdf_samples if a.sampling == "mis" else 0
     relight_chunk = with_march_key("eager_march", relight_chunk)
     tables = R.env_tables(env, names)
     max_diff = 0.0
     out_dir = tempfile.mkdtemp()
     for rep in range(2):                                              # rep 0 warms up
         timers.clear()
+        shadow_rays[0] = 0
         for k in phases:
             phases[k] = 0.0
         for v, item in enumerate(items):
@@ -105,6 +120,11 @@ def main():
                                                                               white_bg=True, ndc_ray=False, N_samples=-1)
                 phases["render"] += tick() - t0
                 maps = (depth, normal, albedo, rough, fresnel, acc)
+                if a.sampling == "mis":
+                    u_l, u_b = MIS.mis_uniforms(L, e - s, S - S_b, S_b, dev)
+                    relight_chunk_mis(model, env, names, rays[s:e], maps, rescale, u_l, u_b,
+                                      out=(with_map, without_map), row0=s, tables=tables)
+                    continue
                 u = R._uniforms(L, e - s, S, dev)
                 relight_chunk_fused(model, env, names, rays[s:e], maps, rescale, u, S, out=(with_map, without_map),
                                     row0=s, tables=tables)
@@ -131,9 +151,40 @@ def main():
         for k in ("sample", "march", "shade", "eager_march"):
             phases[k] = timers.get(k, 0.0)
     n = len(items)
+    rays_per_view = shadow_rays[0] / n
+    # noise figure on the middle chunk of every view, which holds the object (not timed)
+    sq, cnt = 0.0, 0
+    for item in items:
+        mid = (item["rays"].shape[0] - a.batch) // 2
+        rays = item["rays"].to(dev)[mid:mid + a.batch]
+        m = rays.shape[0]
+        li = torch.zeros(m, 1, dtype=torch.int32, device=dev)
+        with torch.no_grad():
+            _, depth, normal, albedo, rough, fresnel, acc, *_ = model(rays, li, is_train=False, white_bg=True,
+                                                                      ndc_ray=False, N_samples=-1)
+        maps = (depth, normal, albedo, rough, fresnel, acc)
+
+        def mis_linear(sb):
+            lin = torch.zeros(L, m, 3, device=dev)
+            u_l, u_b = MIS.mis_uniforms(L, m, S - sb, sb, dev)
+            MIS.relight_chunk_mis(model, env, names, rays, maps, rescale, u_l, u_b, tables=tables, linear_out=lin)
+            return lin
+        ref = sum(mis_linear(128) for _ in range(16)) / 16
+        mask = (acc.reshape(-1) > 0.5)[None, :, None] & (ref < 0.98)
+        if a.sampling == "mis":
+            est = mis_linear(S_b)
+        else:
+            _, wo = R.relight_chunk_fused(model, env, names, rays, maps, rescale, R._uniforms(L, m, S, dev), S,
+                                          tables=tables)
+            est = torch.where(wo <= 0.0031308 * 12.92, wo / 12.92, ((wo + 0.055) / 1.055) ** 2.4 - 1e-6)
+            mask = mask & (wo < 0.999)
+        sq += float(((est - ref) ** 2)[mask].sum())
+        cnt += int(mask.sum())
     name, power = gpu_info()
     print(json.dumps({"tool": "relight_views", "gpu": name, "power_limit": power, "views": n, "size": a.size,
-                      "grid": a.grid, "maps": L, "samples": S, "batch": a.batch,
+                      "grid": a.grid, "maps": L, "samples": S, "batch": a.batch, "sampling": a.sampling,
+                      "brdf_samples": S_b, "shadow_rays_per_view": rays_per_view,
+                      "linear_rmse_middle_chunk": (sq / max(cnt, 1)) ** 0.5,
                       **{f"{k}_s_per_view": v / n for k, v in phases.items() if k not in ("eager", "eager_march")},
                       "fused_relight_s_per_view": (phases["sample"] + phases["march"] + phases["shade"]) / n,
                       "fused_without_march_s_per_view": (phases["sample"] + phases["shade"]) / n,
