@@ -244,7 +244,7 @@ int tir_secondary_march_vol(const TirField* field, const float* surf_xyz, const 
  *   The view dir of a sample is ray_dirs[ray] ([n_rays,3]) when n_dirs == 0, or the [n_dirs,3] table row ray % n_dirs
  *   when n_dirs > 0.  light_idx indexed by ray (n_dirs == 0) or by ray / n_dirs.
  * Runs the sm_90a wgmma kernel (csrc/tir_mlp_wgmma.cu): A operand and accumulator in registers, split-BF16 weights
- * resident in shared memory, two warpgroups per CTA on different 64-sample tiles. */
+ * resident in shared memory, three warpgroups per CTA on different 64-sample tiles. */
 int tir_app_mlp(const TirField* field, const TirMlp* mlp, const TirAppSample* samples,
                 const uint32_t* sample_count, int64_t max_samples, const float* ray_dirs, int32_t n_dirs,
                 const int32_t* light_idx, float* rgb_out, void* stream);

@@ -13,8 +13,9 @@
 //     basis GEMM a thread's four A elements of a k16 step are four adjacent channels (one float4 per tap), in layer 0
 //     they are the positional encodings of the basis features that thread's accumulator fragment produced; the weights
 //     are staged with the same permutation;
-//   * two warpgroups per CTA work on different tiles, so one warpgroup's L2-latency-bound gather overlaps the other's
-//     tensor-core work;
+//   * three warpgroups per CTA work on different tiles, so one warpgroup's L2-latency-bound gather overlaps the others'
+//     tensor-core work (the kernel is latency-bound: one warpgroup per CTA takes 1.70x the time of two, three take
+//     0.87x of two);
 //   * three GEMMs per tile: basis_mat (K = 144, N = 32), layer 0 (K = 160, N = 128), layer 1 (K = 128, N = 128).
 //   The last layer (128 -> 3, < 1 % of the FLOPs) runs in fp32 on the CUDA cores with a quad shuffle reduction.
 #include <cuda_bf16.h>
@@ -32,7 +33,7 @@ constexpr int HID = 128;
 constexpr int IN = 150;
 constexpr int K1 = 160;           // IN padded to k16
 constexpr int ROWS = 64;          // samples per tile = wgmma M
-constexpr int NWG = 2;            // warpgroups per CTA, each on its own tiles
+constexpr int NWG = 3;            // warpgroups per CTA, each on its own tiles (at most 168 registers per thread)
 constexpr int NTHREADS = NWG * 128;
 
 struct SmemW {
