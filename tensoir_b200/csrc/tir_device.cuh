@@ -273,4 +273,31 @@ __device__ __forceinline__ unsigned long long warp_sum_u64(unsigned long long v)
   return v;
 }
 
+// The environment maps of one relighting launch, passed by value in the kernel parameters
+struct EnvTable {
+  TirEnvMap e[TIR_RELIGHT_MAX_LIGHTS];
+};
+
+// Warp-aggregated append of this lane's (o, d) row to a visibility list of `capacity` rows, one atomic per warp.
+// -> the row, or -1 when the lane does not append or its row is at or past capacity (count still counts it).
+// All 32 lanes of the warp must call it: lanes with nothing to append pass append = false.
+__device__ __forceinline__ int32_t list_append(float* list_o, float* list_d, int64_t capacity,
+                                               unsigned long long* count, bool append, const float o[3],
+                                               const float d[3]) {
+  const int lane = threadIdx.x & 31;
+  const unsigned ballot = __ballot_sync(0xffffffffu, append);
+  unsigned long long base = 0;
+  if (ballot) {
+    const int leader = __ffs(ballot) - 1;
+    if (lane == leader) base = atomicAdd(count, (unsigned long long)__popc(ballot));
+    base = __shfl_sync(0xffffffffu, base, leader);
+  }
+  if (!append) return -1;
+  const long long row = (long long)(base + __popc(ballot & ((1u << lane) - 1u)));
+  if (row >= capacity) return -1;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) { list_o[row * 3 + c] = o[c]; list_d[row * 3 + c] = d[c]; }
+  return (int32_t)row;
+}
+
 }  // namespace tir

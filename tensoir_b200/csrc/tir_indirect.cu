@@ -26,10 +26,6 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kWarps = 8;
 
-struct EnvTable {
-  TirEnvMap e[TIR_RELIGHT_MAX_LIGHTS];
-};
-
 struct SampleParams {
   const float* rays; const float* depth; const float* normal; const float* albedo; const float* rough;
   int rough_stride; const float* fresnel; const float* acc;
@@ -44,7 +40,6 @@ struct SampleParams {
 __global__ void __launch_bounds__(kThreads) indirect_sample_kernel(const __grid_constant__ SampleParams p) {
   const int64_t total = p.n * p.K;
   const int64_t t = (int64_t)blockIdx.x * kThreads + threadIdx.x;
-  const int lane = threadIdx.x & 31;
   bool append = false;
   float o[3], om[3] = {0.f, 0.f, 0.f}, T[3] = {0.f, 0.f, 0.f};
   if (t < total) {
@@ -60,24 +55,8 @@ __global__ void __launch_bounds__(kThreads) indirect_sample_kernel(const __grid_
       if (append) rl_surface(p.rays + i * 6, p.depth[i], o);
     }
   }
-  // warp-aggregated append: one atomic per warp
-  const unsigned ballot = __ballot_sync(0xffffffffu, append);
-  unsigned long long base = 0;
-  if (ballot) {
-    const int leader = __ffs(ballot) - 1;
-    if (lane == leader) base = atomicAdd(p.count, (unsigned long long)__popc(ballot));
-    base = __shfl_sync(0xffffffffu, base, leader);
-  }
+  const int32_t slot = list_append(p.list_o, p.list_d, p.capacity, p.count, append, o, om);
   if (t >= total) return;
-  int32_t slot = -1;
-  if (append) {
-    const long long row = (long long)(base + __popc(ballot & ((1u << lane) - 1u)));
-    if (row < p.capacity) {
-      slot = (int32_t)row;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) { p.list_o[row * 3 + c] = o[c]; p.list_d[row * 3 + c] = om[c]; }
-    }
-  }
 #pragma unroll
   for (int c = 0; c < 3; ++c) { p.dir[t * 3 + c] = om[c]; p.T[t * 3 + c] = T[c]; }
   p.pos[t] = slot;
@@ -249,8 +228,8 @@ extern "C" int tir_indirect_sample(const float* rays, const float* depth, const 
       !count)
     return TIR_ERR_NULL;
   if (rough_stride != 1 && rough_stride != 3) return TIR_ERR_SHAPE;
-  if (capacity < 0 || capacity > INT32_MAX) return TIR_ERR_SHAPE;
-  if (capacity > 0 && (!list_o || !list_d)) return TIR_ERR_NULL;
+  const int lrc = rl_check_list(capacity, list_o, list_d);
+  if (lrc) return lrc;
   if (n == 0) return TIR_OK;
   SampleParams p{};
   p.rays = rays; p.depth = depth; p.normal = normal; p.albedo = albedo; p.rough = rough; p.rough_stride = rough_stride;

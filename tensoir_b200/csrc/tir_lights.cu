@@ -36,7 +36,6 @@ struct LightsSampleParams {
 __global__ void __launch_bounds__(kSampleThreads) lights_sample_kernel(const __grid_constant__ LightsSampleParams p) {
   const int64_t total = p.n * p.lt.prefix[p.n_lights];
   const int64_t t = (int64_t)blockIdx.x * kSampleThreads + threadIdx.x;
-  const int lane = threadIdx.x & 31;
   bool append = false;
   float o[3], L3[3] = {0.f, 0.f, 0.f}, fall = 0.f;
   if (t < total) {
@@ -52,24 +51,8 @@ __global__ void __launch_bounds__(kSampleThreads) lights_sample_kernel(const __g
       append = rl_cosine(L3, nrm) > 1e-6f && fall > 0.f;
     }
   }
-  // warp-aggregated append: one atomic per warp
-  const unsigned ballot = __ballot_sync(0xffffffffu, append);
-  unsigned long long base = 0;
-  if (ballot) {
-    const int leader = __ffs(ballot) - 1;
-    if (lane == leader) base = atomicAdd(p.count, (unsigned long long)__popc(ballot));
-    base = __shfl_sync(0xffffffffu, base, leader);
-  }
+  const int32_t slot = list_append(p.list_o, p.list_d, p.capacity, p.count, append, o, L3);
   if (t >= total) return;
-  int32_t slot = -1;
-  if (append) {
-    const long long row = (long long)(base + __popc(ballot & ((1u << lane) - 1u)));
-    if (row < p.capacity) {
-      slot = (int32_t)row;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) { p.list_o[row * 3 + c] = o[c]; p.list_d[row * 3 + c] = L3[c]; }
-    }
-  }
 #pragma unroll
   for (int c = 0; c < 3; ++c) p.L[t * 3 + c] = L3[c];
   p.falloff[t] = fall;
@@ -106,7 +89,7 @@ __global__ void __launch_bounds__(kWarps * 32) lights_shade_kernel(const __grid_
       for (int s = lane; s < K; s += 32) {
         const int q = p.pos[k0 + s];
         if (q < 0) continue;
-        const float vis = p.vis_kind ? 1.f - p.vis[q] : p.vis[q];
+        const float vis = rl_vis(p.vis, p.vis_kind, q);
         const float Ld[3] = {p.L[(k0 + s) * 3], p.L[(k0 + s) * 3 + 1], p.L[(k0 + s) * 3 + 2]};
         lt_contrib(c, Ld, p.falloff[k0 + s], vis, acc);
       }
@@ -137,8 +120,8 @@ extern "C" int tir_lights_sample(const TirLight* lights, int32_t n_lights, const
   const int rc = lt_validate(lights, n_lights, n, p.lt);
   if (rc <= 0) return rc;
   if (!rays || !depth || !normal || !acc || !u || !L || !falloff || !pos || !count) return TIR_ERR_NULL;
-  if (capacity < 0 || capacity > INT32_MAX) return TIR_ERR_SHAPE;
-  if (capacity > 0 && (!list_o || !list_d)) return TIR_ERR_NULL;
+  const int lrc = rl_check_list(capacity, list_o, list_d);
+  if (lrc) return lrc;
   p.n_lights = n_lights;
   p.rays = rays; p.depth = depth; p.normal = normal; p.acc = acc; p.n = n; p.thr = acc_mask_threshold; p.u = u;
   p.L = L; p.falloff = falloff; p.pos = pos; p.list_o = list_o; p.list_d = list_d; p.capacity = capacity;

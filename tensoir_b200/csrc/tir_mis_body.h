@@ -199,7 +199,7 @@ RL_HD void mis_lane(const TirEnvMap& e, const tir::PointCtx& c, const MisPoint& 
     int b;
     const float pdf = mis_denominator(e, c, m, S_l, S_b, w, b);
     if (!(pdf > 0.f)) continue;
-    const float vis = vis_kind ? 1.f - vis_list[q] : vis_list[q];
+    const float vis = rl_vis(vis_list, vis_kind, q);
     float rgb[3];
     for (int ch = 0; ch < 3; ++ch) rgb[ch] = RL_LDG(e.rgb + (int64_t)b * 3 + ch);
     rl_contrib(c, w, rgb, pdf, vis, acc);

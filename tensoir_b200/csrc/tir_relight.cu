@@ -21,10 +21,6 @@ namespace {
 constexpr int kSampleThreads = 256;
 constexpr int kWarps = 8;
 
-struct EnvTable {
-  TirEnvMap e[TIR_RELIGHT_MAX_LIGHTS];
-};
-
 struct SampleParams {
   EnvTable env;
   const float* rays; const float* depth; const float* normal; const float* acc;
@@ -39,7 +35,6 @@ struct SampleParams {
 __global__ void __launch_bounds__(kSampleThreads) relight_sample_kernel(const SampleParams p, int L) {
   const int64_t total = (int64_t)L * p.n * p.S;
   const int64_t t = (int64_t)blockIdx.x * kSampleThreads + threadIdx.x;
-  const int lane = threadIdx.x & 31;
   bool append = false;
   float o[3], L3[3];
   int b = 0;
@@ -57,24 +52,8 @@ __global__ void __launch_bounds__(kSampleThreads) relight_sample_kernel(const Sa
       if (append) rl_surface(p.rays + i * 6, p.depth[i], o);
     }
   }
-  // warp-aggregated append: one atomic per warp
-  const unsigned ballot = __ballot_sync(0xffffffffu, append);
-  unsigned long long base = 0;
-  if (ballot) {
-    const int leader = __ffs(ballot) - 1;
-    if (lane == leader) base = atomicAdd(p.count, (unsigned long long)__popc(ballot));
-    base = __shfl_sync(0xffffffffu, base, leader);
-  }
+  const int32_t slot = list_append(p.list_o, p.list_d, p.capacity, p.count, append, o, L3);
   if (t >= total) return;
-  int32_t slot = -1;
-  if (append) {
-    const long long row = (long long)(base + __popc(ballot & ((1u << lane) - 1u)));
-    if (row < p.capacity) {
-      slot = (int32_t)row;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) { p.list_o[row * 3 + c] = o[c]; p.list_d[row * 3 + c] = L3[c]; }
-    }
-  }
   p.bin[t] = b;
   p.pos[t] = slot;
 }
@@ -127,9 +106,8 @@ extern "C" int tir_relight_sample(const TirEnvMap* envs, int32_t n_lights, const
   const int rc = rl_validate(envs, n_lights, n, n_samples);
   if (rc <= 0 || n_samples == 0) return rc < 0 ? rc : TIR_OK;
   if (!rays || !depth || !normal || !acc || !u || !bin || !pos || !count) return TIR_ERR_NULL;
-  if (capacity < 0) return TIR_ERR_SHAPE;
-  if (capacity > 0 && (!list_o || !list_d)) return TIR_ERR_NULL;
-  if (capacity > INT32_MAX) return TIR_ERR_SHAPE;
+  const int lrc = rl_check_list(capacity, list_o, list_d);
+  if (lrc) return lrc;
   SampleParams p{};
   for (int l = 0; l < n_lights; ++l) p.env.e[l] = envs[l];
   p.rays = rays; p.depth = depth; p.normal = normal; p.acc = acc; p.n = n; p.S = n_samples;

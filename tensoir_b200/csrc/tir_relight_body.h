@@ -92,6 +92,11 @@ RL_HD void rl_contrib(const tir::PointCtx& c, const float L[3], const float rgb[
 #define RL_LDG(p) (*(p))
 #endif
 
+// Visibility of list row q as relight() reads it from the march: vis_kind 0 (nerv) t_last, 1 (nerfactor) 1 - acc
+RL_HD float rl_vis(const float* vis_list, int vis_kind, int q) {
+  return vis_kind ? 1.f - vis_list[q] : vis_list[q];
+}
+
 // The direct per-sample loop of one (map, point): lane `lane` of `lanes` adds rl_contrib of samples lane, lane + lanes,
 // ... (bin and list row from bin[] / pos[], vis as relight() reads it from the march) to acc[3].  The kernels run it on
 // the 32 lanes of a warp and reduce with warp_sum; the host builds run the 32 lanes in turn and reduce with the same
@@ -102,7 +107,7 @@ RL_HD void rl_direct_lane(const TirEnvMap& e, const tir::PointCtx& c, const int3
     const int b = bin[s];
     const int q = pos[s];
     float vis = 0.f;
-    if (q >= 0) vis = vis_kind ? 1.f - vis_list[q] : vis_list[q];
+    if (q >= 0) vis = rl_vis(vis_list, vis_kind, q);
     float Ld[3], rgb[3];
     for (int ch = 0; ch < 3; ++ch) { Ld[ch] = RL_LDG(e.dir + (int64_t)b * 3 + ch); rgb[ch] = RL_LDG(e.rgb + (int64_t)b * 3 + ch); }
     rl_contrib(c, Ld, rgb, RL_LDG(e.pdf_return + b), vis, acc);
@@ -129,4 +134,12 @@ inline int rl_validate(const TirEnvMap* envs, int32_t n_lights, int64_t n, int32
     if (!envs[l].rgb || !envs[l].dir || !envs[l].pdf_return || !envs[l].cdf) return TIR_ERR_NULL;
   }
   return 1;
+}
+
+// argument checks of a visibility list (list_o, list_d: capacity rows of 3), shared by every tir_*_sample entry and
+// its host build: TIR_OK or a TirStatus
+inline int rl_check_list(int64_t capacity, const float* list_o, const float* list_d) {
+  if (capacity < 0 || capacity > INT32_MAX) return TIR_ERR_SHAPE;
+  if (capacity > 0 && (!list_o || !list_d)) return TIR_ERR_NULL;
+  return TIR_OK;
 }

@@ -21,10 +21,6 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kWarps = 8;
 
-struct EnvTable {
-  TirEnvMap e[TIR_RELIGHT_MAX_LIGHTS];
-};
-
 struct SampleParams {
   EnvTable env;
   const float* rays; const float* depth; const float* normal; const float* albedo; const float* rough;
@@ -41,7 +37,6 @@ __global__ void __launch_bounds__(kThreads) mis_sample_kernel(const __grid_const
   const int64_t n_light = (int64_t)L * p.n * p.S_l;
   const int64_t total = n_light + p.n * p.S_b;
   const int64_t t = (int64_t)blockIdx.x * kThreads + threadIdx.x;
-  const int lane = threadIdx.x & 31;
   bool append = false;
   float o[3], w[3] = {0.f, 0.f, 0.f};
   if (t < total) {
@@ -65,24 +60,8 @@ __global__ void __launch_bounds__(kThreads) mis_sample_kernel(const __grid_const
       if (append) rl_surface(p.rays + i * 6, p.depth[i], o);
     }
   }
-  // warp-aggregated append: one atomic per warp
-  const unsigned ballot = __ballot_sync(0xffffffffu, append);
-  unsigned long long base = 0;
-  if (ballot) {
-    const int leader = __ffs(ballot) - 1;
-    if (lane == leader) base = atomicAdd(p.count, (unsigned long long)__popc(ballot));
-    base = __shfl_sync(0xffffffffu, base, leader);
-  }
+  const int32_t slot = list_append(p.list_o, p.list_d, p.capacity, p.count, append, o, w);
   if (t >= total) return;
-  int32_t slot = -1;
-  if (append) {
-    const long long row = (long long)(base + __popc(ballot & ((1u << lane) - 1u)));
-    if (row < p.capacity) {
-      slot = (int32_t)row;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) { p.list_o[row * 3 + c] = o[c]; p.list_d[row * 3 + c] = w[c]; }
-    }
-  }
 #pragma unroll
   for (int c = 0; c < 3; ++c) p.dir[t * 3 + c] = w[c];
   p.pos[t] = slot;
@@ -147,12 +126,14 @@ extern "C" int tir_relight_mis_sample(const TirEnvMap* envs, int32_t n_lights, c
                                       int64_t capacity, int64_t* count, void* stream) {
   const int rc = mis_validate(envs, n_lights, n, S_l, S_b, rough_stride);
   if (rc < 0) return rc;
-  if (capacity < 0 || capacity > INT32_MAX) return TIR_ERR_SHAPE;
+  // a bad capacity fails even with nothing to do; missing lists only when there is
+  const int lrc = rl_check_list(capacity, list_o, list_d);
+  if (lrc == TIR_ERR_SHAPE) return lrc;
   if (rc == 0) return TIR_OK;
   if (!rays || !depth || !normal || !albedo || !rough || !fresnel || !acc || !u_light || !dir || !pos || !count)
     return TIR_ERR_NULL;
   if (S_b > 0 && !u_brdf) return TIR_ERR_NULL;
-  if (capacity > 0 && (!list_o || !list_d)) return TIR_ERR_NULL;
+  if (lrc) return lrc;
   SampleParams p{};
   for (int l = 0; l < n_lights; ++l) p.env.e[l] = envs[l];
   p.rays = rays; p.depth = depth; p.normal = normal; p.albedo = albedo; p.rough = rough; p.rough_stride = rough_stride;

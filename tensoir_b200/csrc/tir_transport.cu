@@ -32,7 +32,6 @@ struct TransportSampleParams {
 __global__ void __launch_bounds__(kSampleThreads) transport_sample_kernel(const __grid_constant__ TransportSampleParams p) {
   const int64_t total = p.n * p.K;
   const int64_t t = (int64_t)blockIdx.x * kSampleThreads + threadIdx.x;
-  const int lane = threadIdx.x & 31;
   bool append = false;
   float o[3], L3[3];
   if (t < total) {
@@ -46,24 +45,8 @@ __global__ void __launch_bounds__(kSampleThreads) transport_sample_kernel(const 
       if (append) rl_surface(p.rays + i * 6, p.depth[i], o);
     }
   }
-  // warp-aggregated append: one atomic per warp
-  const unsigned ballot = __ballot_sync(0xffffffffu, append);
-  unsigned long long base = 0;
-  if (ballot) {
-    const int leader = __ffs(ballot) - 1;
-    if (lane == leader) base = atomicAdd(p.count, (unsigned long long)__popc(ballot));
-    base = __shfl_sync(0xffffffffu, base, leader);
-  }
+  const int32_t slot = list_append(p.list_o, p.list_d, p.capacity, p.count, append, o, L3);
   if (t >= total) return;
-  int32_t slot = -1;
-  if (append) {
-    const long long row = (long long)(base + __popc(ballot & ((1u << lane) - 1u)));
-    if (row < p.capacity) {
-      slot = (int32_t)row;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) { p.list_o[row * 3 + c] = o[c]; p.list_d[row * 3 + c] = L3[c]; }
-    }
-  }
   p.pos[t] = slot;
 }
 
@@ -96,7 +79,7 @@ __global__ void __launch_bounds__(kWarps * 32) transport_build_kernel(const __gr
     const int q = pos[k];
     float t[3] = {0.f, 0.f, 0.f};
     if (q >= 0) {
-      const float vis = p.vis_kind ? 1.f - p.vis[q] : p.vis[q];
+      const float vis = rl_vis(p.vis, p.vis_kind, q);
       const float L[3] = {__ldg(p.dirs + (int64_t)k * 3), __ldg(p.dirs + (int64_t)k * 3 + 1),
                           __ldg(p.dirs + (int64_t)k * 3 + 2)};
       tt_contrib(c, L, __ldg(p.domega + k), vis, t);
@@ -116,8 +99,8 @@ extern "C" int tir_transport_sample(const float* dirs, int32_t K, const float* r
   const int rc = tt_validate(K, n);
   if (rc <= 0) return rc;
   if (!dirs || !rays || !depth || !normal || !acc || !pos || !count) return TIR_ERR_NULL;
-  if (capacity < 0 || capacity > INT32_MAX) return TIR_ERR_SHAPE;
-  if (capacity > 0 && (!list_o || !list_d)) return TIR_ERR_NULL;
+  const int lrc = rl_check_list(capacity, list_o, list_d);
+  if (lrc) return lrc;
   TransportSampleParams p{};
   p.dirs = dirs; p.K = K; p.rays = rays; p.depth = depth; p.normal = normal; p.acc = acc; p.n = n;
   p.thr = acc_mask_threshold; p.pos = pos; p.list_o = list_o; p.list_d = list_d; p.capacity = capacity;

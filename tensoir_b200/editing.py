@@ -173,7 +173,7 @@ def edit_materials(maps, edits, scale, thr, points=None, rays=None):
         points, depth_p, rays_p = f32(points), None, None
     else:
         points, depth_p, rays_p = None, f32(depth).reshape(-1), f32(rays)
-    scale = torch.as_tensor(scale, dtype=torch.float32).to(dev).reshape(-1).expand(3).contiguous()
+    scale = R.rescale3(scale, dev)
     table = rule_table(edits)
     a_out, r_out, f_out = torch.empty_like(albedo), torch.empty_like(rough), torch.empty_like(fresnel)
     sel = torch.empty(n, dtype=torch.int32, device=dev)
@@ -200,48 +200,42 @@ def relight_edited(dataset, args, variants, tensoIR=None, include_original=True)
     relight()'s format.  Per-light videos go to {geo_buffer_path}/{variant}/video_{with,without}_bg/ when imageio is
     installed.  Returns {variant: {light: [PSNR per view]}} (empty lists without rgbs)."""
     from .relight import Environment_Light
-    from .evaluation import _lpips, compute_rescale_ratio
+    from .evaluation import compute_rescale_ratio
     runs = ([(ORIGINAL, [])] if include_original else []) + list(load_edits(variants).items())
     if not runs:
         raise ValueError("no variant to render")
     opt = {k: getattr(args, k, v) for k, v in R.SCRIPT_DEFAULTS.items()}
+    tensoIR, device = R._model(args, tensoIR)
     if tensoIR is None:
-        tensoIR = R._load_model(args, torch.device("cuda"))
-        if tensoIR is None:
-            return None
-    device = tensoIR.device if hasattr(tensoIR, "device") else torch.device("cuda")
+        return None
     W, H = dataset.img_wh
     if H < 11 or W < 11:
         raise ValueError(f"SSIM needs images of at least 11x11 pixels, got {W}x{H}")
     names = list(dataset.light_names)
-    L, S, G = len(names), R.NUM_SAMPLES, _lib.RELIGHT_MAX_LIGHTS
+    L, S = len(names), R.NUM_SAMPLES
     thr = float(opt["acc_mask_threshold"])
     vis_eq = opt["vis_equation"]
-    if vis_eq not in ('nerv', 'nerfactor'):
-        raise ValueError(vis_eq)
+    R.vis_kind(vis_eq)
     envir_light = Environment_Light(args.hdrdir, device=device)
     envs, keep = R.env_tables(envir_light, names)
     _, rescale_value = compute_rescale_ratio(tensoIR, dataset)
-    scale = torch.as_tensor(rescale_value, dtype=torch.float32).to(device).reshape(-1).expand(3).contiguous()
+    scale = R.rescale3(rescale_value, device)
     ones = torch.ones(3, device=device)
     gp = args.geo_buffer_path
     V = len(runs)
-    metrics = {v: {k: {n: [] for n in names} for k in ("psnr", "ssim", "alex", "vgg")} for v, _ in runs}
+    metrics = {v: R._new_metrics(names) for v, _ in runs}
     for idx in range(len(dataset)):
         view_dir = os.path.join(gp, f'{dataset.split}_{idx:0>3d}')
         item = dataset[idx]
         frame_rays = item['rays'].squeeze(0).to(device)
         n_pix = frame_rays.shape[0]
-        light_idx = torch.zeros((n_pix, 1), dtype=torch.int32, device=device)
         with_map = torch.empty(V, L, n_pix, 3, device=device)
         without_map = torch.empty(V, L, n_pix, 3, device=device)
         alb = torch.empty(V, n_pix, 3, device=device)
         sel = torch.empty(V, n_pix, dtype=torch.int32, device=device)
         acc_v, rgh = torch.empty(n_pix, device=device), None
-        for s in range(0, n_pix, args.batch_size):
-            e = min(s + args.batch_size, n_pix)
-            _, depth, normal, albedo, rough, fresnel, acc, *_ = tensoIR(
-                frame_rays[s:e], light_idx[s:e], is_train=False, white_bg=True, ndc_ray=False, N_samples=-1)
+        for s, e, (_, depth, normal, albedo, rough, fresnel, acc, *_) in R._primary_chunks(tensoIR, frame_rays,
+                                                                                           args.batch_size):
             rays, maps = R.chunk_inputs(frame_rays[s:e], (depth, normal, albedo, rough, fresnel, acc))
             depth, normal, albedo, rough, fresnel, acc = maps
             acc_v[s:e] = acc
@@ -251,29 +245,21 @@ def relight_edited(dataset, args, variants, tensoIR=None, include_original=True)
             if tuple(u.shape) != (L, e - s, S) or u.dtype != torch.float64:
                 raise ValueError(f"u must be float64 [{L}, {e - s}, {S}], got {u.dtype} {tuple(u.shape)}")
             u = u.to(device).contiguous()
-            groups = [(g, min(G, L - g)) for g in range(0, L, G)]
-            vis = [R.relight_visibility(tensoIR, R.env_group(envs, g), Lg, rays, depth, normal, acc,
-                                        u[g:g + Lg].contiguous(), S, thr, vis_eq) for g, Lg in groups]
+            groups = list(R.env_groups(envs, L))
+            vis = [R.relight_visibility(tensoIR, eg, Lg, rays, depth, normal, acc, u[g:g + Lg].contiguous(), S, thr,
+                                        vis_eq) for g, Lg, eg in groups]
             for v, (_, rules) in enumerate(runs):
                 a_o, r_o, f_o, sel_o = edit_materials(maps, rules, scale, thr, rays=rays)
                 alb[v, s:e], rgh[v, s:e], sel[v, s:e] = a_o, r_o, sel_o
-                for (g, Lg), vs in zip(groups, vis):
-                    R.relight_shade(R.env_group(envs, g), Lg, rays, normal, a_o, r_o, f_o, acc, S, thr, ones, vs,
-                                    vis_eq, (with_map[v, g:g + Lg], without_map[v, g:g + Lg]), s)
+                for (g, Lg, eg), vs in zip(groups, vis):
+                    R.relight_shade(eg, Lg, rays, normal, a_o, r_o, f_o, acc, S, thr, ones, vs, vis_eq,
+                                    (with_map[v, g:g + Lg], without_map[v, g:g + Lg]), s)
 
-        acc_t = acc_v.clone()
-        acc_t[acc_t <= 0.9] = 0.0           # relight()'s thresholded acc (the reference's in-place acc_temp)
-        acc_u8 = (acc_t.reshape(H, W, 1) * 255).to(torch.uint8).cpu().numpy()
+        acc_u8 = R._acc_u8(acc_v, H, W)
         gt_rgb = item['rgbs'].squeeze(0).reshape(L, H * W, 3).to(device) if 'rgbs' in item else None
         for v, (vname, _) in enumerate(runs):
             d = os.path.join(view_dir, vname)
-            for sub in ('with_bg', 'without_bg'):
-                os.makedirs(os.path.join(d, f'relighting_{sub}'), exist_ok=True)
-            u8w = (with_map[v] * 255).to(torch.uint8).reshape(L, H, W, 3).cpu().numpy()
-            u8o = (without_map[v] * 255).to(torch.uint8).reshape(L, H, W, 3).cpu().numpy()
-            for k, name in enumerate(names):
-                R._imwrite(os.path.join(d, 'relighting_with_bg', f'{name}.png'), u8w[k])
-                R._imwrite(os.path.join(d, 'relighting_without_bg', f'{name}.png'), u8o[k])
+            R._write_pairs(d, names, H, W, with_map[v], without_map[v])
             gamma_u8 = (alb[v].clamp(0.0, 1.0).reshape(H, W, 3) ** (1 / 2.2) * 255).to(torch.uint8).cpu().numpy()
             R._imwrite(os.path.join(d, 'albedo_gamma_corrected.png'), np.concatenate([gamma_u8, acc_u8], axis=2))
             r = rgh[v].reshape(H, W, -1).expand(-1, -1, 3) * 255
@@ -283,18 +269,8 @@ def relight_edited(dataset, args, variants, tensoIR=None, include_original=True)
                        .numpy())
             if gt_rgb is None:
                 continue
-            m = metrics[vname]
-            met = R.pair_metrics(without_map[v], gt_rgb, H, W).cpu().numpy()
-            for k, name in enumerate(names):
-                m["psnr"][name].append(-10.0 * np.log(met[k, 0] / (H * W * 3)) / np.log(10.0))
-                m["ssim"][name].append(float(met[k, 1]))
-                img, gt_img = without_map[v, k].reshape(H, W, 3), gt_rgb[k].reshape(H, W, 3)
-                m["alex"][name].append(_lpips(gt_img, img, 'alex', device))
-                m["vgg"][name].append(_lpips(gt_img, img, 'vgg', device))
-            with open(os.path.join(d, 'relighting_without_bg', 'relight_psnr.txt'), 'w') as f:
-                for name in names:
-                    f.write(f'{name}: PNSR {m["psnr"][name][-1]}; SSIM {m["ssim"][name][-1]}; '
-                            f'L_Alex {m["alex"][name][-1]}; L_VGG {m["vgg"][name][-1]}\n')
+            R._view_metrics(metrics[vname], names, without_map[v], gt_rgb, H, W, device,
+                            os.path.join(d, 'relighting_without_bg', 'relight_psnr.txt'))
     del keep
 
     for vname, _ in runs:
@@ -302,17 +278,12 @@ def relight_edited(dataset, args, variants, tensoIR=None, include_original=True)
         vdir = os.path.join(gp, vname)
         os.makedirs(vdir, exist_ok=True)
         if len(dataset) and all(m["psnr"][n] for n in names):
-            with open(os.path.join(vdir, 'relight_psnr.txt'), 'w') as f:
-                for name in names:
-                    f.write(f'{name}:  PSNR {np.mean(m["psnr"][name])}; SSIM {np.mean(m["ssim"][name])}; '
-                            f'L_Alex {np.mean(m["alex"][name])}; L_VGG {np.mean(m["vgg"][name])}\n')
+            R._run_metrics(m, names, os.path.join(vdir, 'relight_psnr.txt'))
         if opt["render_video"]:
             for sub in ('without_bg', 'with_bg'):
                 vp = os.path.join(vdir, f'video_{sub}')
                 os.makedirs(vp, exist_ok=True)
                 for name in names:
-                    R._mimsave(os.path.join(vp, f'{name}_video.mp4'),
-                               lambda vname=vname, sub=sub, name=name: [
-                                   R._imread(os.path.join(gp, f'{dataset.split}_{i:0>3d}', vname, f'relighting_{sub}',
-                                                          f'{name}.png')) for i in range(len(dataset))])
+                    R._video(os.path.join(vp, f'{name}_video.mp4'), gp, dataset.split, len(dataset),
+                             os.path.join(vname, f'relighting_{sub}', f'{name}.png'))
     return {v: metrics[v]["psnr"] for v, _ in runs}

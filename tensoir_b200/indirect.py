@@ -29,9 +29,9 @@ import ctypes as C
 import torch
 import torch.nn.functional as F
 
-from . import _lib, ops
-from .relighting import chunk_inputs, env_group, env_tables, relight_visibility, slot_order
-
+from . import _lib, ops  # noqa: F401  (indirect.ops.march_density is where callers substitute the march)
+from .relighting import (append_list, chunk_inputs, env_groups, env_tables, march_list, relight_visibility,
+                         rescale3, vis_kind)
 
 
 def point_materials(tensoIR, x, xn=None):
@@ -72,25 +72,15 @@ def secondary_hits(tensoIR, rays, depth, normal, albedo, rough, fresnel, acc, re
     dirs = torch.empty(n, K, 3, device=dev)
     T = torch.empty(n, K, 3, device=dev)
     pos = torch.empty(n, K, dtype=torch.int32, device=dev)
-    list_o = torch.empty(cap, 3, device=dev)
-    list_d = torch.empty(cap, 3, device=dev)
-    count = torch.zeros(1, dtype=torch.int64, device=dev)
-    _lib.check(lib.tir_indirect_sample(_lib.dptr(rays), _lib.dptr(depth), _lib.dptr(normal), _lib.dptr(albedo),
-                                       _lib.dptr(rough), int(rough.shape[1]), _lib.dptr(fresnel), _lib.dptr(acc), n, K,
-                                       float(acc_mask_threshold), _lib.dptr(rescale),
-                                       _lib.dptr(u, dtype=torch.float64), _lib.dptr(dirs), _lib.dptr(T),
-                                       _lib.dptr(pos, torch.int32), _lib.dptr(list_o), _lib.dptr(list_d), cap,
-                                       _lib.dptr(count, torch.int64), _lib.stream_ptr()), "tir_indirect_sample")
-    m = int(count.item())                          # sizes the secondary march
-    if m > cap:
-        raise _lib.TirError(f"secondary list overflow: {m} > {cap}")
-    if m > 0:
-        list_o, list_d = slot_order(pos, list_o[:m], list_d[:m])
-        table = ops.equal_z_table(96, 0.05, 1.5, dev)
-        t_last, acc_s, depth_s = (t.contiguous() for t in ops.march_density(
-            tensoIR, list_o[:m], list_d[:m], table=table, counters=tensoIR.__dict__.get("_tir_counters")))
-    else:
-        t_last = acc_s = depth_s = torch.zeros(1, device=dev)
+    list_o, list_d = append_list(
+        cap, dev, "secondary list", pos,
+        lambda *tail: _lib.check(lib.tir_indirect_sample(
+            _lib.dptr(rays), _lib.dptr(depth), _lib.dptr(normal), _lib.dptr(albedo), _lib.dptr(rough),
+            int(rough.shape[1]), _lib.dptr(fresnel), _lib.dptr(acc), n, K, float(acc_mask_threshold),
+            _lib.dptr(rescale), _lib.dptr(u, dtype=torch.float64), _lib.dptr(dirs), _lib.dptr(T),
+            _lib.dptr(pos, torch.int32), *tail, _lib.stream_ptr()), "tir_indirect_sample"))
+    m = int(list_o.shape[0])
+    t_last, acc_s, depth_s = march_list(tensoIR, list_o, list_d)
     hit = torch.empty(n, K, dtype=torch.int32, device=dev)
     hit_rays = torch.empty(cap, 6, device=dev)
     xn = torch.empty(cap, 3, device=dev)
@@ -100,14 +90,16 @@ def secondary_hits(tensoIR, rays, depth, normal, albedo, rough, fresnel, acc, re
     work = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=dev)
     aabb = (C.c_float * 6)(*tensoIR.aabb[0].tolist(), *tensoIR.invaabbSize.tolist())
     count_h = torch.zeros(1, dtype=torch.int64, device=dev)
-    _lib.check(lib.tir_indirect_hits(n, K, _lib.dptr(pos, torch.int32), _lib.dptr(list_o), _lib.dptr(list_d),
+    # an empty list has no rows to point at; tir_indirect_hits never reads them but takes non-null pointers
+    rows_o, rows_d = (list_o, list_d) if m else (t_last, t_last)
+    _lib.check(lib.tir_indirect_hits(n, K, _lib.dptr(pos, torch.int32), _lib.dptr(rows_o), _lib.dptr(rows_d),
                                      _lib.dptr(t_last), _lib.dptr(acc_s), _lib.dptr(depth_s),
-                                     0 if vis_equation == 'nerv' else 1, aabb, _lib.dptr(hit_rays), _lib.dptr(xn),
+                                     vis_kind(vis_equation), aabb, _lib.dptr(hit_rays), _lib.dptr(xn),
                                      _lib.dptr(w), _lib.dptr(hit, torch.int32), cap, _lib.dptr(count_h, torch.int64),
                                      _lib.dptr(work, torch.uint8), nbytes.value, _lib.stream_ptr()),
                "tir_indirect_hits")
     m_h = int(count_h.item())                      # sizes the material query and the secondary light
-    return dict(dirs=dirs, T=T, pos=pos, list_o=list_o[:m], list_d=list_d[:m], t_last=t_last[:m], acc=acc_s[:m],
+    return dict(dirs=dirs, T=T, pos=pos, list_o=list_o, list_d=list_d, t_last=t_last[:m], acc=acc_s[:m],
                 depth=depth_s[:m], hit=hit, rays=hit_rays[:m_h], xn=xn[:m_h], w=w[:m_h])
 
 
@@ -124,7 +116,7 @@ def secondary_radiance(tensoIR, envs, L, hits, mats, rescale, Lo, h0, u2, vis_eq
     _lib.check(lib.tir_indirect_radiance(envs, L, _lib.dptr(rays), _lib.dptr(normal), _lib.dptr(albedo),
                                          _lib.dptr(rough), int(rough.shape[1]), _lib.dptr(fresnel), m, S2,
                                          _lib.dptr(rescale), _lib.dptr(bins, torch.int32), _lib.dptr(pos, torch.int32),
-                                         _lib.dptr(vis), 0 if vis_equation == 'nerv' else 1, _lib.dptr(Lo),
+                                         _lib.dptr(vis), vis_kind(vis_equation), _lib.dptr(Lo),
                                          int(Lo.shape[1]), int(h0), _lib.stream_ptr()), "tir_indirect_radiance")
 
 
@@ -139,8 +131,7 @@ def relight_chunk_indirect(tensoIR, envir_light, light_names, rays, maps, rescal
     points [m,3] -> (normal, albedo, rough [m,1], fresnel); None is point_materials.  ``indirect_out`` [L, R, 3]
     receives the un-toned indirect term at rows row0.. (0 on rows without a secondary hit).
     -> (with_bg, without_bg) [L, n, 3], as relight_chunk_fused."""
-    if vis_equation not in ('nerv', 'nerfactor'):
-        raise ValueError(vis_equation)
+    kind = vis_kind(vis_equation)
     K, S2 = int(indirect_samples), int(indirect_light_samples)
     if not (1 <= K <= 1024 and 1 <= S2 <= 1024):
         raise ValueError(f"indirect_samples and indirect_light_samples must be in [1, 1024], got {K}, {S2}")
@@ -158,9 +149,8 @@ def relight_chunk_indirect(tensoIR, envir_light, light_names, rays, maps, rescal
     if n == 0 or L == 0:
         return with_bg[:, row0:row0 + n], without_bg[:, row0:row0 + n]
     envs, keep = tables if tables is not None else env_tables(envir_light, light_names)
-    resc = torch.as_tensor(rescale_value, dtype=torch.float32).to(dev).reshape(-1).expand(3).contiguous()
+    resc = rescale3(rescale_value, dev)
     thr = float(acc_mask_threshold)
-    G = _lib.RELIGHT_MAX_LIGHTS
 
     # the map-independent half: one secondary march and one material query for every map
     u_ind = torch.rand(n, K, 2, generator=gen, device=dev, dtype=torch.float64)
@@ -176,25 +166,22 @@ def relight_chunk_indirect(tensoIR, envir_light, light_names, rays, maps, rescal
         for h0 in range(0, m_h, step):
             m = min(step, m_h - h0)
             u2 = torch.rand(L, m, S2, generator=gen, device=dev, dtype=torch.float64)
-            for g in range(0, L, G):
-                secondary_radiance(tensoIR, env_group(envs, g), min(G, L - g), hits, mats, resc, Lo[g:g + G], h0,
-                                   u2[g:g + G], vis_equation)
+            for g, Lg, eg in env_groups(envs, L):
+                secondary_radiance(tensoIR, eg, Lg, hits, mats, resc, Lo[g:g + Lg], h0, u2[g:g + Lg], vis_equation)
 
     lib = _lib.load()
-    for g in range(0, L, G):
-        Lg = min(G, L - g)
-        eg = env_group(envs, g)
-        bins, pos, vis = relight_visibility(tensoIR, eg, Lg, rays, depth, normal, acc, u[g:g + G], S, thr,
+    for g, Lg, eg in env_groups(envs, L):
+        bins, pos, vis = relight_visibility(tensoIR, eg, Lg, rays, depth, normal, acc, u[g:g + Lg], S, thr,
                                             vis_equation, ordered=True)
-        ind = indirect_out[g:g + G] if indirect_out is not None else None
+        ind = indirect_out[g:g + Lg] if indirect_out is not None else None
         _lib.check(lib.tir_indirect_shade(eg, Lg, _lib.dptr(rays), _lib.dptr(normal), _lib.dptr(albedo),
                                           _lib.dptr(rough), int(rough.shape[1]), _lib.dptr(fresnel), _lib.dptr(acc), n,
                                           S, thr, _lib.dptr(resc), _lib.dptr(bins, torch.int32),
-                                          _lib.dptr(pos, torch.int32), _lib.dptr(vis),
-                                          0 if vis_equation == 'nerv' else 1, K, _lib.dptr(hits["T"]),
-                                          _lib.dptr(hits["hit"], torch.int32), _lib.dptr(hits["w"]),
-                                          _lib.dptr(Lo[g:g + G]), m_h, _lib.dptr(with_bg[g:g + G]),
-                                          _lib.dptr(without_bg[g:g + G]), _lib.dptr(ind, allow_none=True),
+                                          _lib.dptr(pos, torch.int32), _lib.dptr(vis), kind, K,
+                                          _lib.dptr(hits["T"]), _lib.dptr(hits["hit"], torch.int32),
+                                          _lib.dptr(hits["w"]), _lib.dptr(Lo[g:g + Lg]), m_h,
+                                          _lib.dptr(with_bg[g:g + Lg]), _lib.dptr(without_bg[g:g + Lg]),
+                                          _lib.dptr(ind, allow_none=True),
                                           int(with_bg.shape[1]), int(row0), _lib.stream_ptr()), "tir_indirect_shade")
     del keep
     return with_bg[:, row0:row0 + n], without_bg[:, row0:row0 + n]

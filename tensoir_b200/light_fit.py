@@ -31,7 +31,7 @@ import types
 import numpy as np
 import torch
 
-from . import _lib, ops
+from . import _lib
 from . import relighting as R
 
 FIT_RES = (16, 32)
@@ -131,19 +131,13 @@ def transport_sample(grid, rays, depth, normal, acc, acc_mask_threshold):
     lib = _lib.load()
     dirs, _ = grid
     n, K = int(rays.shape[0]), int(dirs.shape[0])
-    cap = n * K
     pos = torch.empty(n, K, dtype=torch.int32, device=rays.device)
-    list_o = torch.empty(cap, 3, device=rays.device)
-    list_d = torch.empty(cap, 3, device=rays.device)
-    count = torch.zeros(1, dtype=torch.int64, device=rays.device)
-    _lib.check(lib.tir_transport_sample(_lib.dptr(dirs), K, _lib.dptr(rays), _lib.dptr(depth), _lib.dptr(normal),
-                                        _lib.dptr(acc), n, float(acc_mask_threshold), _lib.dptr(pos, torch.int32),
-                                        _lib.dptr(list_o), _lib.dptr(list_d), cap, _lib.dptr(count, torch.int64),
-                                        _lib.stream_ptr()), "tir_transport_sample")
-    m = int(count.item())
-    if m > cap:
-        raise _lib.TirError(f"transport visibility list overflow: {m} > {cap}")
-    return pos, list_o[:m], list_d[:m]
+    list_o, list_d = R.append_list(
+        n * K, rays.device, "transport visibility list", None,
+        lambda *tail: _lib.check(lib.tir_transport_sample(
+            _lib.dptr(dirs), K, _lib.dptr(rays), _lib.dptr(depth), _lib.dptr(normal), _lib.dptr(acc), n,
+            float(acc_mask_threshold), _lib.dptr(pos, torch.int32), *tail, _lib.stream_ptr()), "tir_transport_sample"))
+    return pos, list_o, list_d
 
 
 def transport_build(grid, rays, normal, albedo, rough, fresnel, acc, acc_mask_threshold, rescale_value, pos, vis,
@@ -154,19 +148,14 @@ def transport_build(grid, rays, normal, albedo, rough, fresnel, acc, acc_mask_th
     n, K = int(rays.shape[0]), int(dirs.shape[0])
     dev = rays.device
     T = torch.empty(3, n, K, device=dev)
-    resc = torch.as_tensor(rescale_value, dtype=torch.float32).to(dev).reshape(-1).expand(3).contiguous()
+    resc = R.rescale3(rescale_value, dev)
     _lib.check(lib.tir_transport_build(_lib.dptr(dirs), _lib.dptr(domega), K, _lib.dptr(rays), _lib.dptr(normal),
                                        _lib.dptr(albedo), _lib.dptr(rough), int(rough.shape[1]), _lib.dptr(fresnel),
                                        _lib.dptr(acc), n, float(acc_mask_threshold), _lib.dptr(resc),
-                                       _lib.dptr(pos, torch.int32), _lib.dptr(vis),
-                                       0 if vis_equation == 'nerv' else 1, _lib.dptr(T), _lib.stream_ptr()),
+                                       _lib.dptr(pos, torch.int32), _lib.dptr(vis), R.vis_kind(vis_equation),
+                                       _lib.dptr(T), _lib.stream_ptr()),
                "tir_transport_build")
     return T
-
-
-def shadow_table(device):
-    """relight()'s visibility march: 96 equal-z samples over [0.05, 1.5]."""
-    return ops.equal_z_table(96, 0.05, 1.5, device)
 
 
 @torch.no_grad()
@@ -174,14 +163,12 @@ def transport_chunk(tensoIR, rays, maps, rescale_value, grid, acc_mask_threshold
     """The transport T [3, n, K] of one chunk of primary rays to the texels of ``grid`` = texel_tables(...) on the
     device.  ``maps`` = (depth, normal, albedo, roughness [n,1] or [n,3], fresnel, acc), the tuple relight_chunk_fused
     takes.  Rows with acc <= acc_mask_threshold are 0."""
-    from .lighting import rig_march
-    if vis_equation not in ('nerv', 'nerfactor'):
-        raise ValueError(vis_equation)
+    R.vis_kind(vis_equation)
     if int(rays.shape[0]) == 0:
         return torch.zeros(3, 0, int(grid[0].shape[0]), device=rays.device)
     rays, (depth, normal, albedo, rough, fresnel, acc) = R.chunk_inputs(rays, maps)
     pos, list_o, list_d = transport_sample(grid, rays, depth, normal, acc, acc_mask_threshold)
-    vis = rig_march(tensoIR, list_o, list_d, shadow_table(rays.device), vis_equation)
+    vis = R.march_list(tensoIR, list_o, list_d, vis_equation)
     return transport_build(grid, rays, normal, albedo, rough, fresnel, acc, acc_mask_threshold, rescale_value, pos,
                            vis, vis_equation)
 
@@ -398,8 +385,7 @@ def fit_lights(dataset, args, tensoIR=None):
                seed=int(_opt(args, "seed", SEED)),
                acc_mask_threshold=float(_opt(args, "acc_mask_threshold", R.SCRIPT_DEFAULTS["acc_mask_threshold"])),
                vis_equation=_opt(args, "vis_equation", R.SCRIPT_DEFAULTS["vis_equation"]))
-    if opt["vis_equation"] not in ('nerv', 'nerfactor'):
-        raise ValueError(opt["vis_equation"])
+    R.vis_kind(opt["vis_equation"])
     smooth, ridge = float(_opt(args, "smooth", SMOOTH)), float(_opt(args, "ridge", RIDGE))
     if smooth < 0 or ridge < 0:
         raise ValueError(f"smooth and ridge must be >= 0, got {smooth}, {ridge}")

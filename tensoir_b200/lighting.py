@@ -242,33 +242,19 @@ def rig_sample(setup, rays, depth, normal, acc, u, acc_mask_threshold):
     L = torch.empty(slots, 3, device=dev)
     falloff = torch.empty(slots, device=dev)
     pos = torch.empty(slots, dtype=torch.int32, device=dev)
-    list_o = torch.empty(slots, 3, device=dev)
-    list_d = torch.empty(slots, 3, device=dev)
-    count = torch.zeros(1, dtype=torch.int64, device=dev)
-    _lib.check(lib.tir_lights_sample(light_table(setup), len(setup.lights), _lib.dptr(rays), _lib.dptr(depth),
-                                     _lib.dptr(normal), _lib.dptr(acc), n, float(acc_mask_threshold),
-                                     _lib.dptr(u, torch.float64), _lib.dptr(L), _lib.dptr(falloff),
-                                     _lib.dptr(pos, torch.int32), _lib.dptr(list_o), _lib.dptr(list_d), slots,
-                                     _lib.dptr(count, torch.int64), _lib.stream_ptr()), "tir_lights_sample")
-    m = int(count.item())
-    if m > slots:
-        raise _lib.TirError(f"shadow-ray list overflow: {m} > {slots}")
-    return L, falloff, pos, list_o[:m], list_d[:m]
-
-
-def rig_march(tensoIR, list_o, list_d, z_table, vis_equation):
-    """The density march on the shadow-ray list -> the visibility list tir_lights_shade reads."""
-    if list_o.shape[0] == 0:
-        return torch.zeros(1, device=list_o.device)
-    t_last, acc_s, _ = ops.march_density(tensoIR, list_o, list_d, table=z_table,
-                                         counters=tensoIR.__dict__.get("_tir_counters"))
-    return (t_last if vis_equation == 'nerv' else acc_s).contiguous()
+    list_o, list_d = R.append_list(
+        slots, dev, "shadow-ray list", None,
+        lambda *tail: _lib.check(lib.tir_lights_sample(
+            light_table(setup), len(setup.lights), _lib.dptr(rays), _lib.dptr(depth), _lib.dptr(normal),
+            _lib.dptr(acc), n, float(acc_mask_threshold), _lib.dptr(u, torch.float64), _lib.dptr(L),
+            _lib.dptr(falloff), _lib.dptr(pos, torch.int32), *tail, _lib.stream_ptr()), "tir_lights_sample"))
+    return L, falloff, pos, list_o, list_d
 
 
 def rig_visibility(tensoIR, setup, rays, depth, normal, acc, u, acc_mask_threshold, vis_equation, z_table):
     """The material-independent half of relight_chunk_rig -> (L, falloff, pos, vis), what rig_shade reads."""
     L, falloff, pos, list_o, list_d = rig_sample(setup, rays, depth, normal, acc, u, acc_mask_threshold)
-    return L, falloff, pos, rig_march(tensoIR, list_o, list_d, z_table, vis_equation)
+    return L, falloff, pos, R.march_list(tensoIR, list_o, list_d, vis_equation, z_table)
 
 
 def rig_shade(setup, rays, normal, albedo, rough, fresnel, acc, acc_mask_threshold, rescale_value, visibility,
@@ -279,14 +265,14 @@ def rig_shade(setup, rays, normal, albedo, rough, fresnel, acc, acc_mask_thresho
     L, falloff, pos, vis = visibility
     with_bg, without_bg, linear = out
     dev = rays.device
-    resc = torch.as_tensor(rescale_value, dtype=torch.float32).to(dev).reshape(-1).expand(3).contiguous()
+    resc = R.rescale3(rescale_value, dev)
     bg = torch.tensor(setup.background, dtype=torch.float32, device=dev)
     assert with_bg.is_contiguous() and without_bg.is_contiguous() and (linear is None or linear.is_contiguous())
     _lib.check(lib.tir_lights_shade(light_table(setup), len(setup.lights), _lib.dptr(rays), _lib.dptr(normal),
                                     _lib.dptr(albedo), _lib.dptr(rough), int(rough.shape[1]), _lib.dptr(fresnel),
                                     _lib.dptr(acc), int(rays.shape[0]), float(acc_mask_threshold), _lib.dptr(resc),
                                     _lib.dptr(bg), _lib.dptr(L), _lib.dptr(falloff), _lib.dptr(pos, torch.int32),
-                                    _lib.dptr(vis), 0 if vis_equation == 'nerv' else 1, _lib.dptr(with_bg),
+                                    _lib.dptr(vis), R.vis_kind(vis_equation), _lib.dptr(with_bg),
                                     _lib.dptr(without_bg), _lib.dptr(linear, allow_none=True),
                                     int(with_bg.shape[0]), int(row0), _lib.stream_ptr()), "tir_lights_shade")
 
@@ -299,8 +285,7 @@ def relight_chunk_rig(tensoIR, setup, rays, maps, rescale_value, u, acc_mask_thr
     2] fp64 uniforms.  ``shadow_far``: how far a shadow ray is marched, default the aabb diagonal, or a z table from
     shadow_table.  -> (with_bg, without_bg, linear) [n, 3]; with ``out`` = three [R, 3] device maps the rows go to
     out[k][row0:row0+n] and views of them are returned."""
-    if vis_equation not in ('nerv', 'nerfactor'):
-        raise ValueError(vis_equation)
+    R.vis_kind(vis_equation)
     n = int(rays.shape[0])
     rays, (depth, normal, albedo, rough, fresnel, acc) = R.chunk_inputs(rays, maps)
     dev = rays.device
@@ -327,16 +312,13 @@ def relight_rig(dataset, args, rig, tensoIR=None):
     from .evaluation import compute_rescale_ratio
     from .relight import write_hdr
     rig = load_rig(rig)
+    tensoIR, device = R._model(args, tensoIR)
     if tensoIR is None:
-        tensoIR = R._load_model(args, torch.device("cuda"))
-        if tensoIR is None:
-            return
-    device = tensoIR.device if hasattr(tensoIR, "device") else torch.device("cuda")
+        return
     check_outside(rig, tensoIR.aabb)
     thr = float(getattr(args, "acc_mask_threshold", R.SCRIPT_DEFAULTS["acc_mask_threshold"]))
     vis_eq = getattr(args, "vis_equation", R.SCRIPT_DEFAULTS["vis_equation"])
-    if vis_eq not in ('nerv', 'nerfactor'):
-        raise ValueError(vis_eq)
+    R.vis_kind(vis_eq)
     save_linear = bool(getattr(args, "save_linear", False))
     far = getattr(args, "shadow_far", None)
     z_table = shadow_table(default_shadow_far(tensoIR) if far is None else far, device)
@@ -350,22 +332,15 @@ def relight_rig(dataset, args, rig, tensoIR=None):
         view_dir = os.path.join(gp, f'{dataset.split}_{idx:0>3d}')
         frame_rays = dataset[idx]['rays'].squeeze(0).to(device)
         n_pix = frame_rays.shape[0]
-        light_idx = torch.zeros((n_pix, 1), dtype=torch.int32, device=device)
         with_map, without_map, linear_map = (torch.empty(len(names), n_pix, 3, device=device) for _ in range(3))
-        for s in range(0, n_pix, args.batch_size):
-            e = min(s + args.batch_size, n_pix)
-            _, depth, normal, albedo, rough, fresnel, acc, *_ = tensoIR(
-                frame_rays[s:e], light_idx[s:e], is_train=False, white_bg=True, ndc_ray=False, N_samples=-1)
+        for s, e, (_, depth, normal, albedo, rough, fresnel, acc, *_) in R._primary_chunks(tensoIR, frame_rays,
+                                                                                           args.batch_size):
             for k, name in enumerate(names):
                 u = _uniforms((e - s) * slots_per_ray(rig[name]), device, gen)
                 relight_chunk_rig(tensoIR, rig[name], frame_rays[s:e], (depth, normal, albedo, rough, fresnel, acc),
                                   rescale_value, u, thr, vis_eq, z_table,
                                   out=(with_map[k], without_map[k], linear_map[k]), row0=s)
-        for sub, m in (('with_bg', with_map), ('without_bg', without_map)):
-            os.makedirs(os.path.join(view_dir, f'relighting_{sub}'), exist_ok=True)
-            u8 = (m * 255).to(torch.uint8).reshape(len(names), H, W, 3).cpu().numpy()
-            for k, name in enumerate(names):
-                R._imwrite(os.path.join(view_dir, f'relighting_{sub}', f'{name}.png'), u8[k])
+        R._write_pairs(view_dir, names, H, W, with_map, without_map)
         if save_linear:
             os.makedirs(os.path.join(view_dir, 'relighting_linear'), exist_ok=True)
             lin = linear_map.reshape(len(names), H, W, 3).cpu().numpy()
@@ -373,7 +348,5 @@ def relight_rig(dataset, args, rig, tensoIR=None):
                 write_hdr(os.path.join(view_dir, 'relighting_linear', f'{name}.hdr'), lin[k])
     if getattr(args, "render_video", R.SCRIPT_DEFAULTS["render_video"]):
         for name in names:
-            R._mimsave(os.path.join(gp, f'{name}.mp4'),
-                       lambda name=name: [R._imread(os.path.join(gp, f'{dataset.split}_{i:0>3d}',
-                                                                 'relighting_with_bg', f'{name}.png'))
-                                          for i in range(len(dataset))])
+            R._video(os.path.join(gp, f'{name}.mp4'), gp, dataset.split, len(dataset),
+                     os.path.join('relighting_with_bg', f'{name}.png'))

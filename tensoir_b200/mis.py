@@ -22,7 +22,7 @@ from __future__ import annotations
 import torch
 
 from . import _lib
-from .relighting import chunk_inputs, env_group, env_tables, march_list
+from .relighting import append_list, chunk_inputs, env_groups, env_tables, march_list, rescale3, vis_kind
 
 
 def mis_uniforms(L, n, S_l, S_b, device):
@@ -41,17 +41,14 @@ def mis_visibility(tensoIR, envs, L, rays, depth, normal, albedo, rough, fresnel
     slots = L * n * S_l + n * S_b
     dirs = torch.empty(slots, 3, device=dev)
     pos = torch.empty(slots, dtype=torch.int32, device=dev)
-    list_o = torch.empty(slots, 3, device=dev)
-    list_d = torch.empty(slots, 3, device=dev)
-    count = torch.zeros(1, dtype=torch.int64, device=dev)
-    _lib.check(lib.tir_relight_mis_sample(envs, L, _lib.dptr(rays), _lib.dptr(depth), _lib.dptr(normal),
-                                          _lib.dptr(albedo), _lib.dptr(rough), int(rough.shape[1]), _lib.dptr(fresnel),
-                                          _lib.dptr(acc), n, S_l, S_b, float(acc_mask_threshold),
-                                          _lib.dptr(u_light, torch.float64), _lib.dptr(u_brdf, torch.float64),
-                                          _lib.dptr(dirs), _lib.dptr(pos, torch.int32), _lib.dptr(list_o),
-                                          _lib.dptr(list_d), slots, _lib.dptr(count, torch.int64), _lib.stream_ptr()),
-               "tir_relight_mis_sample")
-    return dirs, pos, march_list(tensoIR, pos, list_o, list_d, count, vis_equation, ordered=True)
+    list_o, list_d = append_list(
+        slots, dev, "relight visibility list", pos,
+        lambda *tail: _lib.check(lib.tir_relight_mis_sample(
+            envs, L, _lib.dptr(rays), _lib.dptr(depth), _lib.dptr(normal), _lib.dptr(albedo), _lib.dptr(rough),
+            int(rough.shape[1]), _lib.dptr(fresnel), _lib.dptr(acc), n, S_l, S_b, float(acc_mask_threshold),
+            _lib.dptr(u_light, torch.float64), _lib.dptr(u_brdf, torch.float64), _lib.dptr(dirs),
+            _lib.dptr(pos, torch.int32), *tail, _lib.stream_ptr()), "tir_relight_mis_sample"))
+    return dirs, pos, march_list(tensoIR, list_o, list_d, vis_equation)
 
 
 @torch.no_grad()
@@ -61,8 +58,7 @@ def relight_chunk_mis(tensoIR, envir_light, light_names, rays, maps, rescale_val
     albedo, roughness [n,1] or [n,3], fresnel, acc) of the primary render of ``rays``.  ``u_light`` [L, n, S_l, 3] and
     ``u_brdf`` [n, S_b, 3] fp64 uniforms (mis_uniforms; S_l >= 1, S_b >= 0).  ``linear_out`` [L, R, 3] receives the
     un-toned estimate at rows row0.. (0 on non-hit rows).  -> (with_bg, without_bg) [L, n, 3]."""
-    if vis_equation not in ('nerv', 'nerfactor'):
-        raise ValueError(vis_equation)
+    kind = vis_kind(vis_equation)
     dev = rays.device
     L, n = len(light_names), int(rays.shape[0])
     rays, (depth, normal, albedo, rough, fresnel, acc) = chunk_inputs(rays, maps)
@@ -79,23 +75,19 @@ def relight_chunk_mis(tensoIR, envir_light, light_names, rays, maps, rescale_val
     if n == 0 or L == 0:
         return with_bg[:, row0:row0 + n], without_bg[:, row0:row0 + n]
     envs, keep = tables if tables is not None else env_tables(envir_light, light_names)
-    resc = torch.as_tensor(rescale_value, dtype=torch.float32).to(dev).reshape(-1).expand(3).contiguous()
+    resc = rescale3(rescale_value, dev)
     thr = float(acc_mask_threshold)
-    vis_kind = 0 if vis_equation == 'nerv' else 1
     S_l, S_b = int(u_light.shape[2]), int(u_brdf.shape[1])
     lib = _lib.load()
-    G = _lib.RELIGHT_MAX_LIGHTS
-    for g in range(0, L, G):     # the kernels take up to TIR_RELIGHT_MAX_LIGHTS maps per call: groups of maps
-        Lg = min(G, L - g)
-        eg = env_group(envs, g)
+    for g, Lg, eg in env_groups(envs, L):
         dirs, pos, vis = mis_visibility(tensoIR, eg, Lg, rays, depth, normal, albedo, rough, fresnel, acc,
-                                        u_light[g:g + G], u_brdf, thr, vis_equation)
-        lin = linear_out[g:g + G] if linear_out is not None else None
+                                        u_light[g:g + Lg], u_brdf, thr, vis_equation)
+        lin = linear_out[g:g + Lg] if linear_out is not None else None
         _lib.check(lib.tir_relight_mis_shade(eg, Lg, _lib.dptr(rays), _lib.dptr(normal), _lib.dptr(albedo),
                                              _lib.dptr(rough), int(rough.shape[1]), _lib.dptr(fresnel), _lib.dptr(acc),
                                              n, S_l, S_b, thr, _lib.dptr(resc), _lib.dptr(dirs),
-                                             _lib.dptr(pos, torch.int32), _lib.dptr(vis), vis_kind,
-                                             _lib.dptr(with_bg[g:g + G]), _lib.dptr(without_bg[g:g + G]),
+                                             _lib.dptr(pos, torch.int32), _lib.dptr(vis), kind,
+                                             _lib.dptr(with_bg[g:g + Lg]), _lib.dptr(without_bg[g:g + Lg]),
                                              _lib.dptr(lin, allow_none=True), int(with_bg.shape[1]), int(row0),
                                              _lib.stream_ptr()), "tir_relight_mis_shade")
     del keep

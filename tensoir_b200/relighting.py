@@ -72,6 +72,32 @@ def env_group(envs, g):
     return C.cast(C.byref(envs, g * C.sizeof(_lib.TirEnvMap)), C.POINTER(_lib.TirEnvMap))
 
 
+def env_groups(envs, L):
+    """The kernels take up to RELIGHT_MAX_LIGHTS maps per call: -> (g, Lg, env_group(envs, g)) of each group of the
+    L maps of ``envs``, maps g..g+Lg-1."""
+    G = _lib.RELIGHT_MAX_LIGHTS
+    for g in range(0, L, G):
+        yield g, min(G, L - g), env_group(envs, g)
+
+
+def vis_kind(vis_equation):
+    """relight()'s vis_equation as the kernels take it: 0 for 'nerv' (t_last), 1 for 'nerfactor' (1 - acc).
+    ValueError for anything else."""
+    if vis_equation not in ('nerv', 'nerfactor'):
+        raise ValueError(vis_equation)
+    return 0 if vis_equation == 'nerv' else 1
+
+
+def rescale3(rescale_value, device):
+    """An albedo scale of one value or three as the kernels take it: contiguous fp32 [3] on ``device``."""
+    return torch.as_tensor(rescale_value, dtype=torch.float32).to(device).reshape(-1).expand(3).contiguous()
+
+
+def relight_table(device):
+    """relight()'s visibility march: 96 equal-z samples over [0.05, 1.5]."""
+    return ops.equal_z_table(96, 0.05, 1.5, device)
+
+
 @torch.no_grad()
 def relight_chunk_fused(tensoIR, envir_light, light_names, rays, maps, rescale_value, u, num_samples=NUM_SAMPLES,
                         acc_mask_threshold=0.5, vis_equation='nerv', out=None, row0=0, tables=None):
@@ -80,8 +106,7 @@ def relight_chunk_fused(tensoIR, envir_light, light_names, rays, maps, rescale_v
     ``u`` [L, n, num_samples] fp64 uniforms (rows of non-hit rays are ignored).  Draws nothing itself.
     -> (with_bg, without_bg) [L, n, 3]; with ``out`` = ([L, R, 3], [L, R, 3]) device maps the rows go to
     out[:, row0:row0+n] and views of them are returned."""
-    if vis_equation not in ('nerv', 'nerfactor'):
-        raise ValueError(vis_equation)
+    vis_kind(vis_equation)
     dev = rays.device
     L, n, S = len(light_names), int(rays.shape[0]), int(num_samples)
     rays, (depth, normal, albedo, rough, fresnel, acc) = chunk_inputs(rays, maps)
@@ -95,19 +120,11 @@ def relight_chunk_fused(tensoIR, envir_light, light_names, rays, maps, rescale_v
     if n == 0 or L == 0:
         return with_bg[:, row0:row0 + n], without_bg[:, row0:row0 + n]
     envs, keep = tables if tables is not None else env_tables(envir_light, light_names)
-    G = _lib.RELIGHT_MAX_LIGHTS
-    if L > G:                  # the kernels take up to TIR_RELIGHT_MAX_LIGHTS maps per call: groups of maps
-        for g in range(0, L, G):
-            sub = (env_group(envs, g), keep)
-            relight_chunk_fused(tensoIR, envir_light, light_names[g:g + G], rays, maps, rescale_value, u[g:g + G],
-                                num_samples, acc_mask_threshold, vis_equation, out=(with_bg[g:g + G],
-                                                                                    without_bg[g:g + G]),
-                                row0=row0, tables=sub)
-        return with_bg[:, row0:row0 + n], without_bg[:, row0:row0 + n]
-    bins, pos, vis = relight_visibility(tensoIR, envs, L, rays, depth, normal, acc, u, S, acc_mask_threshold,
-                                        vis_equation)
-    relight_shade(envs, L, rays, normal, albedo, rough, fresnel, acc, S, acc_mask_threshold, rescale_value,
-                  (bins, pos, vis), vis_equation, out, row0)
+    for g, Lg, eg in env_groups(envs, L):
+        vis = relight_visibility(tensoIR, eg, Lg, rays, depth, normal, acc, u[g:g + Lg], S, acc_mask_threshold,
+                                 vis_equation)
+        relight_shade(eg, Lg, rays, normal, albedo, rough, fresnel, acc, S, acc_mask_threshold, rescale_value, vis,
+                      vis_equation, (with_bg[g:g + Lg], without_bg[g:g + Lg]), row0)
     del keep
     return with_bg[:, row0:row0 + n], without_bg[:, row0:row0 + n]
 
@@ -131,36 +148,48 @@ def relight_visibility(tensoIR, envs, L, rays, depth, normal, acc, u, num_sample
     lib = _lib.load()
     dev = rays.device
     n, S = int(rays.shape[0]), int(num_samples)
-    cap = L * n * S
     bins = torch.empty(L, n, S, dtype=torch.int32, device=dev)
     pos = torch.empty(L, n, S, dtype=torch.int32, device=dev)
-    list_o = torch.empty(cap, 3, device=dev)
-    list_d = torch.empty(cap, 3, device=dev)
-    count = torch.zeros(1, dtype=torch.int64, device=dev)
-    thr = float(acc_mask_threshold)
-    _lib.check(lib.tir_relight_sample(envs, L, _lib.dptr(rays), _lib.dptr(depth), _lib.dptr(normal), _lib.dptr(acc),
-                                      n, S, thr, _lib.dptr(u, dtype=torch.float64), _lib.dptr(bins, torch.int32),
-                                      _lib.dptr(pos, torch.int32), _lib.dptr(list_o), _lib.dptr(list_d), cap,
-                                      _lib.dptr(count, torch.int64), _lib.stream_ptr()), "tir_relight_sample")
-    return bins, pos, march_list(tensoIR, pos, list_o, list_d, count, vis_equation, ordered)
+    list_o, list_d = append_list(
+        L * n * S, dev, "relight visibility list", pos if ordered else None,
+        lambda *tail: _lib.check(lib.tir_relight_sample(
+            envs, L, _lib.dptr(rays), _lib.dptr(depth), _lib.dptr(normal), _lib.dptr(acc), n, S,
+            float(acc_mask_threshold), _lib.dptr(u, dtype=torch.float64), _lib.dptr(bins, torch.int32),
+            _lib.dptr(pos, torch.int32), *tail, _lib.stream_ptr()), "tir_relight_sample"))
+    return bins, pos, march_list(tensoIR, list_o, list_d, vis_equation)
 
 
-def march_list(tensoIR, pos, list_o, list_d, count, vis_equation, ordered=False):
-    """The density march of an appended visibility list: reads back its length (``count``, the one host sync of the
-    chunk) and marches its rows with relight()'s 96-sample table over [0.05, 1.5].  ``ordered``: put the list in slot
-    order first (slot_order, rewriting pos).  -> vis per list row (t_last for nerv, acc for nerfactor)."""
-    cap = int(list_o.shape[0])
+def append_list(cap, device, what, pos, sample):
+    """The visibility list of a tir_*_sample entry: allocates ``cap`` (origin, direction) rows, runs ``sample(list_o,
+    list_d, capacity, count)`` with the entry's four trailing list arguments, and reads the list length back (the
+    one host sync of the chunk; TirError naming ``what`` if it overflowed).  ``pos``: the entry's slot map, to put the
+    list in slot order (slot_order, rewriting pos), or None to keep the append order.
+    -> (list_o, list_d) cut to the list length."""
+    list_o = torch.empty(cap, 3, device=device)
+    list_d = torch.empty(cap, 3, device=device)
+    count = torch.zeros(1, dtype=torch.int64, device=device)
+    sample(_lib.dptr(list_o), _lib.dptr(list_d), cap, _lib.dptr(count, torch.int64))
     m = int(count.item())
     if m > cap:
-        raise _lib.TirError(f"relight visibility list overflow: {m} > {cap}")
-    if m == 0:
-        return torch.zeros(1, device=list_o.device)
-    if ordered:
-        list_o, list_d = slot_order(pos, list_o[:m], list_d[:m])
-    table = ops.equal_z_table(96, 0.05, 1.5, list_o.device)
-    t_last, acc_s, _ = ops.march_density(tensoIR, list_o[:m], list_d[:m], table=table,
-                                         counters=tensoIR.__dict__.get("_tir_counters"))
-    return (t_last if vis_equation == 'nerv' else acc_s).contiguous()
+        raise _lib.TirError(f"{what} overflow: {m} > {cap}")
+    if pos is not None and m > 0:
+        return slot_order(pos, list_o[:m], list_d[:m])
+    return list_o[:m], list_d[:m]
+
+
+def march_list(tensoIR, list_o, list_d, vis_equation=None, table=None):
+    """The density march of append_list's rows with ``table`` (default relight_table).  -> the visibility per row the
+    shade kernels read, by ``vis_equation`` (t_last for nerv, acc for nerfactor), or with vis_equation None all three
+    outputs (t_last, acc, depth); a list without rows gives a zero [1] for each."""
+    if list_o.shape[0] == 0:
+        out = (torch.zeros(1, device=list_o.device),) * 3
+    else:
+        out = ops.march_density(tensoIR, list_o, list_d,
+                                table=relight_table(list_o.device) if table is None else table,
+                                counters=tensoIR.__dict__.get("_tir_counters"))
+    if vis_equation is not None:
+        return out[vis_kind(vis_equation)].contiguous()
+    return tuple(t.contiguous() for t in out)
 
 
 def relight_shade(envs, L, rays, normal, albedo, rough, fresnel, acc, num_samples, acc_mask_threshold, rescale_value,
@@ -172,13 +201,13 @@ def relight_shade(envs, L, rays, normal, albedo, rough, fresnel, acc, num_sample
     bins, pos, vis = visibility
     with_bg, without_bg = out
     n, dev = int(rays.shape[0]), rays.device
-    resc = torch.as_tensor(rescale_value, dtype=torch.float32).to(dev).reshape(-1).expand(3).contiguous()
+    resc = rescale3(rescale_value, dev)
     assert with_bg.is_contiguous() and without_bg.is_contiguous()
     _lib.check(lib.tir_relight_shade(envs, L, _lib.dptr(rays), _lib.dptr(normal), _lib.dptr(albedo), _lib.dptr(rough),
                                      int(rough.shape[1]), _lib.dptr(fresnel), _lib.dptr(acc), n, int(num_samples),
                                      float(acc_mask_threshold), _lib.dptr(resc), _lib.dptr(bins, torch.int32),
-                                     _lib.dptr(pos, torch.int32), _lib.dptr(vis),
-                                     0 if vis_equation == 'nerv' else 1, _lib.dptr(with_bg), _lib.dptr(without_bg),
+                                     _lib.dptr(pos, torch.int32), _lib.dptr(vis), vis_kind(vis_equation),
+                                     _lib.dptr(with_bg), _lib.dptr(without_bg),
                                      int(with_bg.shape[1]), int(row0), _lib.stream_ptr()), "tir_relight_shade")
 
 
@@ -241,6 +270,75 @@ def _load_model(args, device):
     return model
 
 
+def _model(args, tensoIR):
+    """``tensoIR``, or the checkpoint args.ckpt loaded on cuda -> (model, its device); (None, None) without one."""
+    if tensoIR is None:
+        tensoIR = _load_model(args, torch.device("cuda"))
+        if tensoIR is None:
+            return None, None
+    return tensoIR, tensoIR.device if hasattr(tensoIR, "device") else torch.device("cuda")
+
+
+def _primary_chunks(tensoIR, frame_rays, batch_size):
+    """The primary render of one view's rays in chunks of ``batch_size`` -> (s, e, outputs of the eval forward)."""
+    n_pix = frame_rays.shape[0]
+    light_idx = torch.zeros((n_pix, 1), dtype=torch.int32, device=frame_rays.device)
+    for s in range(0, n_pix, batch_size):
+        e = min(s + batch_size, n_pix)
+        yield s, e, tensoIR(frame_rays[s:e], light_idx[s:e], is_train=False, white_bg=True, ndc_ray=False,
+                            N_samples=-1)
+
+
+def _write_pairs(view_dir, names, H, W, with_map, without_map):
+    """{view_dir}/relighting_with_bg/{name}.png and relighting_without_bg/{name}.png of [L, H*W, 3] maps."""
+    for sub, m in (('with_bg', with_map), ('without_bg', without_map)):
+        os.makedirs(os.path.join(view_dir, f'relighting_{sub}'), exist_ok=True)
+        u8 = (m * 255).to(torch.uint8).reshape(len(names), H, W, 3).cpu().numpy()
+        for k, name in enumerate(names):
+            _imwrite(os.path.join(view_dir, f'relighting_{sub}', f'{name}.png'), u8[k])
+
+
+def _acc_u8(acc, H, W):
+    """The alpha of the view's images: the reference's `acc_temp = acc_chunk[..., None]; acc_temp[acc_temp <= 0.9] = 0`
+    (relight_importance.py:179-180) zeroes the primary acc in place -> uint8 [H, W, 1]."""
+    acc_t = acc.reshape(-1).clone()
+    acc_t[acc_t <= 0.9] = 0.0
+    return (acc_t.reshape(H, W, 1) * 255).to(torch.uint8).cpu().numpy()
+
+
+def _new_metrics(names):
+    return {k: {n: [] for n in names} for k in ("psnr", "ssim", "alex", "vgg")}
+
+
+def _view_metrics(m, names, without_map, gt_rgb, H, W, device, path):
+    """PSNR, SSIM and LPIPS of each map of one view against its ground truth (:212-226), appended to ``m``
+    (_new_metrics), and the view's relight_psnr.txt at ``path``."""
+    met = pair_metrics(without_map, gt_rgb, H, W).cpu().numpy()
+    for k, name in enumerate(names):
+        m["psnr"][name].append(-10.0 * np.log(met[k, 0] / (H * W * 3)) / np.log(10.0))
+        m["ssim"][name].append(float(met[k, 1]))
+        img, gt_img = without_map[k].reshape(H, W, 3), gt_rgb[k].reshape(H, W, 3)
+        m["alex"][name].append(_lpips(gt_img, img, 'alex', device))
+        m["vgg"][name].append(_lpips(gt_img, img, 'vgg', device))
+    with open(path, 'w') as f:
+        for name in names:
+            f.write(f'{name}: PNSR {m["psnr"][name][-1]}; SSIM {m["ssim"][name][-1]}; L_Alex {m["alex"][name][-1]}; '
+                    f'L_VGG {m["vgg"][name][-1]}\n')
+
+
+def _run_metrics(m, names, path):
+    """The run's relight_psnr.txt: the mean of each metric of ``m`` over the views."""
+    with open(path, 'w') as f:
+        for name in names:
+            f.write(f'{name}:  PSNR {np.mean(m["psnr"][name])}; SSIM {np.mean(m["ssim"][name])}; '
+                    f'L_Alex {np.mean(m["alex"][name])}; L_VGG {np.mean(m["vgg"][name])}\n')
+
+
+def _video(path, gp, split, n_views, rel):
+    """The video of one image over the views: {gp}/{split}_{i:03d}/{rel} for i < n_views."""
+    _mimsave(path, lambda: [_imread(os.path.join(gp, f'{split}_{i:0>3d}', rel)) for i in range(n_views)])
+
+
 def mis_options(args):
     """relight()'s estimator options from ``args``: -> (sampling, brdf_samples).  ValueError for an unknown sampling,
     brdf_samples outside [0, NUM_SAMPLES - 1], or sampling 'mis' with indirect light."""
@@ -274,12 +372,9 @@ def relight(dataset, args, tensoIR=None, *, rescale_value=None):
     from .relight import Environment_Light
     sampling, n_brdf = mis_options(args)
     opt = {k: getattr(args, k, v) for k, v in SCRIPT_DEFAULTS.items()}
-    device = torch.device("cuda")
+    tensoIR, device = _model(args, tensoIR)
     if tensoIR is None:
-        tensoIR = _load_model(args, device)
-        if tensoIR is None:
-            return
-    device = tensoIR.device if hasattr(tensoIR, "device") else device
+        return
     W, H = dataset.img_wh
     if H < 11 or W < 11:
         raise ValueError(f"SSIM needs images of at least 11x11 pixels, got {W}x{H}")
@@ -307,7 +402,7 @@ def relight(dataset, args, tensoIR=None, *, rescale_value=None):
         ind_kw = dict(indirect_samples=n_ind, indirect_light_samples=int(getattr(args, "indirect_light_samples", 32)
                                                                            or 32))
 
-    psnr, ssim, l_alex, l_vgg = ({n: [] for n in names} for _ in range(4))
+    metrics = _new_metrics(names)
     rgb_frames, aligned_albedo_list, roughness_list = [], [], []
     gp = args.geo_buffer_path
     for idx in range(len(dataset)):
@@ -319,17 +414,14 @@ def relight(dataset, args, tensoIR=None, *, rescale_value=None):
         gt_mask = item['rgbs_mask'].squeeze(0).squeeze(-1).cpu()
         gt_rgb = item['rgbs'].squeeze(0).reshape(L, H * W, 3).to(device)
         gt_albedo = item['albedo'].squeeze(0).to(device)
-        light_idx = torch.zeros((n_pix, 1), dtype=torch.int32, device=device)
 
         with_map = torch.empty(L, n_pix, 3, device=device)
         without_map = torch.empty(L, n_pix, 3, device=device)
         ind_map = torch.empty(L, n_pix, 3, device=device) if save_ind else None
         prim = {}
-        for s in range(0, n_pix, args.batch_size):
-            e = min(s + args.batch_size, n_pix)
+        for s, e, (rgb, depth, normal, albedo, rough, fresnel, acc, *_) in _primary_chunks(tensoIR, frame_rays,
+                                                                                            args.batch_size):
             rays = frame_rays[s:e]
-            rgb, depth, normal, albedo, rough, fresnel, acc, *_ = tensoIR(
-                rays, light_idx[s:e], is_train=False, white_bg=True, ndc_ray=False, N_samples=-1)
             for k, t in (("rgb", rgb), ("depth", depth), ("normal", normal), ("albedo", albedo), ("rough", rough),
                          ("acc", acc)):
                 t = t.detach()
@@ -353,41 +445,24 @@ def relight(dataset, args, tensoIR=None, *, rescale_value=None):
                                     rescale_value, u, NUM_SAMPLES, thr, opt["vis_equation"],
                                     out=(with_map, without_map), row0=s, tables=tables)
 
-        # metrics of every map against its ground truth (:212-226): the image without background
-        met = pair_metrics(without_map, gt_rgb, H, W).cpu().numpy()
-        for k, name in enumerate(names):
-            loss = met[k, 0] / (H * W * 3)
-            psnr[name].append(-10.0 * np.log(loss) / np.log(10.0))
-            ssim[name].append(float(met[k, 1]))
-            img, gt_img = without_map[k].reshape(H, W, 3), gt_rgb[k].reshape(H, W, 3)
-            l_alex[name].append(_lpips(gt_img, img, 'alex', device))
-            l_vgg[name].append(_lpips(gt_img, img, 'vgg', device))
-        os.makedirs(os.path.join(cur_dir_path, 'relighting_with_bg'), exist_ok=True)
-        os.makedirs(os.path.join(cur_dir_path, 'relighting_without_bg'), exist_ok=True)
+        # metrics of every map against its ground truth: the image without background
+        for sub in ('with_bg', 'without_bg'):
+            os.makedirs(os.path.join(cur_dir_path, f'relighting_{sub}'), exist_ok=True)
+        _view_metrics(metrics, names, without_map, gt_rgb, H, W, device,
+                      os.path.join(cur_dir_path, 'relighting_without_bg', 'relight_psnr.txt'))
         if opt["if_save_relight_rgb"]:
-            u8w = (with_map * 255).to(torch.uint8).reshape(L, H, W, 3).cpu().numpy()
-            u8o = (without_map * 255).to(torch.uint8).reshape(L, H, W, 3).cpu().numpy()
-            for k, name in enumerate(names):
-                _imwrite(os.path.join(cur_dir_path, 'relighting_with_bg', f'{name}.png'), u8w[k])
-                _imwrite(os.path.join(cur_dir_path, 'relighting_without_bg', f'{name}.png'), u8o[k])
+            _write_pairs(cur_dir_path, names, H, W, with_map, without_map)
         if save_ind:
             from .relight import write_hdr
             os.makedirs(os.path.join(cur_dir_path, 'relighting_indirect'), exist_ok=True)
             ind_np = ind_map.reshape(L, H, W, 3).cpu().numpy()
             for k, name in enumerate(names):
                 write_hdr(os.path.join(cur_dir_path, 'relighting_indirect', f'{name}.hdr'), ind_np[k])
-        with open(os.path.join(cur_dir_path, 'relighting_without_bg', 'relight_psnr.txt'), 'w') as f:
-            for name in names:
-                f.write(f'{name}: PNSR {psnr[name][-1]}; SSIM {ssim[name][-1]}; L_Alex {l_alex[name][-1]}; '
-                        f'L_VGG {l_vgg[name][-1]}\n')
 
-        # the reference's `acc_temp = acc_chunk[..., None]; acc_temp[acc_temp <= 0.9] = 0` (:179-180) zeroes the
-        # primary acc in place: every image below uses the thresholded acc
-        acc_t = prim["acc"].reshape(-1).clone()
-        acc_t[acc_t <= 0.9] = 0.0
+        # every image below uses the thresholded acc
         rgb_u8 = (prim["rgb"].reshape(H, W, 3) * 255).to(torch.uint8).cpu().numpy()
         rgb_frames.append(rgb_u8)
-        acc_u8 = (acc_t.reshape(H, W, 1) * 255).to(torch.uint8).cpu().numpy()
+        acc_u8 = _acc_u8(prim["acc"], H, W)
         if opt["if_save_rgb"]:
             _imwrite(os.path.join(cur_dir_path, 'rgb.png'), rgb_u8)
         if opt["if_save_depth"]:
@@ -421,10 +496,7 @@ def relight(dataset, args, tensoIR=None, *, rescale_value=None):
             nrm_u8 = (nrm.reshape(H, W, 3) * 255).to(torch.uint8).cpu().numpy()
             _imwrite(os.path.join(cur_dir_path, 'normal.png'), np.concatenate([nrm_u8, acc_u8], axis=2))
 
-    with open(os.path.join(gp, 'relight_psnr.txt'), 'w') as f:
-        for name in names:
-            f.write(f'{name}:  PSNR {np.mean(psnr[name])}; SSIM {np.mean(ssim[name])}; '
-                    f'L_Alex {np.mean(l_alex[name])}; L_VGG {np.mean(l_vgg[name])}\n')
+    _run_metrics(metrics, names, os.path.join(gp, 'relight_psnr.txt'))
 
     if opt["if_save_rgb_video"]:
         os.makedirs(os.path.join(gp, 'video'), exist_ok=True)
@@ -451,7 +523,6 @@ def relight(dataset, args, tensoIR=None, *, rescale_value=None):
             vp = os.path.join(gp, f'video_{sub}')
             os.makedirs(vp, exist_ok=True)
             for name in names:
-                _mimsave(os.path.join(vp, f'{name}_video.mp4'),
-                         lambda: [_imread(os.path.join(gp, f'{dataset.split}_{i:0>3d}', f'relighting_{sub}',
-                                                       f'{name}.png')) for i in range(len(dataset))])
+                _video(os.path.join(vp, f'{name}_video.mp4'), gp, dataset.split, len(dataset),
+                       os.path.join(f'relighting_{sub}', f'{name}.png'))
 

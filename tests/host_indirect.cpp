@@ -35,8 +35,8 @@ extern "C" int tir_indirect_sample(const float* rays, const float* depth, const 
       !count)
     return TIR_ERR_NULL;
   if (rough_stride != 1 && rough_stride != 3) return TIR_ERR_SHAPE;
-  if (capacity < 0 || capacity > INT32_MAX) return TIR_ERR_SHAPE;
-  if (capacity > 0 && (!list_o || !list_d)) return TIR_ERR_NULL;
+  const int lrc = rl_check_list(capacity, list_o, list_d);
+  if (lrc) return lrc;
   for (int64_t i = 0; i < n; ++i)
     for (int k = 0; k < K; ++k) {
       const int64_t t = i * K + k;

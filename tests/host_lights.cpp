@@ -12,8 +12,8 @@ extern "C" int tir_lights_sample(const TirLight* lights, int32_t n_lights, const
   const int rc = lt_validate(lights, n_lights, n, lt);
   if (rc <= 0) return rc;
   if (!rays || !depth || !normal || !acc || !u || !L || !falloff || !pos || !count) return TIR_ERR_NULL;
-  if (capacity < 0 || capacity > INT32_MAX) return TIR_ERR_SHAPE;
-  if (capacity > 0 && (!list_o || !list_d)) return TIR_ERR_NULL;
+  const int lrc = rl_check_list(capacity, list_o, list_d);
+  if (lrc) return lrc;
   for (int j = 0; j < n_lights; ++j)
     for (int64_t i = 0; i < n; ++i)
       for (int s = 0; s < lt.l[j].n_samples; ++s) {
@@ -64,7 +64,7 @@ extern "C" int tir_lights_shade(const TirLight* lights, int32_t n_lights, const 
         for (int s = 0; s < K; ++s) {
           const int q = pos[k0 + s];
           if (q < 0) continue;
-          const float vis = vis_kind ? 1.f - vis_list[q] : vis_list[q];
+          const float vis = rl_vis(vis_list, vis_kind, q);
           lt_contrib(c, L + (k0 + s) * 3, falloff[k0 + s], vis, lane[s % 32]);
         }
         for (int o = 16; o > 0; o >>= 1) {

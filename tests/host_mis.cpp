@@ -14,12 +14,13 @@ extern "C" int tir_relight_mis_sample(const TirEnvMap* envs, int32_t n_lights, c
                                       int64_t capacity, int64_t* count, void*) {
   const int rc = mis_validate(envs, n_lights, n, S_l, S_b, rough_stride);
   if (rc < 0) return rc;
-  if (capacity < 0 || capacity > INT32_MAX) return TIR_ERR_SHAPE;
+  const int lrc = rl_check_list(capacity, list_o, list_d);
+  if (lrc == TIR_ERR_SHAPE) return lrc;
   if (rc == 0) return TIR_OK;
   if (!rays || !depth || !normal || !albedo || !rough || !fresnel || !acc || !u_light || !dir || !pos || !count)
     return TIR_ERR_NULL;
   if (S_b > 0 && !u_brdf) return TIR_ERR_NULL;
-  if (capacity > 0 && (!list_o || !list_d)) return TIR_ERR_NULL;
+  if (lrc) return lrc;
   const int64_t n_light = (int64_t)n_lights * n * S_l, total = n_light + n * S_b;
   for (int64_t t = 0; t < total; ++t) {
     const bool light = t < n_light;

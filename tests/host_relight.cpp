@@ -13,8 +13,8 @@ extern "C" int tir_relight_sample(const TirEnvMap* envs, int32_t n_lights, const
   const int rc = rl_validate(envs, n_lights, n, n_samples);
   if (rc <= 0 || n_samples == 0) return rc < 0 ? rc : TIR_OK;
   if (!rays || !depth || !normal || !acc || !u || !bin || !pos || !count) return TIR_ERR_NULL;
-  if (capacity < 0) return TIR_ERR_SHAPE;
-  if (capacity > 0 && (!list_o || !list_d)) return TIR_ERR_NULL;
+  const int lrc = rl_check_list(capacity, list_o, list_d);
+  if (lrc) return lrc;
   for (int l = 0; l < n_lights; ++l)
     for (int64_t i = 0; i < n; ++i)
       for (int s = 0; s < n_samples; ++s) {
@@ -66,7 +66,7 @@ extern "C" int tir_relight_shade(const TirEnvMap* envs, int32_t n_lights, const 
         for (int s = 0; s < n_samples; ++s) {
           const int64_t t = ((int64_t)l * n + i) * n_samples + s;
           const int b = bin[t], q = pos[t];
-          const float vis = q >= 0 ? (vis_kind ? 1.f - vis_list[q] : vis_list[q]) : 0.f;
+          const float vis = q >= 0 ? rl_vis(vis_list, vis_kind, q) : 0.f;
           rl_contrib(c, e.dir + (int64_t)b * 3, e.rgb + (int64_t)b * 3, e.pdf_return[b], vis, lane[s % 32]);
         }
         for (int o = 16; o > 0; o >>= 1) {

@@ -11,8 +11,8 @@ extern "C" int tir_transport_sample(const float* dirs, int32_t K, const float* r
   const int rc = tt_validate(K, n);
   if (rc <= 0) return rc;
   if (!dirs || !rays || !depth || !normal || !acc || !pos || !count) return TIR_ERR_NULL;
-  if (capacity < 0 || capacity > INT32_MAX) return TIR_ERR_SHAPE;
-  if (capacity > 0 && (!list_o || !list_d)) return TIR_ERR_NULL;
+  const int lrc = rl_check_list(capacity, list_o, list_d);
+  if (lrc) return lrc;
   for (int64_t i = 0; i < n; ++i)
     for (int k = 0; k < K; ++k) {
       const int64_t t = i * K + k;
@@ -52,7 +52,7 @@ extern "C" int tir_transport_build(const float* dirs, const float* domega, int32
       const int64_t t = i * K + k;
       float v[3] = {0.f, 0.f, 0.f};
       if (hit && pos[t] >= 0) {
-        const float vis = vis_kind ? 1.f - vis_list[pos[t]] : vis_list[pos[t]];
+        const float vis = rl_vis(vis_list, vis_kind, pos[t]);
         tt_contrib(c, dirs + (int64_t)k * 3, domega[k], vis, v);
       }
       for (int ch = 0; ch < 3; ++ch) T[ch * plane + t] = v[ch];

@@ -182,6 +182,16 @@ def march64(model, o, d):
     return T[:, -1], w.sum(1), (w * z).sum(1)
 
 
+def test_chunk_without_secondary_rays(lego):
+    """A chunk where no ray counts as a surface hit: the secondary list is empty, and no slot becomes a hit."""
+    rays, maps = lego_chunk(lego)
+    rays_c, (depth, normal, albedo, rough, fresnel, acc) = relighting.chunk_inputs(rays, maps)
+    u = torch.rand(rays.shape[0], 4, 2, generator=torch.Generator(DEV).manual_seed(5), device=DEV, dtype=torch.float64)
+    hits = indirect.secondary_hits(lego, rays_c, depth, normal, albedo, rough, fresnel, acc, torch.ones(3, device=DEV),
+                                   u, 2.0, 'nerv')
+    assert hits["list_o"].shape[0] == 0 and hits["rays"].shape[0] == 0 and bool((hits["hit"] == -1).all())
+
+
 def test_lego_stages(lego, env):
     names, light, hdr = env
     rays, maps = lego_chunk(lego)

@@ -81,7 +81,6 @@ def test_transport_is_the_expectation_of_relight(fx):
     relight_chunk_fused's estimator over Environment_Light's sampling distribution with the same visibility; and
     relight_chunk_fused with 8192 samples lands within 6 estimated standard errors of it on every hit row."""
     from tensoir_b200 import light_fit as LF, relighting as R
-    from tensoir_b200.lighting import rig_march
     from tensoir_b200.relight import Environment_Light
     m = model_from_fixture(fx, DEV)
     rays, maps = R.chunk_inputs(fx["rays"].to(DEV), tuple(t.to(DEV) for t in fx["relight_maps"]))
@@ -92,7 +91,7 @@ def test_transport_is_the_expectation_of_relight(fx):
     rescale = 1.1
     grid = LF.texel_tables(H_E, W_E, DEV)
     pos, lo, ld = LF.transport_sample(grid, rays, depth, normal, acc, 0.5)
-    vis = rig_march(m, lo, ld, LF.shadow_table(DEV), 'nerv')
+    vis = R.march_list(m, lo, ld, 'nerv')
     T = LF.transport_build(grid, rays, normal, albedo, rough, fresnel, acc, 0.5, rescale, pos, vis, 'nerv')
     hit = (acc > 0.5).cpu()
     assert hit.sum() > 10

@@ -35,7 +35,6 @@ def main():
     g.build()
     import tensoir_b200.relighting as R
     from eval_views import gpu_info
-    from tensoir_b200.lighting import rig_march
     from tensoir_b200.synthetic import SyntheticViews, hemisphere_poses, make_lego_model
     dev = "cuda:0"
     model = make_lego_model(a.grid, dev)
@@ -43,7 +42,7 @@ def main():
     items = [ds[i] for i in range(len(ds))]
     grid = LF.texel_tables(H_e, W_e, dev)
     K = H_e * W_e
-    table = LF.shadow_table(dev)
+    table = R.relight_table(dev)
     gpu, power = gpu_info()
 
     def tick():
@@ -72,7 +71,7 @@ def main():
                 t1 = tick()
                 pos, list_o, list_d = LF.transport_sample(grid, rays, depth, normal, acc, 0.5)
                 t2 = tick()
-                vis = rig_march(model, list_o, list_d, table, 'nerv')
+                vis = R.march_list(model, list_o, list_d, 'nerv', table)
                 t3 = tick()
                 T = LF.transport_build(grid, rays, normal, albedo, rough, fresnel, acc, 0.5, 1.0, pos, vis, 'nerv')
                 t4 = tick()

@@ -77,7 +77,7 @@ def main():
                     u = LT._uniforms((e - s) * LT.slots_per_ray(setup), dev)
                     L, falloff, pos, list_o, list_d = LT.rig_sample(setup, rays, depth, normal, acc, u, 0.5)
                     t1 = tick()
-                    vis = LT.rig_march(model, list_o, list_d, z_table, 'nerv')
+                    vis = R.march_list(model, list_o, list_d, 'nerv', z_table)
                     t2 = tick()
                     LT.rig_shade(setup, rays, normal, albedo, rough, fresnel, acc, 0.5, scale, (L, falloff, pos, vis),
                                  'nerv', tuple(o[k] for o in out), s)
