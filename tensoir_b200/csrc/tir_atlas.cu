@@ -83,10 +83,8 @@ __global__ void __launch_bounds__(kThreads) atlas_corners_kernel(const int32_t* 
 
 extern "C" int tir_atlas_texels(const int32_t* faces, int64_t n_faces, const float* v, int32_t T, int32_t s,
                                 int64_t first, int64_t n, int32_t* pix, float* pos, void* stream) {
-  int rc = at_validate_layout(n_faces, T, s);
-  if (!rc) rc = at_validate_range(n_faces, s, first, n);
-  if (rc || n == 0) return rc;
-  if (!faces || !v || !pix || !pos) return TIR_ERR_NULL;
+  const int rc = at_texels_check(faces, n_faces, v, T, s, first, n, pix, pos);
+  if (rc <= 0) return rc;
   atlas_texels_kernel<<<grid_for(n), kThreads, 0, (cudaStream_t)stream>>>(faces, v, T, s, first, n, pix, pos);
   return (int)cudaGetLastError();
 }
@@ -95,11 +93,9 @@ extern "C" int tir_atlas_encode(const int32_t* faces, int64_t n_faces, const flo
                                 int64_t first, int64_t n, const float* albedo, const float* rough,
                                 const float* normal, const uint8_t* probed, uint8_t* base_color,
                                 uint8_t* metallic_roughness, uint8_t* normal_map, void* stream) {
-  int rc = at_validate_layout(n_faces, T, s);
-  if (!rc) rc = at_validate_range(n_faces, s, first, n);
-  if (rc || n == 0) return rc;
-  if (!faces || !v || !albedo || !rough || !normal || !probed || !base_color || !metallic_roughness || !normal_map)
-    return TIR_ERR_NULL;
+  const int rc = at_encode_check(faces, n_faces, v, T, s, first, n, albedo, rough, normal, probed, base_color,
+                                 metallic_roughness, normal_map);
+  if (rc <= 0) return rc;
   atlas_encode_kernel<<<grid_for(n), kThreads, 0, (cudaStream_t)stream>>>(
       faces, v, T, s, first, n, albedo, rough, normal, probed, (uint32_t*)base_color, (uint32_t*)metallic_roughness,
       (uint32_t*)normal_map);
@@ -108,9 +104,8 @@ extern "C" int tir_atlas_encode(const int32_t* faces, int64_t n_faces, const flo
 
 extern "C" int tir_atlas_corners(const int32_t* faces, int64_t n_faces, const float* v, int32_t T, int32_t s,
                                  float* position, float* normal, float* tangent, float* texcoord, void* stream) {
-  const int rc = at_validate_layout(n_faces, T, s);
-  if (rc || n_faces == 0) return rc;
-  if (!faces || !v || !position || !normal || !tangent || !texcoord) return TIR_ERR_NULL;
+  const int rc = at_corners_check(faces, n_faces, v, T, s, position, normal, tangent, texcoord);
+  if (rc <= 0) return rc;
   atlas_corners_kernel<<<grid_for(n_faces), kThreads, 0, (cudaStream_t)stream>>>(faces, v, n_faces, T, s, position,
                                                                                   normal, tangent, texcoord);
   return (int)cudaGetLastError();

@@ -84,6 +84,37 @@ inline int at_validate_range(int64_t F, int32_t s, int64_t first, int64_t n) {
   return first + n <= F * at_face_texels(s) ? TIR_OK : TIR_ERR_SHAPE;
 }
 
+// The whole argument check of each entry, run by tir_atlas.cu and its host build before their launch / loop:
+// 1 run, 0 nothing to do, < 0 TirStatus
+inline int at_texels_check(const int32_t* faces, int64_t F, const float* v, int32_t T, int32_t s, int64_t first,
+                           int64_t n, const int32_t* pix, const float* pos) {
+  int rc = at_validate_layout(F, T, s);
+  if (!rc) rc = at_validate_range(F, s, first, n);
+  if (rc || n == 0) return rc;
+  if (!faces || !v || !pix || !pos) return TIR_ERR_NULL;
+  return 1;
+}
+
+inline int at_encode_check(const int32_t* faces, int64_t F, const float* v, int32_t T, int32_t s, int64_t first,
+                           int64_t n, const float* albedo, const float* rough, const float* normal,
+                           const uint8_t* probed, const uint8_t* base_color, const uint8_t* metallic_roughness,
+                           const uint8_t* normal_map) {
+  int rc = at_validate_layout(F, T, s);
+  if (!rc) rc = at_validate_range(F, s, first, n);
+  if (rc || n == 0) return rc;
+  if (!faces || !v || !albedo || !rough || !normal || !probed || !base_color || !metallic_roughness || !normal_map)
+    return TIR_ERR_NULL;
+  return 1;
+}
+
+inline int at_corners_check(const int32_t* faces, int64_t F, const float* v, int32_t T, int32_t s,
+                            const float* position, const float* normal, const float* tangent, const float* texcoord) {
+  const int rc = at_validate_layout(F, T, s);
+  if (rc || F == 0) return rc;
+  if (!faces || !v || !position || !normal || !tangent || !texcoord) return TIR_ERR_NULL;
+  return 1;
+}
+
 // Texel t of the face-major enumeration: face t / q, then its owned texels by anti-diagonal d = i + j of A's frame
 // and by i along it.  -> face, A-frame (ia, ja), image texel (x, y).
 struct AtTexel {

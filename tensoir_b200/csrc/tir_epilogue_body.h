@@ -4,6 +4,8 @@
 // the compositing kernel.  Shared by the CUDA kernels and a host build checked against torch autograd on the CPU.
 #pragma once
 #include <math.h>
+#include <stdint.h>
+#include "../../include/tensoir_b200.h"
 
 #if defined(__CUDACC__)
 #define EPI_HD __host__ __device__ __forceinline__
@@ -85,4 +87,22 @@ EPI_HD void epi_backward(const EpiIn& in, const EpiOut& g, float gP[14], float* 
   g_om += gP[9];
   gP[10] = g.ac; gP[11] = g.rc; gP[12] = g.nd; gP[13] = g.no;
   *g_acc = in.bg ? -g_om : 0.f;
+}
+
+// The whole argument check of each entry, run by tir_tail.cu and its host build before their launch / loop:
+// 1 run, 0 nothing to do, < 0 TirStatus.  The maps of g_out and the loss gradients are optional.
+inline int epi_fwd_check(int64_t n, const float* packed, const float* acc, const float* depth, const float* rays,
+                         const TirRayMaps* out, const uint8_t* acc_mask, const float* losses) {
+  if (n <= 0) return 0;
+  if (!packed || !acc || !depth || !rays || !out || !acc_mask || !losses) return TIR_ERR_NULL;
+  if (!out->rgb || !out->depth || !out->normal || !out->albedo || !out->rough || !out->fresnel || !out->nd || !out->no)
+    return TIR_ERR_NULL;
+  return 1;
+}
+
+inline int epi_bwd_check(int64_t n, const float* packed, const float* acc, const float* depth, const float* rays,
+                         const TirRayMaps* g_out, const float* g_packed, const float* g_acc, const float* g_depth) {
+  if (n <= 0) return 0;
+  if (!packed || !acc || !depth || !rays || !g_out || !g_packed || !g_acc || !g_depth) return TIR_ERR_NULL;
+  return 1;
 }

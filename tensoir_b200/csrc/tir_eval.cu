@@ -203,8 +203,8 @@ __global__ void __launch_bounds__(kThreads) eval_pairs_finalize_kernel(const dou
 }  // namespace
 
 extern "C" int tir_eval_pairs_work_size(int32_t P, int32_t H, int32_t W, int64_t* n_doubles) {
-  if (!n_doubles) return TIR_ERR_NULL;
-  if (P < 0 || H < 0 || W < 0) return TIR_ERR_SHAPE;
+  const int rc = eval_pairs_work_size_check(P, H, W, n_doubles);
+  if (rc <= 0) return rc;
   *n_doubles = eval_pairs_work_doubles(P, H, W);
   return TIR_OK;
 }
@@ -236,8 +236,8 @@ extern "C" int tir_eval_pairs(const float* a, const float* b, int32_t P, int32_t
 }
 
 extern "C" int tir_eval_work_size(int32_t H, int32_t W, int64_t* n_doubles) {
-  if (!n_doubles) return TIR_ERR_NULL;
-  if (H < 0 || W < 0) return TIR_ERR_SHAPE;
+  const int rc = eval_work_size_check(H, W, n_doubles);
+  if (rc <= 0) return rc;
   *n_doubles = eval_work_doubles(H, W);
   return TIR_OK;
 }
@@ -245,12 +245,10 @@ extern "C" int tir_eval_work_size(int32_t H, int32_t W, int64_t* n_doubles) {
 extern "C" int tir_eval_view(const TirEvalView* view, double* work, int64_t work_cap, double* out, void* stream) {
   bool has_albedo = false, has_normal = false;
   int n_ssim = 0;
-  const int rc = eval_validate(view, &has_albedo, &has_normal, &n_ssim);
+  const int rc = eval_view_check(view, work, work_cap, out, &has_albedo, &has_normal, &n_ssim);
   if (rc <= 0) return rc;
-  if (!work || !out) return TIR_ERR_NULL;
   const TirEvalView v = *view;
   const int64_t n_tiles = n_ssim ? eval_ssim_tiles(v.H, v.W) : 0;
-  if (work_cap < eval_work_doubles(v.H, v.W)) return TIR_ERR_CAPACITY;
   cudaStream_t s = (cudaStream_t)stream;
   eval_pixel_kernel<<<EVAL_PIX_BLOCKS, kThreads, 0, s>>>(v, has_albedo, has_normal, work);
   if (n_ssim) {

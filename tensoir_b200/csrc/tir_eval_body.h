@@ -131,7 +131,14 @@ inline int64_t eval_work_doubles(int32_t H, int32_t W) {
   return (int64_t)EVAL_N_PIX * EVAL_PIX_BLOCKS + 4 * eval_ssim_tiles(H, W);
 }
 
-// 1: run, 0: nothing to do (zero pixels), < 0: TirStatus
+// The whole argument check of each entry, run by tir_eval.cu and its host builds before their launches / loops:
+// 1 run, 0 nothing to do, < 0 TirStatus
+inline int eval_work_size_check(int32_t H, int32_t W, const int64_t* n_doubles) {
+  if (!n_doubles) return TIR_ERR_NULL;
+  return (H < 0 || W < 0) ? TIR_ERR_SHAPE : 1;
+}
+
+// the view's own fields; 0 for zero pixels
 inline int eval_validate(const TirEvalView* v, bool* has_albedo, bool* has_normal, int* n_ssim) {
   if (!v) return TIR_ERR_NULL;
   if (v->H < 0 || v->W < 0) return TIR_ERR_SHAPE;
@@ -150,6 +157,14 @@ inline int eval_validate(const TirEvalView* v, bool* has_albedo, bool* has_norma
   return 1;
 }
 
+inline int eval_view_check(const TirEvalView* v, const double* work, int64_t work_cap, const double* out,
+                           bool* has_albedo, bool* has_normal, int* n_ssim) {
+  const int rc = eval_validate(v, has_albedo, has_normal, n_ssim);
+  if (rc <= 0) return rc;
+  if (!work || !out) return TIR_ERR_NULL;
+  return work_cap < eval_work_doubles(v->H, v->W) ? TIR_ERR_CAPACITY : 1;
+}
+
 // ---- tir_eval_pairs: [P * EVAL_PAIR_SSE_BLOCKS] squared-error partials, then [P * tiles] SSIM partials -------------
 #define EVAL_PAIR_SSE_BLOCKS 64
 
@@ -157,7 +172,12 @@ inline int64_t eval_pairs_work_doubles(int32_t P, int32_t H, int32_t W) {
   return (int64_t)P * (EVAL_PAIR_SSE_BLOCKS + eval_ssim_tiles(H, W));
 }
 
-// 1: run, 0: nothing to do (no pairs), < 0: TirStatus
+inline int eval_pairs_work_size_check(int32_t P, int32_t H, int32_t W, const int64_t* n_doubles) {
+  if (!n_doubles) return TIR_ERR_NULL;
+  return (P < 0 || H < 0 || W < 0) ? TIR_ERR_SHAPE : 1;
+}
+
+// 0 for no pairs
 inline int eval_pairs_validate(const float* a, const float* b, int32_t P, int32_t H, int32_t W, const double* work,
                                int64_t work_cap, const double* out) {
   if (P < 0 || H < 0 || W < 0) return TIR_ERR_SHAPE;

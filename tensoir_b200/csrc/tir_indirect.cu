@@ -222,15 +222,9 @@ extern "C" int tir_indirect_sample(const float* rays, const float* depth, const 
                                    int64_t n, int32_t K, float acc_mask_threshold, const float* rescale,
                                    const double* u, float* dir, float* T, int32_t* pos, float* list_o, float* list_d,
                                    int64_t capacity, int64_t* count, void* stream) {
-  const int rc = ind_check_slots(n, K);
+  const int rc = ind_sample_check(rays, depth, normal, albedo, rough, rough_stride, fresnel, acc, n, K, rescale, u, dir,
+                                  T, pos, list_o, list_d, capacity, count);
   if (rc <= 0) return rc;
-  if (!rays || !depth || !normal || !albedo || !rough || !fresnel || !acc || !rescale || !u || !dir || !T || !pos ||
-      !count)
-    return TIR_ERR_NULL;
-  if (rough_stride != 1 && rough_stride != 3) return TIR_ERR_SHAPE;
-  const int lrc = rl_check_list(capacity, list_o, list_d);
-  if (lrc) return lrc;
-  if (n == 0) return TIR_OK;
   SampleParams p{};
   p.rays = rays; p.depth = depth; p.normal = normal; p.albedo = albedo; p.rough = rough; p.rough_stride = rough_stride;
   p.fresnel = fresnel; p.acc = acc; p.n = n; p.K = K; p.thr = acc_mask_threshold; p.u = u; p.dir = dir; p.T = T;
@@ -243,8 +237,7 @@ extern "C" int tir_indirect_sample(const float* rays, const float* depth, const 
 }
 
 extern "C" int tir_indirect_hits_work_size(int64_t n, int32_t K, int64_t* bytes) {
-  if (!bytes) return TIR_ERR_NULL;
-  const int rc = ind_check_slots(n, K);
+  const int rc = ind_hits_work_size_check(n, K, bytes);
   if (rc <= 0) return rc;
   size_t b = 0;
   const cudaError_t e = scan_temp_bytes(n * K, &b);
@@ -257,15 +250,10 @@ extern "C" int tir_indirect_hits(int64_t n, int32_t K, const int32_t* pos, const
                                  const float* t_last, const float* acc, const float* depth, int32_t vis_kind,
                                  const float* aabb, float* hit_rays, float* xn, float* w, int32_t* hit,
                                  int64_t capacity, int64_t* count, void* work, int64_t work_bytes, void* stream) {
-  const int rc = ind_check_slots(n, K);
-  if (rc <= 0) return rc;
-  if (!pos || !aabb || !hit || !count) return TIR_ERR_NULL;
-  if (vis_kind != 0 && vis_kind != 1) return TIR_ERR_CONFIG;
-  if (capacity < 0 || capacity > INT32_MAX) return TIR_ERR_SHAPE;
-  if (capacity > 0 && (!hit_rays || !xn || !w)) return TIR_ERR_NULL;
-  if (n == 0) return (int)cudaMemsetAsync(count, 0, sizeof(int64_t), (cudaStream_t)stream);
-  // an empty secondary list has no march outputs: every slot then has pos -1 and they are never read
-  if (!list_o || !list_d || !t_last || !acc || !depth) return TIR_ERR_NULL;
+  const int rc = ind_hits_check(n, K, pos, list_o, list_d, t_last, acc, depth, vis_kind, aabb, hit_rays, xn, w, hit,
+                                capacity, count);
+  if (rc < 0) return rc;
+  if (rc == 0) return (int)cudaMemsetAsync(count, 0, sizeof(int64_t), (cudaStream_t)stream);
   const int64_t slots = n * K;
   size_t temp = 0;
   cudaError_t e = scan_temp_bytes(slots, &temp);
@@ -293,15 +281,9 @@ extern "C" int tir_indirect_radiance(const TirEnvMap* envs, int32_t n_lights, co
                                      const float* rescale, const int32_t* bin, const int32_t* pos,
                                      const float* vis_list, int32_t vis_kind, float* Lo, int64_t out_rows,
                                      int64_t row0, void* stream) {
-  const int rc = rl_validate(envs, n_lights, m, n_samples);
-  if (rc < 0) return rc;
-  if (ind_check_samples(n_samples) < 0) return TIR_ERR_SHAPE;
-  if (!hit_rays || !normal || !albedo || !rough || !fresnel || !rescale || !bin || !pos || !vis_list || !Lo)
-    return TIR_ERR_NULL;
-  if (rough_stride != 1 && rough_stride != 3) return TIR_ERR_SHAPE;
-  if (vis_kind != 0 && vis_kind != 1) return TIR_ERR_CONFIG;
-  if (row0 < 0 || row0 + m > out_rows || m > INT32_MAX) return TIR_ERR_SHAPE;
-  if (rc == 0) return TIR_OK;
+  const int rc = ind_radiance_check(envs, n_lights, hit_rays, normal, albedo, rough, rough_stride, fresnel, m,
+                                    n_samples, rescale, bin, pos, vis_list, vis_kind, Lo, out_rows, row0);
+  if (rc <= 0) return rc;
   RadianceParams p{};
   copy_envs(p.env, envs, n_lights);
   p.rays = hit_rays; p.normal = normal; p.albedo = albedo; p.rough = rough; p.rough_stride = rough_stride;
@@ -321,17 +303,10 @@ extern "C" int tir_indirect_shade(const TirEnvMap* envs, int32_t n_lights, const
                                   int32_t vis_kind, int32_t K, const float* T, const int32_t* hit, const float* w,
                                   const float* Lo, int64_t m_h, float* with_bg, float* without_bg, float* indirect,
                                   int64_t out_rows, int64_t row0, void* stream) {
-  const int rc = rl_validate(envs, n_lights, n, n_samples);
-  if (rc < 0) return rc;
-  if (n_samples <= 0 || ind_check_slots(n, K) < 0 || m_h < 0 || m_h > INT32_MAX) return TIR_ERR_SHAPE;
-  if (!rays || !normal || !albedo || !rough || !fresnel || !acc || !rescale || !bin || !pos || !T || !hit ||
-      !with_bg || !without_bg)
-    return TIR_ERR_NULL;
-  if (m_h > 0 && (!w || !Lo)) return TIR_ERR_NULL;
-  if (rough_stride != 1 && rough_stride != 3) return TIR_ERR_SHAPE;
-  if (vis_kind != 0 && vis_kind != 1) return TIR_ERR_CONFIG;
-  if (row0 < 0 || row0 + n > out_rows) return TIR_ERR_SHAPE;
-  if (rc == 0) return TIR_OK;
+  const int rc = ind_shade_check(envs, n_lights, rays, normal, albedo, rough, rough_stride, fresnel, acc, n, n_samples,
+                                 rescale, bin, pos, vis_kind, K, T, hit, w, Lo, m_h, with_bg, without_bg, out_rows,
+                                 row0);
+  if (rc <= 0) return rc;
   ShadeParams p{};
   copy_envs(p.env, envs, n_lights);
   p.rays = rays; p.normal = normal; p.albedo = albedo; p.rough = rough; p.rough_stride = rough_stride;

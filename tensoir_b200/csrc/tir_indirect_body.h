@@ -74,3 +74,76 @@ inline int ind_check_slots(int64_t n, int32_t K) {
   return 1;
 }
 inline int ind_check_samples(int32_t S2) { return (S2 < 1 || S2 > 1024) ? TIR_ERR_SHAPE : 1; }
+
+// The whole argument check of each entry, run by tir_indirect.cu and its host build before their launch / loop:
+// 1 run, 0 nothing to do, < 0 TirStatus
+inline int ind_sample_check(const float* rays, const float* depth, const float* normal, const float* albedo,
+                            const float* rough, int32_t rough_stride, const float* fresnel, const float* acc, int64_t n,
+                            int32_t K, const float* rescale, const double* u, const float* dir, const float* T,
+                            const int32_t* pos, const float* list_o, const float* list_d, int64_t capacity,
+                            const int64_t* count) {
+  const int rc = ind_check_slots(n, K);
+  if (rc <= 0) return rc;
+  if (!rays || !depth || !normal || !albedo || !rough || !fresnel || !acc || !rescale || !u || !dir || !T || !pos ||
+      !count)
+    return TIR_ERR_NULL;
+  if (rough_stride != 1 && rough_stride != 3) return TIR_ERR_SHAPE;
+  const int lrc = rl_check_list(capacity, list_o, list_d);
+  if (lrc) return lrc;
+  return n == 0 ? 0 : 1;
+}
+
+inline int ind_hits_work_size_check(int64_t n, int32_t K, const int64_t* bytes) {
+  if (!bytes) return TIR_ERR_NULL;
+  return ind_check_slots(n, K);
+}
+
+// 0 (n == 0): the caller only zeroes *count
+inline int ind_hits_check(int64_t n, int32_t K, const int32_t* pos, const float* list_o, const float* list_d,
+                          const float* t_last, const float* acc, const float* depth, int32_t vis_kind,
+                          const float* aabb, const float* hit_rays, const float* xn, const float* w, const int32_t* hit,
+                          int64_t capacity, const int64_t* count) {
+  const int rc = ind_check_slots(n, K);
+  if (rc <= 0) return rc;
+  if (!pos || !aabb || !hit || !count) return TIR_ERR_NULL;
+  if (vis_kind != 0 && vis_kind != 1) return TIR_ERR_CONFIG;
+  if (capacity < 0 || capacity > INT32_MAX) return TIR_ERR_SHAPE;
+  if (capacity > 0 && (!hit_rays || !xn || !w)) return TIR_ERR_NULL;
+  if (n == 0) return 0;
+  // an empty secondary list has no march outputs: every slot then has pos -1 and they are never read
+  if (!list_o || !list_d || !t_last || !acc || !depth) return TIR_ERR_NULL;
+  return 1;
+}
+
+inline int ind_radiance_check(const TirEnvMap* envs, int32_t n_lights, const float* hit_rays, const float* normal,
+                              const float* albedo, const float* rough, int32_t rough_stride, const float* fresnel,
+                              int64_t m, int32_t n_samples, const float* rescale, const int32_t* bin,
+                              const int32_t* pos, const float* vis_list, int32_t vis_kind, const float* Lo,
+                              int64_t out_rows, int64_t row0) {
+  const int rc = rl_validate(envs, n_lights, m, n_samples);
+  if (rc < 0) return rc;
+  if (ind_check_samples(n_samples) < 0) return TIR_ERR_SHAPE;
+  if (!hit_rays || !normal || !albedo || !rough || !fresnel || !rescale || !bin || !pos || !vis_list || !Lo)
+    return TIR_ERR_NULL;
+  const int wrc = rl_check_window(rough_stride, vis_kind, m, out_rows, row0);
+  if (wrc) return wrc;
+  if (m > INT32_MAX) return TIR_ERR_SHAPE;
+  return rc;
+}
+
+inline int ind_shade_check(const TirEnvMap* envs, int32_t n_lights, const float* rays, const float* normal,
+                           const float* albedo, const float* rough, int32_t rough_stride, const float* fresnel,
+                           const float* acc, int64_t n, int32_t n_samples, const float* rescale, const int32_t* bin,
+                           const int32_t* pos, int32_t vis_kind, int32_t K, const float* T, const int32_t* hit,
+                           const float* w, const float* Lo, int64_t m_h, const float* with_bg,
+                           const float* without_bg, int64_t out_rows, int64_t row0) {
+  const int rc = rl_validate(envs, n_lights, n, n_samples);
+  if (rc < 0) return rc;
+  if (n_samples <= 0 || ind_check_slots(n, K) < 0 || m_h < 0 || m_h > INT32_MAX) return TIR_ERR_SHAPE;
+  if (!rays || !normal || !albedo || !rough || !fresnel || !acc || !rescale || !bin || !pos || !T || !hit ||
+      !with_bg || !without_bg)
+    return TIR_ERR_NULL;
+  if (m_h > 0 && (!w || !Lo)) return TIR_ERR_NULL;
+  const int wrc = rl_check_window(rough_stride, vis_kind, n, out_rows, row0);
+  return wrc ? wrc : rc;
+}

@@ -117,11 +117,9 @@ extern "C" int tir_lights_sample(const TirLight* lights, int32_t n_lights, const
                                  const double* u, float* L, float* falloff, int32_t* pos, float* list_o, float* list_d,
                                  int64_t capacity, int64_t* count, void* stream) {
   LightsSampleParams p{};
-  const int rc = lt_validate(lights, n_lights, n, p.lt);
+  const int rc = lt_sample_check(lights, n_lights, rays, depth, normal, acc, n, u, L, falloff, pos, list_o, list_d,
+                                 capacity, count, p.lt);
   if (rc <= 0) return rc;
-  if (!rays || !depth || !normal || !acc || !u || !L || !falloff || !pos || !count) return TIR_ERR_NULL;
-  const int lrc = rl_check_list(capacity, list_o, list_d);
-  if (lrc) return lrc;
   p.n_lights = n_lights;
   p.rays = rays; p.depth = depth; p.normal = normal; p.acc = acc; p.n = n; p.thr = acc_mask_threshold; p.u = u;
   p.L = L; p.falloff = falloff; p.pos = pos; p.list_o = list_o; p.list_d = list_d; p.capacity = capacity;
@@ -139,14 +137,10 @@ extern "C" int tir_lights_shade(const TirLight* lights, int32_t n_lights, const 
                                 const float* vis_list, int32_t vis_kind, float* with_bg, float* without_bg,
                                 float* linear, int64_t out_rows, int64_t row0, void* stream) {
   LightsShadeParams p{};
-  const int rc = lt_validate(lights, n_lights, n, p.lt);
+  const int rc = lt_shade_check(lights, n_lights, rays, normal, albedo, rough, rough_stride, fresnel, acc, n, rescale,
+                                background, L, falloff, pos, vis_list, vis_kind, with_bg, without_bg, out_rows, row0,
+                                p.lt);
   if (rc <= 0) return rc;
-  if (!rays || !normal || !albedo || !rough || !fresnel || !acc || !rescale || !background || !L || !falloff || !pos ||
-      !vis_list || !with_bg || !without_bg)
-    return TIR_ERR_NULL;
-  if (rough_stride != 1 && rough_stride != 3) return TIR_ERR_SHAPE;
-  if (vis_kind != 0 && vis_kind != 1) return TIR_ERR_CONFIG;
-  if (row0 < 0 || row0 + n > out_rows) return TIR_ERR_SHAPE;
   p.n_lights = n_lights;
   p.rays = rays; p.normal = normal; p.albedo = albedo; p.rough = rough; p.rough_stride = rough_stride;
   p.fresnel = fresnel; p.acc = acc; p.n = n; p.thr = acc_mask_threshold; p.rescale = rescale;

@@ -129,3 +129,31 @@ inline int lt_validate(const TirLight* lights, int32_t n_lights, int64_t n, Ligh
   if (n * (int64_t)t.prefix[n_lights] > INT32_MAX) return TIR_ERR_SHAPE;
   return 1;
 }
+
+// The whole argument check of each entry, run by tir_lights.cu and its host build before their launch / loop:
+// 1 run, 0 nothing to do, < 0 TirStatus.  Fills the table.
+inline int lt_sample_check(const TirLight* lights, int32_t n_lights, const float* rays, const float* depth,
+                           const float* normal, const float* acc, int64_t n, const double* u, const float* L,
+                           const float* falloff, const int32_t* pos, const float* list_o, const float* list_d,
+                           int64_t capacity, const int64_t* count, LightTable& t) {
+  const int rc = lt_validate(lights, n_lights, n, t);
+  if (rc <= 0) return rc;
+  if (!rays || !depth || !normal || !acc || !u || !L || !falloff || !pos || !count) return TIR_ERR_NULL;
+  const int lrc = rl_check_list(capacity, list_o, list_d);
+  return lrc ? lrc : 1;
+}
+
+inline int lt_shade_check(const TirLight* lights, int32_t n_lights, const float* rays, const float* normal,
+                          const float* albedo, const float* rough, int32_t rough_stride, const float* fresnel,
+                          const float* acc, int64_t n, const float* rescale, const float* background, const float* L,
+                          const float* falloff, const int32_t* pos, const float* vis_list, int32_t vis_kind,
+                          const float* with_bg, const float* without_bg, int64_t out_rows, int64_t row0,
+                          LightTable& t) {
+  const int rc = lt_validate(lights, n_lights, n, t);
+  if (rc <= 0) return rc;
+  if (!rays || !normal || !albedo || !rough || !fresnel || !acc || !rescale || !background || !L || !falloff || !pos ||
+      !vis_list || !with_bg || !without_bg)
+    return TIR_ERR_NULL;
+  const int wrc = rl_check_window(rough_stride, vis_kind, n, out_rows, row0);
+  return wrc ? wrc : 1;
+}

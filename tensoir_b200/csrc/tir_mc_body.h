@@ -250,3 +250,25 @@ MC_HD int mc_validate_dims(int32_t X, int32_t Y, int32_t Z) {
   if ((int64_t)X * Y * Z > (int64_t)INT32_MAX) return TIR_ERR_SHAPE;    // the scans index points with int32
   return 1;
 }
+
+// The null and dims checks of each entry, run by tir_mesh.cu and its host build before their scratch-size check
+// (the CUB scratch differs between the builds): 1 run, < 0 TirStatus
+inline int mc_work_size_check(int32_t X, int32_t Y, int32_t Z, const int64_t* bytes) {
+  if (!bytes) return TIR_ERR_NULL;
+  return mc_validate_dims(X, Y, Z);
+}
+
+inline int mc_count_check(const float* volume, int32_t X, int32_t Y, int32_t Z, const void* work,
+                          const int64_t* totals) {
+  if (!volume || !work || !totals) return TIR_ERR_NULL;
+  return mc_validate_dims(X, Y, Z);
+}
+
+inline int mc_emit_check(const float* volume, int32_t X, int32_t Y, int32_t Z, const void* work, int64_t n_verts,
+                         int64_t n_faces, const float* verts, const int32_t* faces) {
+  if (!volume || !work) return TIR_ERR_NULL;
+  if (n_verts < 0 || n_faces < 0) return TIR_ERR_SHAPE;
+  if (n_verts > INT32_MAX || n_faces > INT32_MAX) return TIR_ERR_SHAPE;   // vertex ids and offsets are int32
+  if ((n_verts > 0 && !verts) || (n_faces > 0 && !faces)) return TIR_ERR_NULL;
+  return mc_validate_dims(X, Y, Z);
+}

@@ -175,42 +175,42 @@ cudaError_t cub_temp_bytes(int n, size_t* bytes) {
   return e;
 }
 
-int work_layout(int32_t X, int32_t Y, int32_t Z, McWork* w, size_t* temp) {
-  const int rc = mc_validate_dims(X, Y, Z);
-  if (rc < 0) return rc;
+// the scratch layout of dims that passed the entry's check
+cudaError_t work_layout(int32_t X, int32_t Y, int32_t Z, McWork* w, size_t* temp) {
   const int64_t n = (int64_t)X * Y * Z;
   const cudaError_t e = cub_temp_bytes((int)n, temp);
-  if (e) return (int)e;
-  *w = mc_work_layout(n, (int64_t)*temp);
-  return TIR_OK;
+  if (!e) *w = mc_work_layout(n, (int64_t)*temp);
+  return e;
 }
 
 }  // namespace
 
 extern "C" int tir_marching_cubes_work_size(int32_t X, int32_t Y, int32_t Z, int64_t* bytes) {
-  if (!bytes) return TIR_ERR_NULL;
+  const int rc = mc_work_size_check(X, Y, Z, bytes);
+  if (rc < 0) return rc;
   McWork w;
   size_t temp = 0;
-  const int rc = work_layout(X, Y, Z, &w, &temp);
-  if (rc) return rc;
+  const cudaError_t e = work_layout(X, Y, Z, &w, &temp);
+  if (e) return (int)e;
   *bytes = w.total;
   return TIR_OK;
 }
 
 extern "C" int tir_marching_cubes_count(const float* volume, int32_t X, int32_t Y, int32_t Z, float level, void* work,
                                         int64_t work_bytes, int64_t* totals, void* stream) {
-  if (!volume || !work || !totals) return TIR_ERR_NULL;
+  const int rc = mc_count_check(volume, X, Y, Z, work, totals);
+  if (rc < 0) return rc;
   McWork w;
   size_t temp = 0;
-  const int rc = work_layout(X, Y, Z, &w, &temp);
-  if (rc) return rc;
+  cudaError_t e = work_layout(X, Y, Z, &w, &temp);
+  if (e) return (int)e;
   if (work_bytes < w.total) return TIR_ERR_CAPACITY;
   const cudaStream_t s = (cudaStream_t)stream;
   const int n = (int)((int64_t)X * Y * Z);
   uint8_t* base = (uint8_t*)work;
   uint8_t* bits = base + w.bits;
   uint8_t* tris = base + w.tris;
-  cudaError_t e = cudaMemsetAsync(totals, 0, 2 * sizeof(int64_t), s);
+  e = cudaMemsetAsync(totals, 0, 2 * sizeof(int64_t), s);
   if (e) return (int)e;
   const dim3 grid((Z + kTZ - 1) / kTZ, (Y + kTY - 1) / kTY, (X + kXSteps - 1) / kXSteps);
   mc_count_kernel<<<grid, dim3(kTZ, kTY), 0, s>>>(volume, X, Y, Z, level, bits, tris,
@@ -228,14 +228,12 @@ extern "C" int tir_marching_cubes_count(const float* volume, int32_t X, int32_t 
 extern "C" int tir_marching_cubes_emit(const float* volume, int32_t X, int32_t Y, int32_t Z, float level, double sx,
                                        double sy, double sz, const void* work, int64_t work_bytes, int64_t n_verts,
                                        int64_t n_faces, float* verts, int32_t* faces, void* stream) {
-  if (!volume || !work) return TIR_ERR_NULL;
-  if (n_verts < 0 || n_faces < 0) return TIR_ERR_SHAPE;
-  if (n_verts > INT32_MAX || n_faces > INT32_MAX) return TIR_ERR_SHAPE;   // vertex ids and offsets are int32
-  if ((n_verts > 0 && !verts) || (n_faces > 0 && !faces)) return TIR_ERR_NULL;
+  const int rc = mc_emit_check(volume, X, Y, Z, work, n_verts, n_faces, verts, faces);
+  if (rc < 0) return rc;
   McWork w;
   size_t temp = 0;
-  const int rc = work_layout(X, Y, Z, &w, &temp);
-  if (rc) return rc;
+  cudaError_t e = work_layout(X, Y, Z, &w, &temp);
+  if (e) return (int)e;
   if (work_bytes < w.total) return TIR_ERR_CAPACITY;
   const uint8_t* base = (const uint8_t*)work;
   EmitParams p{};
@@ -249,7 +247,7 @@ extern "C" int tir_marching_cubes_emit(const float* volume, int32_t X, int32_t Y
   p.cap_v = n_verts; p.cap_f = n_faces; p.verts = verts; p.faces = faces;
   const cudaStream_t s = (cudaStream_t)stream;
   int dev = 0, sms = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  e = cudaGetDevice(&dev);
   if (!e) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   if (e) return (int)e;
   const int64_t n = (int64_t)X * Y * Z;

@@ -213,3 +213,38 @@ inline int mis_validate(const TirEnvMap* envs, int32_t n_lights, int64_t n, int3
   if (rough_stride != 1 && rough_stride != 3) return TIR_ERR_SHAPE;
   return rl_validate(envs, n_lights, n, S_l);
 }
+
+// The whole argument check of each entry, run by tir_relight_mis.cu and its host build before their launch / loop:
+// 1 run, 0 nothing to do, < 0 TirStatus
+inline int mis_sample_check(const TirEnvMap* envs, int32_t n_lights, const float* rays, const float* depth,
+                            const float* normal, const float* albedo, const float* rough, int32_t rough_stride,
+                            const float* fresnel, const float* acc, int64_t n, int32_t S_l, int32_t S_b,
+                            const double* u_light, const double* u_brdf, const float* dir, const int32_t* pos,
+                            const float* list_o, const float* list_d, int64_t capacity, const int64_t* count) {
+  const int rc = mis_validate(envs, n_lights, n, S_l, S_b, rough_stride);
+  if (rc < 0) return rc;
+  // a bad capacity fails even with nothing to do; missing lists only when there is
+  const int lrc = rl_check_list(capacity, list_o, list_d);
+  if (lrc == TIR_ERR_SHAPE) return lrc;
+  if (rc == 0) return 0;
+  if (!rays || !depth || !normal || !albedo || !rough || !fresnel || !acc || !u_light || !dir || !pos || !count)
+    return TIR_ERR_NULL;
+  if (S_b > 0 && !u_brdf) return TIR_ERR_NULL;
+  return lrc ? lrc : 1;
+}
+
+inline int mis_shade_check(const TirEnvMap* envs, int32_t n_lights, const float* rays, const float* normal,
+                           const float* albedo, const float* rough, int32_t rough_stride, const float* fresnel,
+                           const float* acc, int64_t n, int32_t S_l, int32_t S_b, const float* rescale,
+                           const float* dir, const int32_t* pos, const float* vis_list, int32_t vis_kind,
+                           const float* with_bg, const float* without_bg, int64_t out_rows, int64_t row0) {
+  const int rc = mis_validate(envs, n_lights, n, S_l, S_b, rough_stride);
+  if (rc < 0) return rc;
+  const int wrc = rl_check_window(rough_stride, vis_kind, n, out_rows, row0);
+  if (wrc) return wrc;
+  if (rc == 0) return 0;
+  if (!rays || !normal || !albedo || !rough || !fresnel || !acc || !rescale || !dir || !pos || !vis_list ||
+      !with_bg || !without_bg)
+    return TIR_ERR_NULL;
+  return 1;
+}

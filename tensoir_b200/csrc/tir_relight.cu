@@ -103,11 +103,9 @@ extern "C" int tir_relight_sample(const TirEnvMap* envs, int32_t n_lights, const
                                   const float* normal, const float* acc, int64_t n, int32_t n_samples,
                                   float acc_mask_threshold, const double* u, int32_t* bin, int32_t* pos,
                                   float* list_o, float* list_d, int64_t capacity, int64_t* count, void* stream) {
-  const int rc = rl_validate(envs, n_lights, n, n_samples);
-  if (rc <= 0 || n_samples == 0) return rc < 0 ? rc : TIR_OK;
-  if (!rays || !depth || !normal || !acc || !u || !bin || !pos || !count) return TIR_ERR_NULL;
-  const int lrc = rl_check_list(capacity, list_o, list_d);
-  if (lrc) return lrc;
+  const int rc = rl_sample_check(envs, n_lights, rays, depth, normal, acc, n, n_samples, u, bin, pos, list_o, list_d,
+                                 capacity, count);
+  if (rc <= 0) return rc;
   SampleParams p{};
   for (int l = 0; l < n_lights; ++l) p.env.e[l] = envs[l];
   p.rays = rays; p.depth = depth; p.normal = normal; p.acc = acc; p.n = n; p.S = n_samples;
@@ -125,15 +123,9 @@ extern "C" int tir_relight_shade(const TirEnvMap* envs, int32_t n_lights, const 
                                  const float* rescale, const int32_t* bin, const int32_t* pos, const float* vis_list,
                                  int32_t vis_kind, float* with_bg, float* without_bg, int64_t out_rows, int64_t row0,
                                  void* stream) {
-  const int rc = rl_validate(envs, n_lights, n, n_samples);
+  const int rc = rl_shade_check(envs, n_lights, rays, normal, albedo, rough, rough_stride, fresnel, acc, n, n_samples,
+                                rescale, bin, pos, vis_kind, with_bg, without_bg, out_rows, row0);
   if (rc <= 0) return rc;
-  if (n_samples <= 0) return TIR_ERR_SHAPE;
-  if (!rays || !normal || !albedo || !rough || !fresnel || !acc || !rescale || !bin || !pos || !with_bg ||
-      !without_bg)
-    return TIR_ERR_NULL;
-  if (rough_stride != 1 && rough_stride != 3) return TIR_ERR_SHAPE;
-  if (vis_kind != 0 && vis_kind != 1) return TIR_ERR_CONFIG;
-  if (row0 < 0 || row0 + n > out_rows) return TIR_ERR_SHAPE;
   ShadeParams p{};
   for (int l = 0; l < n_lights; ++l) p.env.e[l] = envs[l];
   p.rays = rays; p.normal = normal; p.albedo = albedo; p.rough = rough; p.rough_stride = rough_stride;

@@ -143,3 +143,40 @@ inline int rl_check_list(int64_t capacity, const float* list_o, const float* lis
   if (capacity > 0 && (!list_o || !list_d)) return TIR_ERR_NULL;
   return TIR_OK;
 }
+
+// argument checks of a shade-type entry's window, shared by every shade-type check: the roughness stride, the
+// visibility kind and output rows [row0, row0 + n) inside out_rows.  TIR_OK or a TirStatus
+inline int rl_check_window(int32_t rough_stride, int32_t vis_kind, int64_t n, int64_t out_rows, int64_t row0) {
+  if (rough_stride != 1 && rough_stride != 3) return TIR_ERR_SHAPE;
+  if (vis_kind != 0 && vis_kind != 1) return TIR_ERR_CONFIG;
+  if (row0 < 0 || row0 + n > out_rows) return TIR_ERR_SHAPE;
+  return TIR_OK;
+}
+
+// The whole argument check of each entry, run by tir_relight.cu and its host build before their launch / loop:
+// 1 run, 0 nothing to do, < 0 TirStatus
+inline int rl_sample_check(const TirEnvMap* envs, int32_t n_lights, const float* rays, const float* depth,
+                           const float* normal, const float* acc, int64_t n, int32_t n_samples, const double* u,
+                           const int32_t* bin, const int32_t* pos, const float* list_o, const float* list_d,
+                           int64_t capacity, const int64_t* count) {
+  const int rc = rl_validate(envs, n_lights, n, n_samples);
+  if (rc <= 0 || n_samples == 0) return rc < 0 ? rc : 0;
+  if (!rays || !depth || !normal || !acc || !u || !bin || !pos || !count) return TIR_ERR_NULL;
+  const int lrc = rl_check_list(capacity, list_o, list_d);
+  return lrc ? lrc : 1;
+}
+
+inline int rl_shade_check(const TirEnvMap* envs, int32_t n_lights, const float* rays, const float* normal,
+                          const float* albedo, const float* rough, int32_t rough_stride, const float* fresnel,
+                          const float* acc, int64_t n, int32_t n_samples, const float* rescale, const int32_t* bin,
+                          const int32_t* pos, int32_t vis_kind, const float* with_bg, const float* without_bg,
+                          int64_t out_rows, int64_t row0) {
+  const int rc = rl_validate(envs, n_lights, n, n_samples);
+  if (rc <= 0) return rc;
+  if (n_samples <= 0) return TIR_ERR_SHAPE;
+  if (!rays || !normal || !albedo || !rough || !fresnel || !acc || !rescale || !bin || !pos || !with_bg ||
+      !without_bg)
+    return TIR_ERR_NULL;
+  const int wrc = rl_check_window(rough_stride, vis_kind, n, out_rows, row0);
+  return wrc ? wrc : 1;
+}

@@ -124,16 +124,9 @@ extern "C" int tir_relight_mis_sample(const TirEnvMap* envs, int32_t n_lights, c
                                       int32_t S_l, int32_t S_b, float acc_mask_threshold, const double* u_light,
                                       const double* u_brdf, float* dir, int32_t* pos, float* list_o, float* list_d,
                                       int64_t capacity, int64_t* count, void* stream) {
-  const int rc = mis_validate(envs, n_lights, n, S_l, S_b, rough_stride);
-  if (rc < 0) return rc;
-  // a bad capacity fails even with nothing to do; missing lists only when there is
-  const int lrc = rl_check_list(capacity, list_o, list_d);
-  if (lrc == TIR_ERR_SHAPE) return lrc;
-  if (rc == 0) return TIR_OK;
-  if (!rays || !depth || !normal || !albedo || !rough || !fresnel || !acc || !u_light || !dir || !pos || !count)
-    return TIR_ERR_NULL;
-  if (S_b > 0 && !u_brdf) return TIR_ERR_NULL;
-  if (lrc) return lrc;
+  const int rc = mis_sample_check(envs, n_lights, rays, depth, normal, albedo, rough, rough_stride, fresnel, acc, n,
+                                  S_l, S_b, u_light, u_brdf, dir, pos, list_o, list_d, capacity, count);
+  if (rc <= 0) return rc;
   SampleParams p{};
   for (int l = 0; l < n_lights; ++l) p.env.e[l] = envs[l];
   p.rays = rays; p.depth = depth; p.normal = normal; p.albedo = albedo; p.rough = rough; p.rough_stride = rough_stride;
@@ -152,14 +145,9 @@ extern "C" int tir_relight_mis_shade(const TirEnvMap* envs, int32_t n_lights, co
                                      const int32_t* pos, const float* vis_list, int32_t vis_kind, float* with_bg,
                                      float* without_bg, float* linear_out, int64_t out_rows, int64_t row0,
                                      void* stream) {
-  const int rc = mis_validate(envs, n_lights, n, S_l, S_b, rough_stride);
-  if (rc < 0) return rc;
-  if (vis_kind != 0 && vis_kind != 1) return TIR_ERR_CONFIG;
-  if (row0 < 0 || row0 + n > out_rows) return TIR_ERR_SHAPE;
-  if (rc == 0) return TIR_OK;
-  if (!rays || !normal || !albedo || !rough || !fresnel || !acc || !rescale || !dir || !pos || !vis_list ||
-      !with_bg || !without_bg)
-    return TIR_ERR_NULL;
+  const int rc = mis_shade_check(envs, n_lights, rays, normal, albedo, rough, rough_stride, fresnel, acc, n, S_l, S_b,
+                                 rescale, dir, pos, vis_list, vis_kind, with_bg, without_bg, out_rows, row0);
+  if (rc <= 0) return rc;
   ShadeParams p{};
   for (int l = 0; l < n_lights; ++l) p.env.e[l] = envs[l];
   p.rays = rays; p.normal = normal; p.albedo = albedo; p.rough = rough; p.rough_stride = rough_stride;

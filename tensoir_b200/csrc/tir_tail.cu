@@ -153,8 +153,8 @@ inline int blocks_for(int64_t n, int threads) {
 extern "C" int tir_tail_fwd(int64_t n, const float* w, const int64_t* ray, const float* rgb, const float* brdf,
                             const float* brdfj, const float* vn, const float* dn, const float* viewdirs, float* packed,
                             void* stream) {
-  if (n <= 0) return TIR_OK;
-  if (!w || !ray || !rgb || !brdf || !brdfj || !vn || !viewdirs || !packed) return TIR_ERR_NULL;
+  const int rc = tail_fwd_check(n, w, ray, rgb, brdf, brdfj, vn, viewdirs, packed);
+  if (rc <= 0) return rc;
   tail_fwd_kernel<<<blocks_for(n, 256), 256, 0, (cudaStream_t)stream>>>(n, w, ray, rgb, brdf, brdfj, vn, dn, viewdirs,
                                                                         packed);
   return (int)cudaGetLastError();
@@ -164,10 +164,8 @@ extern "C" int tir_tail_bwd(int64_t n, const float* w, const int64_t* ray, const
                             const float* brdfj, const float* vn, const float* dn, const float* viewdirs,
                             const float* g_packed, float* g_w, float* g_rgb, float* g_brdf, float* g_brdfj, float* g_vn,
                             float* g_dn, void* stream) {
-  if (n <= 0) return TIR_OK;
-  if (!w || !ray || !rgb || !brdf || !brdfj || !vn || !viewdirs || !g_packed || !g_w || !g_rgb || !g_brdf || !g_brdfj ||
-      !g_vn)
-    return TIR_ERR_NULL;
+  const int rc = tail_bwd_check(n, w, ray, rgb, brdf, brdfj, vn, viewdirs, g_packed, g_w, g_rgb, g_brdf, g_brdfj, g_vn);
+  if (rc <= 0) return rc;
   tail_bwd_kernel<<<blocks_for(n, 256), 256, 0, (cudaStream_t)stream>>>(n, w, ray, rgb, brdf, brdfj, vn, dn, viewdirs,
                                                                         g_packed, g_w, g_rgb, g_brdf, g_brdfj, g_vn, g_dn);
   return (int)cudaGetLastError();
@@ -176,10 +174,8 @@ extern "C" int tir_tail_bwd(int64_t n, const float* w, const int64_t* ray, const
 extern "C" int tir_epilogue_fwd(int64_t n, const float* packed, const float* acc, const float* depth, const float* rays,
                                 float fresnel0, int32_t bg, const TirRayMaps* out, uint8_t* acc_mask, float* losses,
                                 void* stream) {
-  if (n <= 0) return TIR_OK;
-  if (!packed || !acc || !depth || !rays || !out || !acc_mask || !losses) return TIR_ERR_NULL;
-  if (!out->rgb || !out->depth || !out->normal || !out->albedo || !out->rough || !out->fresnel || !out->nd || !out->no)
-    return TIR_ERR_NULL;
+  const int rc = epi_fwd_check(n, packed, acc, depth, rays, out, acc_mask, losses);
+  if (rc <= 0) return rc;
   epilogue_fwd_kernel<<<blocks_for(n, 128), 128, 0, (cudaStream_t)stream>>>(n, packed, acc, depth, rays, fresnel0, bg,
                                                                             *out, acc_mask, losses);
   return (int)cudaGetLastError();
@@ -188,8 +184,8 @@ extern "C" int tir_epilogue_fwd(int64_t n, const float* packed, const float* acc
 extern "C" int tir_epilogue_bwd(int64_t n, const float* packed, const float* acc, const float* depth, const float* rays,
                                 float fresnel0, int32_t bg, const TirRayMaps* g_out, const float* g_loss_albedo,
                                 const float* g_loss_rough, float* g_packed, float* g_acc, float* g_depth, void* stream) {
-  if (n <= 0) return TIR_OK;
-  if (!packed || !acc || !depth || !rays || !g_out || !g_packed || !g_acc || !g_depth) return TIR_ERR_NULL;
+  const int rc = epi_bwd_check(n, packed, acc, depth, rays, g_out, g_packed, g_acc, g_depth);
+  if (rc <= 0) return rc;
   epilogue_bwd_kernel<<<blocks_for(n, 128), 128, 0, (cudaStream_t)stream>>>(n, packed, acc, depth, rays, fresnel0, bg,
                                                                             *g_out, g_loss_albedo, g_loss_rough, g_packed,
                                                                             g_acc, g_depth);

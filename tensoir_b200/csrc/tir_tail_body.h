@@ -1,12 +1,13 @@
 // Per-sample math of the fused "primary tail": everything between the appearance heads and the per-ray maps of
 // TensorBase.forward (tensorBase_rotated_lights.py:930-975) for one appearance sample, forward and backward.
-// Shared by the CUDA kernels (tail.cu) and by a host build (tail_host.cpp) that the CPU test checks against
-// torch autograd of the expressions in tensoir_b200/primary.py — the math is validated without a GPU.
+// Shared by the CUDA kernels (tir_tail.cu, tir_primary.cu) and by a host build (tests/host_tail.cpp) that the CPU test
+// checks against torch autograd of the expressions in tensoir_b200/primary.py — the math is validated without a GPU.
 //
 // Channels of the per-ray sums: [rgb 3 | normal 3 | albedo 3 | roughness 1 | albedo cost 1 | roughness cost 1 |
 // normals_diff 1 | orientation 1] = 14, each weighted by the sample's compositing weight.
 #pragma once
 #include <math.h>
+#include "../../include/tensoir_b200.h"
 
 #if defined(__CUDACC__)
 #define TAIL_HD __host__ __device__ __forceinline__
@@ -105,4 +106,24 @@ TAIL_HD void tail_backward_sample(const TailSample& s, bool both_normals, const 
       g.dn[c] = -w * G[12] * 2.f * d;
     }
   }
+}
+
+// The whole argument check of each entry, run by tir_tail.cu and its host build before their launch / loop:
+// 1 run, 0 nothing to do, < 0 TirStatus.  dn and g_dn are optional.
+inline int tail_fwd_check(int64_t n, const float* w, const int64_t* ray, const float* rgb, const float* brdf,
+                          const float* brdfj, const float* vn, const float* viewdirs, const float* packed) {
+  if (n <= 0) return 0;
+  if (!w || !ray || !rgb || !brdf || !brdfj || !vn || !viewdirs || !packed) return TIR_ERR_NULL;
+  return 1;
+}
+
+inline int tail_bwd_check(int64_t n, const float* w, const int64_t* ray, const float* rgb, const float* brdf,
+                          const float* brdfj, const float* vn, const float* viewdirs, const float* g_packed,
+                          const float* g_w, const float* g_rgb, const float* g_brdf, const float* g_brdfj,
+                          const float* g_vn) {
+  if (n <= 0) return 0;
+  if (!w || !ray || !rgb || !brdf || !brdfj || !vn || !viewdirs || !g_packed || !g_w || !g_rgb || !g_brdf || !g_brdfj ||
+      !g_vn)
+    return TIR_ERR_NULL;
+  return 1;
 }

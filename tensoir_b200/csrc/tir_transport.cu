@@ -96,11 +96,8 @@ extern "C" int tir_transport_sample(const float* dirs, int32_t K, const float* r
                                     const float* normal, const float* acc, int64_t n, float acc_mask_threshold,
                                     int32_t* pos, float* list_o, float* list_d, int64_t capacity, int64_t* count,
                                     void* stream) {
-  const int rc = tt_validate(K, n);
+  const int rc = tt_sample_check(dirs, K, rays, depth, normal, acc, n, pos, list_o, list_d, capacity, count);
   if (rc <= 0) return rc;
-  if (!dirs || !rays || !depth || !normal || !acc || !pos || !count) return TIR_ERR_NULL;
-  const int lrc = rl_check_list(capacity, list_o, list_d);
-  if (lrc) return lrc;
   TransportSampleParams p{};
   p.dirs = dirs; p.K = K; p.rays = rays; p.depth = depth; p.normal = normal; p.acc = acc; p.n = n;
   p.thr = acc_mask_threshold; p.pos = pos; p.list_o = list_o; p.list_d = list_d; p.capacity = capacity;
@@ -116,13 +113,9 @@ extern "C" int tir_transport_build(const float* dirs, const float* domega, int32
                                    const float* fresnel, const float* acc, int64_t n, float acc_mask_threshold,
                                    const float* rescale, const int32_t* pos, const float* vis_list, int32_t vis_kind,
                                    float* T, void* stream) {
-  const int rc = tt_validate(K, n);
+  const int rc = tt_build_check(dirs, domega, K, rays, normal, albedo, rough, rough_stride, fresnel, acc, n, rescale,
+                                pos, vis_list, vis_kind, T);
   if (rc <= 0) return rc;
-  if (!dirs || !domega || !rays || !normal || !albedo || !rough || !fresnel || !acc || !rescale || !pos ||
-      !vis_list || !T)
-    return TIR_ERR_NULL;
-  if (rough_stride != 1 && rough_stride != 3) return TIR_ERR_SHAPE;
-  if (vis_kind != 0 && vis_kind != 1) return TIR_ERR_CONFIG;
   TransportBuildParams p{};
   p.dirs = dirs; p.domega = domega; p.K = K; p.rays = rays; p.normal = normal; p.albedo = albedo; p.rough = rough;
   p.rough_stride = rough_stride; p.fresnel = fresnel; p.acc = acc; p.n = n; p.thr = acc_mask_threshold;

@@ -1,7 +1,16 @@
-"""Shared test helpers: build oracle fields from golden fixtures."""
+"""Shared test helpers: build oracle fields from golden fixtures, and run the ctypes wrappers on a host build of their
+C entries (tests/host_*.cpp) with CPU tensors."""
+import contextlib
+import ctypes as C
+import os
+import subprocess
+
 import torch
 
 from oracle import tensoir_oracle as O
+from tensoir_b200 import _lib, ops
+
+HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 def oracle_field(fx, with_mask=True, requires_grad=False):
@@ -40,3 +49,50 @@ def named_oracle_params(f):
     if f.lgt_sgs is not None and f.light_rotation is not None:
         out["lgtSGs"] = f.lgt_sgs[0]
     return out
+
+
+def build_host_lib(tmpdir, *cpp_files):
+    """Compile the host builds ``cpp_files`` (names under tests/) into one shared library in tmpdir and load it, with
+    the restype and argtypes of _lib.EXPORTS bound for every tir_* entry it exports."""
+    so = os.path.join(str(tmpdir), "lib" + "_".join(os.path.splitext(f)[0] for f in cpp_files) + ".so")
+    subprocess.run(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", so]
+                   + [os.path.join(HERE, f) for f in cpp_files], check=True)
+    lib = C.CDLL(so)
+    for name, (res, args) in _lib.EXPORTS.items():
+        if hasattr(lib, name):
+            getattr(lib, name).restype, getattr(lib, name).argtypes = res, args
+    return lib
+
+
+def host_dptr(t, dtype=torch.float32, allow_none=False):
+    """_lib.dptr for a host build: exactly as strict about None, dtype and contiguity, but for a CPU tensor."""
+    if t is None:
+        if allow_none:
+            return None
+        raise _lib.TirError("required tensor is None")
+    if t.device.type != "cpu":
+        raise _lib.TirError("the host build needs CPU tensors")
+    if dtype is not None and t.dtype != dtype:
+        raise _lib.TirError(f"expected {dtype}, got {t.dtype}")
+    if not t.is_contiguous():
+        raise _lib.TirError("tensor must be contiguous")
+    return C.c_void_p(t.data_ptr())
+
+
+def use_host(monkeypatch, lib, march=None):
+    """Point the ctypes wrappers at the host build ``lib``; ``march``, if given, replaces ops.march_density, the
+    density march every relighting module calls."""
+    monkeypatch.setattr(_lib, "load", lambda: lib)
+    monkeypatch.setattr(_lib, "stream_ptr", lambda: None)
+    monkeypatch.setattr(_lib, "dptr", host_dptr)
+    if march is not None:
+        monkeypatch.setattr(ops, "march_density", march)
+
+
+@contextlib.contextmanager
+def on_host(lib):
+    """use_host for the length of a with block."""
+    import pytest
+    with pytest.MonkeyPatch.context() as mp:
+        use_host(mp, lib)
+        yield

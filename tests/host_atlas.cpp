@@ -1,16 +1,14 @@
 // Host twin of csrc/tir_atlas.cu for the CPU tests of tensoir_b200/gltf.py: the SAME C-ABI signatures
-// (include/tensoir_b200.h), argument checks and per-texel / per-face math (csrc/tir_atlas_body.h), with plain loops
-// instead of kernels.  "Device" pointers are host pointers here.
+// (include/tensoir_b200.h), the library's own argument checks (the at_*_check functions) and per-texel / per-face math
+// of csrc/tir_atlas_body.h, with plain loops instead of kernels.  "Device" pointers are host pointers here.
 #include <string.h>
 #include "../include/tensoir_b200.h"
 #include "../tensoir_b200/csrc/tir_atlas_body.h"
 
 extern "C" int tir_atlas_texels(const int32_t* faces, int64_t n_faces, const float* v, int32_t T, int32_t s,
                                 int64_t first, int64_t n, int32_t* pix, float* pos, void*) {
-  int rc = at_validate_layout(n_faces, T, s);
-  if (!rc) rc = at_validate_range(n_faces, s, first, n);
-  if (rc || n == 0) return rc;
-  if (!faces || !v || !pix || !pos) return TIR_ERR_NULL;
+  const int rc = at_texels_check(faces, n_faces, v, T, s, first, n, pix, pos);
+  if (rc <= 0) return rc;
   for (int64_t i = 0; i < n; ++i) {
     const AtTexel tx = at_texel(first + i, T, s);
     int32_t c[3];
@@ -27,11 +25,9 @@ extern "C" int tir_atlas_encode(const int32_t* faces, int64_t n_faces, const flo
                                 int64_t first, int64_t n, const float* albedo, const float* rough,
                                 const float* normal, const uint8_t* probed, uint8_t* base_color,
                                 uint8_t* metallic_roughness, uint8_t* normal_map, void*) {
-  int rc = at_validate_layout(n_faces, T, s);
-  if (!rc) rc = at_validate_range(n_faces, s, first, n);
-  if (rc || n == 0) return rc;
-  if (!faces || !v || !albedo || !rough || !normal || !probed || !base_color || !metallic_roughness || !normal_map)
-    return TIR_ERR_NULL;
+  const int rc = at_encode_check(faces, n_faces, v, T, s, first, n, albedo, rough, normal, probed, base_color,
+                                 metallic_roughness, normal_map);
+  if (rc <= 0) return rc;
   uint8_t* img[3] = {base_color, metallic_roughness, normal_map};
   for (int64_t i = 0; i < n; ++i) {
     const AtTexel tx = at_texel(first + i, T, s);
@@ -48,9 +44,8 @@ extern "C" int tir_atlas_encode(const int32_t* faces, int64_t n_faces, const flo
 
 extern "C" int tir_atlas_corners(const int32_t* faces, int64_t n_faces, const float* v, int32_t T, int32_t s,
                                  float* position, float* normal, float* tangent, float* texcoord, void*) {
-  const int rc = at_validate_layout(n_faces, T, s);
-  if (rc || n_faces == 0) return rc;
-  if (!faces || !v || !position || !normal || !tangent || !texcoord) return TIR_ERR_NULL;
+  const int rc = at_corners_check(faces, n_faces, v, T, s, position, normal, tangent, texcoord);
+  if (rc <= 0) return rc;
   for (int64_t f = 0; f < n_faces; ++f) {
     int32_t c[3];
     at_corners(faces, f, c);

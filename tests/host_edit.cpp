@@ -1,6 +1,6 @@
 // Host twin of csrc/tir_edit.cu for the CPU tests of tensoir_b200/editing.py: the SAME C-ABI signature
-// (include/tensoir_b200.h), argument checks and per-point math (csrc/tir_edit_body.h), with a loop instead of a kernel.
-// "Device" pointers are host pointers here.
+// (include/tensoir_b200.h), the library's own argument check (ed_validate) and per-point math of csrc/tir_edit_body.h,
+// with a loop instead of a kernel.  "Device" pointers are host pointers here.
 #include "../include/tensoir_b200.h"
 #include "../tensoir_b200/csrc/tir_edit_body.h"
 

@@ -1,13 +1,14 @@
 // Host twin of csrc/tir_eval.cu for the CPU tests of tensoir_b200/evaluation.py: the SAME C-ABI signatures
-// (include/tensoir_b200.h), argument checks and per-pixel / per-window math (csrc/tir_eval_body.h), with plain loops
-// instead of kernels.  "Device" pointers are host pointers here.
+// (include/tensoir_b200.h), the library's own argument checks (eval_work_size_check, eval_view_check) and per-pixel /
+// per-window math of csrc/tir_eval_body.h, with plain loops instead of kernels.  "Device" pointers are host pointers
+// here.
 #include <vector>
 #include "../include/tensoir_b200.h"
 #include "../tensoir_b200/csrc/tir_eval_body.h"
 
 extern "C" int tir_eval_work_size(int32_t H, int32_t W, int64_t* n_doubles) {
-  if (!n_doubles) return TIR_ERR_NULL;
-  if (H < 0 || W < 0) return TIR_ERR_SHAPE;
+  const int rc = eval_work_size_check(H, W, n_doubles);
+  if (rc <= 0) return rc;
   *n_doubles = eval_work_doubles(H, W);
   return TIR_OK;
 }
@@ -50,11 +51,9 @@ static double host_ssim(const TirEvalView& v, const float* a, const float* b, bo
 extern "C" int tir_eval_view(const TirEvalView* view, double* work, int64_t work_cap, double* out, void*) {
   bool has_albedo = false, has_normal = false;
   int n_ssim = 0;
-  const int rc = eval_validate(view, &has_albedo, &has_normal, &n_ssim);
+  const int rc = eval_view_check(view, work, work_cap, out, &has_albedo, &has_normal, &n_ssim);
   if (rc <= 0) return rc;
-  if (!work || !out) return TIR_ERR_NULL;
   const TirEvalView& v = *view;
-  if (work_cap < eval_work_doubles(v.H, v.W)) return TIR_ERR_CAPACITY;
   float r1 = 0.f, r3[3] = {0.f, 0.f, 0.f};
   if (has_albedo) { r1 = v.ratio[0]; r3[0] = v.ratio[1]; r3[1] = v.ratio[2]; r3[2] = v.ratio[3]; }
   double acc[EVAL_N_PIX] = {0.0, 0.0, 0.0, 0.0, 0.0};

@@ -1,7 +1,9 @@
 // Host twin of csrc/tir_indirect.cu for the tests of tensoir_b200/indirect.py: the SAME C-ABI signatures
-// (include/tensoir_b200.h), argument checks and per-slot / per-hit math (csrc/tir_indirect_body.h, and the direct loop
-// rl_direct_lane of csrc/tir_relight_body.h), with plain loops instead of kernels.  "Device" pointers are host pointers
-// here.  The secondary list is filled in slot order; the warp sums are the kernels' 32 lanes and xor butterfly.
+// (include/tensoir_b200.h), the library's own argument checks (the ind_*_check functions) and per-slot / per-hit math
+// of csrc/tir_indirect_body.h, and the direct loop rl_direct_lane of csrc/tir_relight_body.h, with plain loops instead
+// of kernels.  Only the scratch size of tir_indirect_hits differs: this build needs none.  "Device" pointers are host
+// pointers here.  The secondary list is filled in slot order; the warp sums are the kernels' 32 lanes and xor
+// butterfly.
 #include "../include/tensoir_b200.h"
 #include "../tensoir_b200/csrc/tir_indirect_body.h"
 
@@ -29,14 +31,9 @@ extern "C" int tir_indirect_sample(const float* rays, const float* depth, const 
                                    int64_t n, int32_t K, float acc_mask_threshold, const float* rescale,
                                    const double* u, float* dir, float* T, int32_t* pos, float* list_o, float* list_d,
                                    int64_t capacity, int64_t* count, void*) {
-  const int rc = ind_check_slots(n, K);
+  const int rc = ind_sample_check(rays, depth, normal, albedo, rough, rough_stride, fresnel, acc, n, K, rescale, u, dir,
+                                  T, pos, list_o, list_d, capacity, count);
   if (rc <= 0) return rc;
-  if (!rays || !depth || !normal || !albedo || !rough || !fresnel || !acc || !rescale || !u || !dir || !T || !pos ||
-      !count)
-    return TIR_ERR_NULL;
-  if (rough_stride != 1 && rough_stride != 3) return TIR_ERR_SHAPE;
-  const int lrc = rl_check_list(capacity, list_o, list_d);
-  if (lrc) return lrc;
   for (int64_t i = 0; i < n; ++i)
     for (int k = 0; k < K; ++k) {
       const int64_t t = i * K + k;
@@ -64,8 +61,7 @@ extern "C" int tir_indirect_sample(const float* rays, const float* depth, const 
 }
 
 extern "C" int tir_indirect_hits_work_size(int64_t n, int32_t K, int64_t* bytes) {
-  if (!bytes) return TIR_ERR_NULL;
-  const int rc = ind_check_slots(n, K);
+  const int rc = ind_hits_work_size_check(n, K, bytes);
   if (rc <= 0) return rc;
   *bytes = 0;
   return TIR_OK;
@@ -75,15 +71,11 @@ extern "C" int tir_indirect_hits(int64_t n, int32_t K, const int32_t* pos, const
                                  const float* t_last, const float* acc, const float* depth, int32_t vis_kind,
                                  const float* aabb, float* hit_rays, float* xn, float* w, int32_t* hit,
                                  int64_t capacity, int64_t* count, void*, int64_t, void*) {
-  const int rc = ind_check_slots(n, K);
-  if (rc <= 0) return rc;
-  if (!pos || !aabb || !hit || !count) return TIR_ERR_NULL;
-  if (vis_kind != 0 && vis_kind != 1) return TIR_ERR_CONFIG;
-  if (capacity < 0 || capacity > INT32_MAX) return TIR_ERR_SHAPE;
-  if (capacity > 0 && (!hit_rays || !xn || !w)) return TIR_ERR_NULL;
+  const int rc = ind_hits_check(n, K, pos, list_o, list_d, t_last, acc, depth, vis_kind, aabb, hit_rays, xn, w, hit,
+                                capacity, count);
+  if (rc < 0) return rc;
   *count = 0;
-  if (n == 0) return TIR_OK;
-  if (!list_o || !list_d || !t_last || !acc || !depth) return TIR_ERR_NULL;
+  if (rc == 0) return TIR_OK;
   int64_t row = 0;
   for (int64_t t = 0; t < n * K; ++t) {
     hit[t] = -1;
@@ -114,15 +106,9 @@ extern "C" int tir_indirect_radiance(const TirEnvMap* envs, int32_t n_lights, co
                                      const float* rescale, const int32_t* bin, const int32_t* pos,
                                      const float* vis_list, int32_t vis_kind, float* Lo, int64_t out_rows,
                                      int64_t row0, void*) {
-  const int rc = rl_validate(envs, n_lights, m, n_samples);
-  if (rc < 0) return rc;
-  if (ind_check_samples(n_samples) < 0) return TIR_ERR_SHAPE;
-  if (!hit_rays || !normal || !albedo || !rough || !fresnel || !rescale || !bin || !pos || !vis_list || !Lo)
-    return TIR_ERR_NULL;
-  if (rough_stride != 1 && rough_stride != 3) return TIR_ERR_SHAPE;
-  if (vis_kind != 0 && vis_kind != 1) return TIR_ERR_CONFIG;
-  if (row0 < 0 || row0 + m > out_rows || m > INT32_MAX) return TIR_ERR_SHAPE;
-  if (rc == 0) return TIR_OK;
+  const int rc = ind_radiance_check(envs, n_lights, hit_rays, normal, albedo, rough, rough_stride, fresnel, m,
+                                    n_samples, rescale, bin, pos, vis_list, vis_kind, Lo, out_rows, row0);
+  if (rc <= 0) return rc;
   for (int l = 0; l < n_lights; ++l)
     for (int64_t h = 0; h < m; ++h) {
       tir::PointCtx c;
@@ -143,17 +129,10 @@ extern "C" int tir_indirect_shade(const TirEnvMap* envs, int32_t n_lights, const
                                   int32_t vis_kind, int32_t K, const float* T, const int32_t* hit, const float* w,
                                   const float* Lo, int64_t m_h, float* with_bg, float* without_bg, float* indirect,
                                   int64_t out_rows, int64_t row0, void*) {
-  const int rc = rl_validate(envs, n_lights, n, n_samples);
-  if (rc < 0) return rc;
-  if (n_samples <= 0 || ind_check_slots(n, K) < 0 || m_h < 0 || m_h > INT32_MAX) return TIR_ERR_SHAPE;
-  if (!rays || !normal || !albedo || !rough || !fresnel || !acc || !rescale || !bin || !pos || !T || !hit ||
-      !with_bg || !without_bg)
-    return TIR_ERR_NULL;
-  if (m_h > 0 && (!w || !Lo)) return TIR_ERR_NULL;
-  if (rough_stride != 1 && rough_stride != 3) return TIR_ERR_SHAPE;
-  if (vis_kind != 0 && vis_kind != 1) return TIR_ERR_CONFIG;
-  if (row0 < 0 || row0 + n > out_rows) return TIR_ERR_SHAPE;
-  if (rc == 0) return TIR_OK;
+  const int rc = ind_shade_check(envs, n_lights, rays, normal, albedo, rough, rough_stride, fresnel, acc, n, n_samples,
+                                 rescale, bin, pos, vis_kind, K, T, hit, w, Lo, m_h, with_bg, without_bg, out_rows,
+                                 row0);
+  if (rc <= 0) return rc;
   for (int l = 0; l < n_lights; ++l)
     for (int64_t i = 0; i < n; ++i) {
       const TirEnvMap& e = envs[l];

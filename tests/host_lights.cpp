@@ -1,6 +1,7 @@
 // Host twin of csrc/tir_lights.cu for the tests of tensoir_b200/lighting.py: the SAME C-ABI signatures
-// (include/tensoir_b200.h), argument checks and per-slot / per-ray math (csrc/tir_lights_body.h), with plain loops
-// instead of kernels.  "Device" pointers are host pointers here.  The shadow-ray list is filled in slot order.
+// (include/tensoir_b200.h), the library's own argument checks (the lt_*_check functions) and per-slot / per-ray math of
+// csrc/tir_lights_body.h, with plain loops instead of kernels.  "Device" pointers are host pointers here.  The
+// shadow-ray list is filled in slot order.
 #include "../include/tensoir_b200.h"
 #include "../tensoir_b200/csrc/tir_lights_body.h"
 
@@ -9,11 +10,9 @@ extern "C" int tir_lights_sample(const TirLight* lights, int32_t n_lights, const
                                  const double* u, float* L, float* falloff, int32_t* pos, float* list_o, float* list_d,
                                  int64_t capacity, int64_t* count, void*) {
   LightTable lt;
-  const int rc = lt_validate(lights, n_lights, n, lt);
+  const int rc = lt_sample_check(lights, n_lights, rays, depth, normal, acc, n, u, L, falloff, pos, list_o, list_d,
+                                 capacity, count, lt);
   if (rc <= 0) return rc;
-  if (!rays || !depth || !normal || !acc || !u || !L || !falloff || !pos || !count) return TIR_ERR_NULL;
-  const int lrc = rl_check_list(capacity, list_o, list_d);
-  if (lrc) return lrc;
   for (int j = 0; j < n_lights; ++j)
     for (int64_t i = 0; i < n; ++i)
       for (int s = 0; s < lt.l[j].n_samples; ++s) {
@@ -41,14 +40,10 @@ extern "C" int tir_lights_shade(const TirLight* lights, int32_t n_lights, const 
                                 const float* vis_list, int32_t vis_kind, float* with_bg, float* without_bg,
                                 float* linear, int64_t out_rows, int64_t row0, void*) {
   LightTable lt;
-  const int rc = lt_validate(lights, n_lights, n, lt);
+  const int rc = lt_shade_check(lights, n_lights, rays, normal, albedo, rough, rough_stride, fresnel, acc, n, rescale,
+                                background, L, falloff, pos, vis_list, vis_kind, with_bg, without_bg, out_rows, row0,
+                                lt);
   if (rc <= 0) return rc;
-  if (!rays || !normal || !albedo || !rough || !fresnel || !acc || !rescale || !background || !L || !falloff || !pos ||
-      !vis_list || !with_bg || !without_bg)
-    return TIR_ERR_NULL;
-  if (rough_stride != 1 && rough_stride != 3) return TIR_ERR_SHAPE;
-  if (vis_kind != 0 && vis_kind != 1) return TIR_ERR_CONFIG;
-  if (row0 < 0 || row0 + n > out_rows) return TIR_ERR_SHAPE;
   for (int64_t i = 0; i < n; ++i) {
     const bool hit = acc[i] > acc_mask_threshold;
     float lin[3] = {0.f, 0.f, 0.f};

@@ -1,6 +1,7 @@
 // Host twin of csrc/tir_mesh.cu for the CPU tests of tensoir_b200/mesh.py: the SAME C-ABI signatures
-// (include/tensoir_b200.h), argument checks, scratch layout and per-cell / per-vertex math (csrc/tir_mc_body.h), with
-// plain loops instead of kernels.  "Device" pointers are host pointers here.  mc_host_cell exposes the polygonisation
+// (include/tensoir_b200.h), the library's own argument checks (the mc_*_check functions), scratch layout and per-cell /
+// per-vertex math of csrc/tir_mc_body.h, with plain loops instead of kernels.  The scratch has no CUB part here, so its
+// size check is this build's own.  "Device" pointers are host pointers here.  mc_host_cell exposes the polygonisation
 // of one cell for the all-configurations test.
 #include <string.h>
 #include "../include/tensoir_b200.h"
@@ -15,8 +16,7 @@ extern "C" int mc_host_face_connected(float v00, float v10, float v01, float v11
 }
 
 extern "C" int tir_marching_cubes_work_size(int32_t X, int32_t Y, int32_t Z, int64_t* bytes) {
-  if (!bytes) return TIR_ERR_NULL;
-  const int rc = mc_validate_dims(X, Y, Z);
+  const int rc = mc_work_size_check(X, Y, Z, bytes);
   if (rc < 0) return rc;
   *bytes = mc_work_layout((int64_t)X * Y * Z, 0).total;
   return TIR_OK;
@@ -31,8 +31,7 @@ static void corners(const float* vol, int64_t cell, int32_t Y, int32_t Z, float 
 
 extern "C" int tir_marching_cubes_count(const float* volume, int32_t X, int32_t Y, int32_t Z, float level, void* work,
                                         int64_t work_bytes, int64_t* totals, void*) {
-  if (!volume || !work || !totals) return TIR_ERR_NULL;
-  const int rc = mc_validate_dims(X, Y, Z);
+  const int rc = mc_count_check(volume, X, Y, Z, work, totals);
   if (rc < 0) return rc;
   const int64_t n = (int64_t)X * Y * Z;
   const McWork w = mc_work_layout(n, 0);
@@ -78,11 +77,7 @@ extern "C" int tir_marching_cubes_count(const float* volume, int32_t X, int32_t 
 extern "C" int tir_marching_cubes_emit(const float* volume, int32_t X, int32_t Y, int32_t Z, float level, double sx,
                                        double sy, double sz, const void* work, int64_t work_bytes, int64_t n_verts,
                                        int64_t n_faces, float* verts, int32_t* faces, void*) {
-  if (!volume || !work) return TIR_ERR_NULL;
-  if (n_verts < 0 || n_faces < 0) return TIR_ERR_SHAPE;
-  if (n_verts > INT32_MAX || n_faces > INT32_MAX) return TIR_ERR_SHAPE;
-  if ((n_verts > 0 && !verts) || (n_faces > 0 && !faces)) return TIR_ERR_NULL;
-  const int rc = mc_validate_dims(X, Y, Z);
+  const int rc = mc_emit_check(volume, X, Y, Z, work, n_verts, n_faces, verts, faces);
   if (rc < 0) return rc;
   const int64_t n = (int64_t)X * Y * Z;
   const McWork w = mc_work_layout(n, 0);

@@ -1,8 +1,8 @@
 // Host twin of csrc/tir_relight_mis.cu for the tests of tensoir_b200/mis.py: the SAME C-ABI signatures
-// (include/tensoir_b200.h), argument checks and per-sample math (csrc/tir_mis_body.h), with plain loops instead of
-// kernels.  "Device" pointers are host pointers here.  The visibility list is filled in slot order; the warp sums are
-// the kernels' 32 lanes and xor butterfly.  Two more entries expose the texel lookup and the BRDF-strategy density
-// to the stage checks.
+// (include/tensoir_b200.h), the library's own argument checks (mis_sample_check, mis_shade_check) and per-sample math
+// of csrc/tir_mis_body.h, with plain loops instead of kernels.  "Device" pointers are host pointers here.  The
+// visibility list is filled in slot order; the warp sums are the kernels' 32 lanes and xor butterfly.  Two more entries
+// expose the texel lookup and the BRDF-strategy density to the stage checks.
 #include "../include/tensoir_b200.h"
 #include "../tensoir_b200/csrc/tir_mis_body.h"
 
@@ -12,15 +12,9 @@ extern "C" int tir_relight_mis_sample(const TirEnvMap* envs, int32_t n_lights, c
                                       int32_t S_l, int32_t S_b, float acc_mask_threshold, const double* u_light,
                                       const double* u_brdf, float* dir, int32_t* pos, float* list_o, float* list_d,
                                       int64_t capacity, int64_t* count, void*) {
-  const int rc = mis_validate(envs, n_lights, n, S_l, S_b, rough_stride);
-  if (rc < 0) return rc;
-  const int lrc = rl_check_list(capacity, list_o, list_d);
-  if (lrc == TIR_ERR_SHAPE) return lrc;
-  if (rc == 0) return TIR_OK;
-  if (!rays || !depth || !normal || !albedo || !rough || !fresnel || !acc || !u_light || !dir || !pos || !count)
-    return TIR_ERR_NULL;
-  if (S_b > 0 && !u_brdf) return TIR_ERR_NULL;
-  if (lrc) return lrc;
+  const int rc = mis_sample_check(envs, n_lights, rays, depth, normal, albedo, rough, rough_stride, fresnel, acc, n,
+                                  S_l, S_b, u_light, u_brdf, dir, pos, list_o, list_d, capacity, count);
+  if (rc <= 0) return rc;
   const int64_t n_light = (int64_t)n_lights * n * S_l, total = n_light + n * S_b;
   for (int64_t t = 0; t < total; ++t) {
     const bool light = t < n_light;
@@ -62,14 +56,9 @@ extern "C" int tir_relight_mis_shade(const TirEnvMap* envs, int32_t n_lights, co
                                      float acc_mask_threshold, const float* rescale, const float* dir,
                                      const int32_t* pos, const float* vis_list, int32_t vis_kind, float* with_bg,
                                      float* without_bg, float* linear_out, int64_t out_rows, int64_t row0, void*) {
-  const int rc = mis_validate(envs, n_lights, n, S_l, S_b, rough_stride);
-  if (rc < 0) return rc;
-  if (vis_kind != 0 && vis_kind != 1) return TIR_ERR_CONFIG;
-  if (row0 < 0 || row0 + n > out_rows) return TIR_ERR_SHAPE;
-  if (rc == 0) return TIR_OK;
-  if (!rays || !normal || !albedo || !rough || !fresnel || !acc || !rescale || !dir || !pos || !vis_list ||
-      !with_bg || !without_bg)
-    return TIR_ERR_NULL;
+  const int rc = mis_shade_check(envs, n_lights, rays, normal, albedo, rough, rough_stride, fresnel, acc, n, S_l, S_b,
+                                 rescale, dir, pos, vis_list, vis_kind, with_bg, without_bg, out_rows, row0);
+  if (rc <= 0) return rc;
   for (int l = 0; l < n_lights; ++l)
     for (int64_t i = 0; i < n; ++i) {
       const TirEnvMap& e = envs[l];

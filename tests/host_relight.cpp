@@ -1,7 +1,8 @@
 // Host twin of csrc/tir_relight.cu and of tir_eval_pairs (csrc/tir_eval.cu) for the CPU tests of
-// tensoir_b200/relighting.py: the SAME C-ABI signatures (include/tensoir_b200.h), argument checks and per-sample /
-// per-ray / per-window math (csrc/tir_relight_body.h, csrc/tir_eval_body.h), with plain loops instead of kernels.
-// "Device" pointers are host pointers here.  The visibility list is filled in slot order.
+// tensoir_b200/relighting.py: the SAME C-ABI signatures (include/tensoir_b200.h), the library's own argument checks
+// (rl_sample_check, rl_shade_check, eval_pairs_work_size_check, eval_pairs_validate) and per-sample / per-ray /
+// per-window math of csrc/tir_relight_body.h and csrc/tir_eval_body.h, with plain loops instead of kernels.  "Device"
+// pointers are host pointers here.  The visibility list is filled in slot order.
 #include <vector>
 #include "../include/tensoir_b200.h"
 #include "../tensoir_b200/csrc/tir_relight_body.h"
@@ -10,11 +11,9 @@ extern "C" int tir_relight_sample(const TirEnvMap* envs, int32_t n_lights, const
                                   const float* normal, const float* acc, int64_t n, int32_t n_samples,
                                   float acc_mask_threshold, const double* u, int32_t* bin, int32_t* pos,
                                   float* list_o, float* list_d, int64_t capacity, int64_t* count, void*) {
-  const int rc = rl_validate(envs, n_lights, n, n_samples);
-  if (rc <= 0 || n_samples == 0) return rc < 0 ? rc : TIR_OK;
-  if (!rays || !depth || !normal || !acc || !u || !bin || !pos || !count) return TIR_ERR_NULL;
-  const int lrc = rl_check_list(capacity, list_o, list_d);
-  if (lrc) return lrc;
+  const int rc = rl_sample_check(envs, n_lights, rays, depth, normal, acc, n, n_samples, u, bin, pos, list_o, list_d,
+                                 capacity, count);
+  if (rc <= 0) return rc;
   for (int l = 0; l < n_lights; ++l)
     for (int64_t i = 0; i < n; ++i)
       for (int s = 0; s < n_samples; ++s) {
@@ -43,15 +42,9 @@ extern "C" int tir_relight_shade(const TirEnvMap* envs, int32_t n_lights, const 
                                  const float* rescale, const int32_t* bin, const int32_t* pos, const float* vis_list,
                                  int32_t vis_kind, float* with_bg, float* without_bg, int64_t out_rows, int64_t row0,
                                  void*) {
-  const int rc = rl_validate(envs, n_lights, n, n_samples);
+  const int rc = rl_shade_check(envs, n_lights, rays, normal, albedo, rough, rough_stride, fresnel, acc, n, n_samples,
+                                rescale, bin, pos, vis_kind, with_bg, without_bg, out_rows, row0);
   if (rc <= 0) return rc;
-  if (n_samples <= 0) return TIR_ERR_SHAPE;
-  if (!rays || !normal || !albedo || !rough || !fresnel || !acc || !rescale || !bin || !pos || !with_bg ||
-      !without_bg)
-    return TIR_ERR_NULL;
-  if (rough_stride != 1 && rough_stride != 3) return TIR_ERR_SHAPE;
-  if (vis_kind != 0 && vis_kind != 1) return TIR_ERR_CONFIG;
-  if (row0 < 0 || row0 + n > out_rows) return TIR_ERR_SHAPE;
   for (int l = 0; l < n_lights; ++l)
     for (int64_t i = 0; i < n; ++i) {
       const TirEnvMap& e = envs[l];
@@ -87,8 +80,8 @@ extern "C" int tir_relight_shade(const TirEnvMap* envs, int32_t n_lights, const 
 }
 
 extern "C" int tir_eval_pairs_work_size(int32_t P, int32_t H, int32_t W, int64_t* n_doubles) {
-  if (!n_doubles) return TIR_ERR_NULL;
-  if (P < 0 || H < 0 || W < 0) return TIR_ERR_SHAPE;
+  const int rc = eval_pairs_work_size_check(P, H, W, n_doubles);
+  if (rc <= 0) return rc;
   *n_doubles = eval_pairs_work_doubles(P, H, W);
   return TIR_OK;
 }

@@ -1,6 +1,7 @@
 // Host twin of csrc/tir_transport.cu for the tests of tensoir_b200/light_fit.py: the SAME C-ABI signatures
-// (include/tensoir_b200.h), argument checks and per-(hit, texel) math (csrc/tir_transport_body.h), with plain loops
-// instead of kernels.  "Device" pointers are host pointers here.  The visibility list is filled in (ray, texel) order.
+// (include/tensoir_b200.h), the library's own argument checks (tt_sample_check, tt_build_check) and per-(hit, texel)
+// math of csrc/tir_transport_body.h, with plain loops instead of kernels.  "Device" pointers are host pointers here.
+// The visibility list is filled in (ray, texel) order.
 #include "../include/tensoir_b200.h"
 #include "../tensoir_b200/csrc/tir_transport_body.h"
 
@@ -8,11 +9,8 @@ extern "C" int tir_transport_sample(const float* dirs, int32_t K, const float* r
                                     const float* normal, const float* acc, int64_t n, float acc_mask_threshold,
                                     int32_t* pos, float* list_o, float* list_d, int64_t capacity, int64_t* count,
                                     void*) {
-  const int rc = tt_validate(K, n);
+  const int rc = tt_sample_check(dirs, K, rays, depth, normal, acc, n, pos, list_o, list_d, capacity, count);
   if (rc <= 0) return rc;
-  if (!dirs || !rays || !depth || !normal || !acc || !pos || !count) return TIR_ERR_NULL;
-  const int lrc = rl_check_list(capacity, list_o, list_d);
-  if (lrc) return lrc;
   for (int64_t i = 0; i < n; ++i)
     for (int k = 0; k < K; ++k) {
       const int64_t t = i * K + k;
@@ -34,13 +32,9 @@ extern "C" int tir_transport_build(const float* dirs, const float* domega, int32
                                    const float* fresnel, const float* acc, int64_t n, float acc_mask_threshold,
                                    const float* rescale, const int32_t* pos, const float* vis_list, int32_t vis_kind,
                                    float* T, void*) {
-  const int rc = tt_validate(K, n);
+  const int rc = tt_build_check(dirs, domega, K, rays, normal, albedo, rough, rough_stride, fresnel, acc, n, rescale,
+                                pos, vis_list, vis_kind, T);
   if (rc <= 0) return rc;
-  if (!dirs || !domega || !rays || !normal || !albedo || !rough || !fresnel || !acc || !rescale || !pos ||
-      !vis_list || !T)
-    return TIR_ERR_NULL;
-  if (rough_stride != 1 && rough_stride != 3) return TIR_ERR_SHAPE;
-  if (vis_kind != 0 && vis_kind != 1) return TIR_ERR_CONFIG;
   const int64_t plane = n * K;
   for (int64_t i = 0; i < n; ++i) {
     const bool hit = acc[i] > acc_mask_threshold;

@@ -1,45 +1,18 @@
-"""Shared pieces of the mesh-export tests: the host build of the tir_marching_cubes_* C ABI (tests/host_mesh.cpp),
-mesh checks, and the random / analytic test volumes."""
-import ctypes as C
-import os
-import subprocess
-
+"""Shared pieces of the mesh-export tests: tensoir_b200.mesh.extract on the host build of the tir_marching_cubes_* C ABI
+(tests/host_mesh.cpp), mesh checks, and the random / analytic test volumes."""
 import numpy as np
 import torch
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ENTRY = ("tir_marching_cubes_work_size", "tir_marching_cubes_count", "tir_marching_cubes_emit")
+from helpers import on_host
+
 LEVEL = 0.5
-
-
-def build_host_lib(dirpath):
-    from tensoir_b200 import _lib
-    so = os.path.join(str(dirpath), "libhost_mesh.so")
-    subprocess.run(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", so,
-                    os.path.join(HERE, "host_mesh.cpp")], check=True)
-    lib = C.CDLL(so)
-    for name in ENTRY:
-        res, args = _lib.EXPORTS[name]
-        getattr(lib, name).restype, getattr(lib, name).argtypes = res, args
-    lib.mc_host_cell.restype, lib.mc_host_cell.argtypes = C.c_int, [C.c_int32, C.c_int32, C.c_void_p]
-    lib.mc_host_face_connected.restype = C.c_int
-    lib.mc_host_face_connected.argtypes = [C.c_float] * 5
-    return lib
 
 
 def host_marching_cubes(lib, vol, level, spacing=(1.0, 1.0, 1.0)):
     """tensoir_b200.mesh.extract through the real ctypes wrapper, on the host build."""
-    from tensoir_b200 import _lib, mesh
-    saved = _lib.load, _lib.stream_ptr, _lib.dptr
-
-    def host_dptr(t, dtype=torch.float32, allow_none=False):
-        assert t.dtype == dtype and t.is_contiguous() and not t.is_cuda
-        return C.c_void_p(t.data_ptr())
-    _lib.load, _lib.stream_ptr, _lib.dptr = (lambda: lib), (lambda: None), host_dptr
-    try:
+    from tensoir_b200 import mesh
+    with on_host(lib):
         v, f = mesh.extract(torch.from_numpy(np.ascontiguousarray(vol, dtype=np.float32)), level, spacing)
-    finally:
-        _lib.load, _lib.stream_ptr, _lib.dptr = saved
     return v.numpy(), f.numpy()
 
 

@@ -6,7 +6,8 @@ import numpy as np
 import pytest
 import torch
 
-from mesh_helpers import LEVEL, build_host_lib, host_marching_cubes, random_volume
+from helpers import build_host_lib
+from mesh_helpers import LEVEL, host_marching_cubes, random_volume
 from oracle import tensoir_oracle as O
 from tensoir_b200 import mesh
 
@@ -23,7 +24,7 @@ RECORD = np.dtype({"names": ["x", "y", "z", "nx", "ny", "nz", "red", "green", "b
 
 @pytest.fixture(scope="module")
 def lib(tmp_path_factory):
-    return build_host_lib(tmp_path_factory.mktemp("host_mesh"))
+    return build_host_lib(tmp_path_factory.mktemp("host_mesh"), "host_mesh.cpp")
 
 
 def _hand_mesh(V=7, F=5, seed=3):

@@ -14,6 +14,7 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import build_host_lib, use_host
 from oracle import eval_oracle as EO
 from tensoir_b200 import _lib, evaluation
 
@@ -23,28 +24,12 @@ REPO = os.path.dirname(HERE)
 
 @pytest.fixture(scope="module")
 def host_so(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("host_eval") / "libhost_eval.so")
-    subprocess.run(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", so, os.path.join(HERE, "host_eval.cpp")],
-                   check=True)
-    lib = C.CDLL(so)
-    for name in ("tir_eval_work_size", "tir_eval_view"):
-        res, args = _lib.EXPORTS[name]
-        getattr(lib, name).restype, getattr(lib, name).argtypes = res, args
-    return lib
+    return build_host_lib(tmp_path_factory.mktemp("host_eval"), "host_eval.cpp")
 
 
 @pytest.fixture
 def host_lib(host_so, monkeypatch):
-    monkeypatch.setattr(_lib, "load", lambda: host_so)
-    monkeypatch.setattr(_lib, "stream_ptr", lambda: None)
-
-    def host_dptr(t, dtype=torch.float32, allow_none=False):
-        if t is None:
-            assert allow_none
-            return None
-        assert t.dtype == dtype and t.is_contiguous()
-        return C.c_void_p(t.data_ptr())
-    monkeypatch.setattr(_lib, "dptr", host_dptr)
+    use_host(monkeypatch, host_so)
     return host_so
 
 

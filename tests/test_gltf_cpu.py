@@ -1,54 +1,24 @@
 """Textured glTF export on the CPU, through the host twin of csrc/tir_atlas.cu (tests/host_atlas.cpp, the same body
 header): the atlas layout and its no-bleed guarantee, the texel enumeration, the probe points against float64, the
 encoding and tangent frames against glTF's decoding rules, the winding, and the .glb writer and reader."""
-import contextlib
 import ctypes as C
-import os
 import struct
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-from mesh_helpers import build_host_lib as build_mesh_lib, host_marching_cubes, sphere_volume
+from helpers import build_host_lib, on_host
+from mesh_helpers import host_marching_cubes, sphere_volume
 from tensoir_b200 import _lib, gltf
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-ENTRY = ("tir_atlas_texels", "tir_atlas_encode", "tir_atlas_corners")
-
-
-def build_host_lib(dirpath):
-    so = os.path.join(str(dirpath), "libhost_atlas.so")
-    subprocess.run(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", so,
-                    os.path.join(HERE, "host_atlas.cpp")], check=True)
-    lib = C.CDLL(so)
-    for name in ENTRY:
-        res, args = _lib.EXPORTS[name]
-        getattr(lib, name).restype, getattr(lib, name).argtypes = res, args
-    lib.at_host_frame.restype = C.c_int
-    lib.at_host_frame.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
-    return lib
-
-
-@contextlib.contextmanager
-def on_host(lib):
-    """tensoir_b200.gltf's ctypes wrappers running on the host build ``lib`` with CPU tensors."""
-    saved = _lib.load, _lib.stream_ptr, _lib.dptr
-
-    def host_dptr(t, dtype=torch.float32, allow_none=False):
-        assert t.dtype == dtype and t.is_contiguous() and not t.is_cuda
-        return C.c_void_p(t.data_ptr())
-    _lib.load, _lib.stream_ptr, _lib.dptr = (lambda: lib), (lambda: None), host_dptr
-    try:
-        yield
-    finally:
-        _lib.load, _lib.stream_ptr, _lib.dptr = saved
 
 
 @pytest.fixture(scope="module")
 def lib(tmp_path_factory):
-    return build_host_lib(tmp_path_factory.mktemp("host_atlas"))
+    lib = build_host_lib(tmp_path_factory.mktemp("host_atlas"), "host_atlas.cpp")
+    lib.at_host_frame.restype = C.c_int
+    lib.at_host_frame.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    return lib
 
 
 def random_mesh(F, V=None, seed=0):
@@ -320,7 +290,7 @@ def test_tangent_frames(lib):
 
 def test_triangles_face_outward_on_the_sphere(lib, tmp_path):
     shape = (41, 37, 45)
-    mesh_lib = build_mesh_lib(tmp_path)
+    mesh_lib = build_host_lib(tmp_path, "host_mesh.cpp")
     verts, faces = host_marching_cubes(mesh_lib, sphere_volume(shape), 0.5)
     F = faces.shape[0]
     T = 256 if (256 // 6) ** 2 >= (F + 1) // 2 else 512

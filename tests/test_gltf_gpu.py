@@ -14,11 +14,11 @@ import torch
 pytestmark = pytest.mark.gpu
 
 from oracle import tensoir_oracle as O                                      # noqa: E402
-from helpers import oracle_field                                           # noqa: E402
+from helpers import build_host_lib, on_host, oracle_field                   # noqa: E402
 from gpu_helpers import load_fixture, load_shrunk_state, model_from_fixture  # noqa: E402
 from test_gpu_parity import DEV, TOL, close                                # noqa: E402
 from test_asset_gpu import _tool                                           # noqa: E402
-from test_gltf_cpu import build_host_lib, on_host, srgb64                  # noqa: E402
+from test_gltf_cpu import srgb64                                           # noqa: E402
 from tensoir_b200 import gltf, mesh                                        # noqa: E402
 from tensoir_b200.editing import MaterialEdit                              # noqa: E402
 
@@ -34,7 +34,7 @@ def smallest_texture(F):
 
 @pytest.fixture(scope="module")
 def host(tmp_path_factory):
-    return build_host_lib(tmp_path_factory.mktemp("host_atlas_gpu"))
+    return build_host_lib(tmp_path_factory.mktemp("host_atlas_gpu"), "host_atlas.cpp")
 
 
 @pytest.fixture(scope="module", params=["rotated", "A", "B"])

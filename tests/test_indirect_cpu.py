@@ -8,13 +8,13 @@ expressions.  The sampler is checked for unbiasedness in float64 against quadrat
 import ctypes as C
 import math
 import os
-import subprocess
 import sys
 
 import numpy as np
 import pytest
 import torch
 
+from helpers import build_host_lib, use_host
 from tensoir_b200 import _lib, indirect, relighting
 from tensoir_b200.relight import Environment_Light
 from tensoir_b200.relight_utils import GGX_specular
@@ -22,21 +22,8 @@ from test_lighting_cpu import random_chunk
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(HERE)
-ENTRY = ("tir_relight_sample", "tir_relight_shade", "tir_indirect_sample", "tir_indirect_hits_work_size",
-         "tir_indirect_hits", "tir_indirect_radiance", "tir_indirect_shade")
 EPS = float(np.finfo(np.float32).eps)
 AABB = torch.tensor([[-1.5] * 3, [1.5] * 3])
-
-
-def build_host_indirect(path):
-    so = os.path.join(str(path), "libhost_indirect.so")
-    subprocess.run(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", so,
-                    os.path.join(HERE, "host_relight.cpp"), os.path.join(HERE, "host_indirect.cpp")], check=True)
-    lib = C.CDLL(so)
-    for name in ENTRY:
-        res, args = _lib.EXPORTS[name]
-        getattr(lib, name).restype, getattr(lib, name).argtypes = res, args
-    return lib
 
 
 class Model:
@@ -60,18 +47,9 @@ def plane_march(z_plane=0.2, t_last=0.25):
     return march
 
 
-def use_host(monkeypatch, lib, march):
-    monkeypatch.setattr(_lib, "load", lambda: lib)
-    monkeypatch.setattr(_lib, "stream_ptr", lambda: None)
-    monkeypatch.setattr(_lib, "dptr", lambda t, dtype=torch.float32, allow_none=False:
-                        None if t is None else C.c_void_p(t.data_ptr()))
-    monkeypatch.setattr(indirect.ops, "march_density", march)
-    monkeypatch.setattr(relighting.ops, "march_density", march)
-
-
 @pytest.fixture(scope="module")
 def host_so(tmp_path_factory):
-    return build_host_indirect(tmp_path_factory.mktemp("host_indirect"))
+    return build_host_lib(tmp_path_factory.mktemp("host_indirect"), "host_relight.cpp", "host_indirect.cpp")
 
 
 @pytest.fixture

@@ -13,6 +13,7 @@ import pytest
 import torch
 
 import test_indirect_cpu as H
+from helpers import build_host_lib, use_host
 from oracle import tensoir_oracle as O
 from tensoir_b200 import _lib, indirect, ops, relighting
 from tensoir_b200.relight import Environment_Light, read_hdr
@@ -29,7 +30,7 @@ def to(ch, dev):
 
 @pytest.fixture(scope="module")
 def host_so(tmp_path_factory):
-    return H.build_host_indirect(tmp_path_factory.mktemp("host_indirect_gpu"))
+    return build_host_lib(tmp_path_factory.mktemp("host_indirect_gpu"), "host_relight.cpp", "host_indirect.cpp")
 
 
 @pytest.fixture(scope="module")
@@ -73,7 +74,7 @@ def test_kernels_match_host_build(host_so, monkeypatch):
                                     dev_ch["rough"], dev_ch["fresnel"], dev_ch["acc"], resc.to(DEV), u.to(DEV), 0.5,
                                     'nerv')
     with monkeypatch.context() as mp:
-        H.use_host(mp, host_so, march)
+        use_host(mp, host_so, march)
         want = indirect.secondary_hits(H.Model(), ch["rays"], ch["depth"], ch["normal"], ch["albedo"], ch["rough"],
                                        ch["fresnel"], ch["acc"], resc, u, 0.5, 'nerv')
     got = {k: v.cpu() for k, v in got.items()}
@@ -115,7 +116,7 @@ def test_chunk_matches_host_build(host_so, monkeypatch, env):
     u_ind = torch.rand(2000, 8, 2, generator=g, device=DEV, dtype=torch.float64).cpu()
     light_cpu = Environment_Light(hdr, device="cpu")
     with monkeypatch.context() as mp:
-        H.use_host(mp, host_so, H.plane_march())
+        use_host(mp, host_so, H.plane_march())
         hits = indirect.secondary_hits(H.Model(), ch["rays"], ch["depth"], ch["normal"], ch["albedo"], ch["rough"],
                                        ch["fresnel"], ch["acc"], torch.ones(3), u_ind, 0.5, 'nerv')
         m_h = hits["rays"].shape[0]

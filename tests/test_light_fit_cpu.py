@@ -16,37 +16,19 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import build_host_lib, use_host
 from tensoir_b200 import _lib, light_fit as LF
 from tensoir_b200.relight_utils import GGX_specular
 from test_lighting_cpu import random_chunk
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(HERE)
-ENTRY = ("tir_transport_sample", "tir_transport_build")
 EPS = float(np.finfo(np.float32).eps)
-
-
-def build_host_transport(path):
-    so = os.path.join(str(path), "libhost_transport.so")
-    subprocess.run(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", so,
-                    os.path.join(HERE, "host_transport.cpp")], check=True)
-    lib = C.CDLL(so)
-    for name in ENTRY:
-        res, args = _lib.EXPORTS[name]
-        getattr(lib, name).restype, getattr(lib, name).argtypes = res, args
-    return lib
-
-
-def use_host(monkeypatch, lib):
-    monkeypatch.setattr(_lib, "load", lambda: lib)
-    monkeypatch.setattr(_lib, "stream_ptr", lambda: None)
-    monkeypatch.setattr(_lib, "dptr", lambda t, dtype=torch.float32, allow_none=False:
-                        None if t is None else C.c_void_p(t.data_ptr()))
 
 
 @pytest.fixture(scope="module")
 def host_so(tmp_path_factory):
-    return build_host_transport(tmp_path_factory.mktemp("host_transport"))
+    return build_host_lib(tmp_path_factory.mktemp("host_transport"), "host_transport.cpp")
 
 
 @pytest.fixture

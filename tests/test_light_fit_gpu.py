@@ -15,8 +15,9 @@ import pytest
 import torch
 
 from gpu_helpers import load_fixture, model_from_fixture
+from helpers import build_host_lib, use_host
 from test_lighting_cpu import random_chunk
-from test_light_fit_cpu import build_host_transport, check_against_definition, transport64, use_host
+from test_light_fit_cpu import check_against_definition, transport64
 from test_material_edit_gpu import Replay
 
 pytestmark = pytest.mark.gpu
@@ -44,7 +45,7 @@ def test_kernels_match_host_build(fx, tmp_path, monkeypatch, stride, vis_kind):
     rescale = [1.2, 0.9, 1.05]
     pos, list_o, list_d = (t.cpu() for t in LF.transport_sample(dgrid, dch["rays"], dch["depth"], dch["normal"],
                                                                  dch["acc"], 0.5))
-    host = build_host_transport(tmp_path)
+    host = build_host_lib(tmp_path, "host_transport.cpp")
     use_host(monkeypatch, host)
     hpos, hlist_o, hlist_d = LF.transport_sample(grid, ch["rays"], ch["depth"], ch["normal"], ch["acc"], 0.5)
     monkeypatch.undo()

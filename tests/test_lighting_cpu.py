@@ -14,44 +14,24 @@ import numpy as np
 import pytest
 import torch
 
+from helpers import build_host_lib, use_host
 from tensoir_b200 import _lib, lighting
 from tensoir_b200.lighting import Light, Setup
 from tensoir_b200.relight_utils import GGX_specular, linear2srgb_torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(HERE)
-ENTRY = ("tir_lights_sample", "tir_lights_shade")
 EPS = float(np.finfo(np.float32).eps)
-
-
-def build_host_lights(path):
-    so = os.path.join(str(path), "libhost_lights.so")
-    subprocess.run(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", so,
-                    os.path.join(HERE, "host_lights.cpp")], check=True)
-    lib = C.CDLL(so)
-    for name in ENTRY:
-        res, args = _lib.EXPORTS[name]
-        getattr(lib, name).restype, getattr(lib, name).argtypes = res, args
-    return lib
 
 
 @pytest.fixture(scope="module")
 def host_so(tmp_path_factory):
-    return build_host_lights(tmp_path_factory.mktemp("host_lights"))
+    return build_host_lib(tmp_path_factory.mktemp("host_lights"), "host_lights.cpp")
 
 
 @pytest.fixture
 def host_lib(host_so, monkeypatch):
-    monkeypatch.setattr(_lib, "load", lambda: host_so)
-    monkeypatch.setattr(_lib, "stream_ptr", lambda: None)
-
-    def host_dptr(t, dtype=torch.float32, allow_none=False):
-        if t is None:
-            assert allow_none
-            return None
-        assert t.dtype == dtype and t.is_contiguous()
-        return C.c_void_p(t.data_ptr())
-    monkeypatch.setattr(_lib, "dptr", host_dptr)
+    use_host(monkeypatch, host_so)
     return host_so
 
 

@@ -16,7 +16,8 @@ import pytest
 import torch
 
 from gpu_helpers import load_fixture, model_from_fixture
-from test_lighting_cpu import MIXED, build_host_lights, check_against_float64, random_chunk, reference64, run_chunk
+from helpers import build_host_lib, use_host
+from test_lighting_cpu import MIXED, check_against_float64, random_chunk, reference64, run_chunk
 from test_material_edit_gpu import Replay
 
 pytestmark = pytest.mark.gpu
@@ -32,7 +33,7 @@ def fx():
 
 @pytest.mark.parametrize("stride,vis_kind", [(1, 0), (3, 1)])
 def test_kernels_match_host_build(fx, tmp_path, monkeypatch, stride, vis_kind):
-    from tensoir_b200 import _lib, lighting
+    from tensoir_b200 import lighting
     n = 6000
     ch = random_chunk(40 + stride, n, stride)
     u = torch.rand(n * lighting.slots_per_ray(MIXED), 2, dtype=torch.float64,
@@ -44,11 +45,7 @@ def test_kernels_match_host_build(fx, tmp_path, monkeypatch, stride, vis_kind):
     assert torch.equal(got["L"], again["L"].cpu()) and torch.equal(got["falloff"], again["falloff"].cpu())
     assert torch.equal(got["pos"] >= 0, again["pos"].cpu() >= 0)
 
-    host = build_host_lights(tmp_path)
-    monkeypatch.setattr(_lib, "load", lambda: host)
-    monkeypatch.setattr(_lib, "stream_ptr", lambda: None)
-    monkeypatch.setattr(_lib, "dptr", lambda t, dtype=torch.float32, allow_none=False:
-                        None if t is None else __import__("ctypes").c_void_p(t.data_ptr()))
+    use_host(monkeypatch, build_host_lib(tmp_path, "host_lights.cpp"))
     want = run_chunk(MIXED, ch, u, vis_kind, rescale, seed=3)
     assert torch.equal(got["L"], want["L"]) and torch.equal(got["falloff"], want["falloff"])
     joined = want["pos"] >= 0

@@ -14,41 +14,24 @@ import numpy as np
 import pytest
 import torch
 
-from helpers import oracle_field
+from helpers import build_host_lib, oracle_field, use_host
 from oracle import tensoir_oracle as O
 from tensoir_b200 import _lib, editing, relighting
 from tensoir_b200.editing import MaterialEdit
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(HERE)
-ENTRY = ("tir_material_edit", "tir_relight_sample", "tir_relight_shade", "tir_eval_pairs_work_size", "tir_eval_pairs")
 f32 = np.float32
 
 
 @pytest.fixture(scope="module")
 def host_so(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("host_edit") / "libhost_edit.so")
-    subprocess.run(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", so, os.path.join(HERE, "host_edit.cpp"),
-                    os.path.join(HERE, "host_relight.cpp")], check=True)
-    lib = C.CDLL(so)
-    for name in ENTRY:
-        res, args = _lib.EXPORTS[name]
-        getattr(lib, name).restype, getattr(lib, name).argtypes = res, args
-    return lib
+    return build_host_lib(tmp_path_factory.mktemp("host_edit"), "host_edit.cpp", "host_relight.cpp")
 
 
 @pytest.fixture
 def host_lib(host_so, monkeypatch):
-    monkeypatch.setattr(_lib, "load", lambda: host_so)
-    monkeypatch.setattr(_lib, "stream_ptr", lambda: None)
-
-    def host_dptr(t, dtype=torch.float32, allow_none=False):
-        if t is None:
-            assert allow_none
-            return None
-        assert t.dtype == dtype and t.is_contiguous()
-        return C.c_void_p(t.data_ptr())
-    monkeypatch.setattr(_lib, "dptr", host_dptr)
+    use_host(monkeypatch, host_so)
     return host_so
 
 

@@ -9,7 +9,6 @@ second (relight_edited shares one visibility pass between its variants by constr
 import ctypes as C
 import os
 import re
-import subprocess
 import types
 
 import cv2
@@ -18,7 +17,8 @@ import pytest
 import torch
 
 from gpu_helpers import load_fixture, model_from_fixture
-from test_material_edit_cpu import ENTRY, HERE, np_edit, random_rules
+from helpers import build_host_lib
+from test_material_edit_cpu import np_edit, random_rules
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -33,15 +33,7 @@ def fx():
 
 @pytest.fixture(scope="module")
 def host_so(tmp_path_factory):
-    from tensoir_b200 import _lib
-    so = str(tmp_path_factory.mktemp("host_edit") / "libhost_edit.so")
-    subprocess.run(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", so, os.path.join(HERE, "host_edit.cpp"),
-                    os.path.join(HERE, "host_relight.cpp")], check=True)
-    lib = C.CDLL(so)
-    for name in ENTRY:
-        res, args = _lib.EXPORTS[name]
-        getattr(lib, name).restype, getattr(lib, name).argtypes = res, args
-    return lib
+    return build_host_lib(tmp_path_factory.mktemp("host_edit"), "host_edit.cpp", "host_relight.cpp")
 
 
 def _host_edit(lib, rules, rays, depth, pts, albedo, rough, fresnel, acc, thr, scale):

@@ -12,8 +12,9 @@ import numpy as np
 import pytest
 import torch
 
-from mesh_helpers import (LEVEL, assert_closed, boundary_edges, build_host_lib, euler, host_marching_cubes,
-                          random_volume, saddle_volume, shared_volumes, signed_volume, sphere_volume, torus_volume)
+from helpers import build_host_lib
+from mesh_helpers import (LEVEL, assert_closed, boundary_edges, euler, host_marching_cubes, random_volume,
+                          saddle_volume, shared_volumes, signed_volume, sphere_volume, torus_volume)
 from oracle import mesh_oracle as MO
 from tensoir_b200 import mesh
 
@@ -23,7 +24,11 @@ HEADER = (b"ply\nformat binary_little_endian 1.0\nelement vertex {V}\nproperty f
 
 @pytest.fixture(scope="module")
 def lib(tmp_path_factory):
-    return build_host_lib(tmp_path_factory.mktemp("host_mesh"))
+    lib = build_host_lib(tmp_path_factory.mktemp("host_mesh"), "host_mesh.cpp")
+    lib.mc_host_cell.restype, lib.mc_host_cell.argtypes = C.c_int, [C.c_int32, C.c_int32, C.c_void_p]
+    lib.mc_host_face_connected.restype = C.c_int
+    lib.mc_host_face_connected.argtypes = [C.c_float] * 5
+    return lib
 
 
 def host_cell(lib, mask, connected):

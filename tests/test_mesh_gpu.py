@@ -10,8 +10,8 @@ import pytest
 import torch
 
 from gpu_helpers import load_fixture, load_shrunk_state, model_from_fixture
-from mesh_helpers import (LEVEL, assert_closed, build_host_lib, host_marching_cubes, shared_volumes, signed_volume,
-                          sphere_volume)
+from helpers import build_host_lib
+from mesh_helpers import LEVEL, assert_closed, host_marching_cubes, shared_volumes, signed_volume, sphere_volume
 from tensoir_b200 import mesh
 
 pytestmark = pytest.mark.gpu
@@ -20,7 +20,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 
 @pytest.fixture(scope="module")
 def lib(tmp_path_factory):
-    return build_host_lib(tmp_path_factory.mktemp("host_mesh"))
+    return build_host_lib(tmp_path_factory.mktemp("host_mesh"), "host_mesh.cpp")
 
 
 @pytest.fixture(scope="module")

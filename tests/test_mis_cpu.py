@@ -8,7 +8,6 @@ the estimator for unbiasedness against a float64 quadrature of the piecewise-con
 import ctypes as C
 import math
 import os
-import subprocess
 import sys
 from types import SimpleNamespace
 
@@ -17,28 +16,14 @@ import pytest
 import torch
 
 import test_indirect_cpu as H
+from helpers import build_host_lib, use_host
 from tensoir_b200 import _lib, mis, relighting
 from tensoir_b200.relight import Environment_Light
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(HERE)
 EPS = H.EPS
-ENTRY = ("tir_relight_sample", "tir_relight_shade", "tir_relight_mis_sample", "tir_relight_mis_shade")
 f32 = np.float32
-
-
-def build_host_mis(path):
-    so = os.path.join(str(path), "libhost_mis.so")
-    subprocess.run(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", so,
-                    os.path.join(HERE, "host_relight.cpp"), os.path.join(HERE, "host_mis.cpp")], check=True)
-    lib = C.CDLL(so)
-    for name in ENTRY:
-        res, args = _lib.EXPORTS[name]
-        getattr(lib, name).restype, getattr(lib, name).argtypes = res, args
-    lib.host_mis_texel.argtypes = [C.POINTER(_lib.TirEnvMap), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
-    lib.host_mis_pdf_brdf.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_int32,
-                                      C.c_void_p]
-    return lib
 
 
 def empty_march(model, rays_o, rays_d, *, table=None, counters=None, **kw):
@@ -49,12 +34,16 @@ def empty_march(model, rays_o, rays_d, *, table=None, counters=None, **kw):
 
 @pytest.fixture(scope="module")
 def host_so(tmp_path_factory):
-    return build_host_mis(tmp_path_factory.mktemp("host_mis"))
+    lib = build_host_lib(tmp_path_factory.mktemp("host_mis"), "host_relight.cpp", "host_mis.cpp")
+    lib.host_mis_texel.argtypes = [C.POINTER(_lib.TirEnvMap), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    lib.host_mis_pdf_brdf.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_int32,
+                                      C.c_void_p]
+    return lib
 
 
 @pytest.fixture
 def host_lib(host_so, monkeypatch):
-    H.use_host(monkeypatch, host_so, H.plane_march())
+    use_host(monkeypatch, host_so, H.plane_march())
     return host_so
 
 
@@ -370,7 +359,7 @@ def shade_ref(lib, env, names, k, ch, dirs, pos, vis, S_l, S_b, resc):
     flat = w.reshape(-1, 3).contiguous()
     bins = torch.empty(flat.shape[0], dtype=torch.int32)
     pl = torch.empty(flat.shape[0], dtype=torch.float64)
-    assert lib.host_mis_texel(relighting.env_group(envs, k), p(flat), flat.shape[0], p(bins), p(pl)) == 0
+    assert lib.host_mis_texel(relighting.env_group(envs, k), p(flat), C.c_int64(flat.shape[0]), p(bins), p(pl)) == 0
     pl = pl.reshape(n, -1)
     assert torch.allclose(pl, pdf_light64(env, name, bins.long()).reshape(n, -1), rtol=1e-9, atol=0)
     den = S_l * pl + (S_b * pdf_brdf64(ch["rays"], ch["normal"], ch["rough"], w) if S_b else 0)
@@ -450,7 +439,7 @@ def quadrature(ch, rgb, sub):
 
 @pytest.mark.parametrize("rough", [0.2, 0.5, 0.99])
 def test_estimator_is_unbiased(host_so, monkeypatch, rough):
-    H.use_host(monkeypatch, host_so, empty_march)
+    use_host(monkeypatch, host_so, empty_march)
     Hh, W = 8, 16
     view, normal = (0.5, -0.2, 0.8), (0.1, 0.05, 0.99)
     ch, maps = one_hit(1 << 16, view, normal, rough)
@@ -486,7 +475,7 @@ def test_mis_agrees_with_the_default_within_the_texel_bound(host_so, monkeypatch
     """A diffuse surface under a smooth 32x64 map: the MIS mean (continuous integral) and the default estimator's
     mean (texel centres, sin of the row centre) differ by at most the discretisation bound of DESIGN.md §3.7:
     sum_b E_b (dOmega_b osc_b(g) + |g(c_b)| |dOmega_b - dOmega'_b|), plus 5 standard errors."""
-    H.use_host(monkeypatch, host_so, empty_march)
+    use_host(monkeypatch, host_so, empty_march)
     Hh, W = 32, 64
     th = (torch.arange(Hh, dtype=torch.float64) + 0.5) / Hh * math.pi
     ph = (torch.arange(W, dtype=torch.float64) + 0.5) / W * 2 * math.pi

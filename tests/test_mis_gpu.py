@@ -14,6 +14,7 @@ import torch
 
 import test_indirect_cpu as H
 import test_mis_cpu as M
+from helpers import build_host_lib, use_host
 from tensoir_b200 import mis, relighting
 from tensoir_b200.relight import Environment_Light
 from tensoir_b200.synthetic import SyntheticViews, hemisphere_poses, make_lego_model
@@ -25,7 +26,7 @@ EPS = H.EPS
 
 @pytest.fixture(scope="module")
 def host_so(tmp_path_factory):
-    return M.build_host_mis(tmp_path_factory.mktemp("host_mis_gpu"))
+    return build_host_lib(tmp_path_factory.mktemp("host_mis_gpu"), "host_relight.cpp", "host_mis.cpp")
 
 
 @pytest.fixture(scope="module")
@@ -77,7 +78,7 @@ def test_kernels_match_host_build(lego, host_so, monkeypatch):
     assert torch.equal(lin, lin2)
     env_cpu = Environment_Light(hdr, device="cpu")
     with monkeypatch.context() as mp:
-        H.use_host(mp, host_so, H.plane_march())
+        use_host(mp, host_so, H.plane_march())
         _, _, hdirs, hpos, hvis = M.run_sample(env_cpu, names, ch, S_l, S_b, seed=5)
     dirs, pos, vis = dirs.cpu(), pos.cpu(), vis.cpu()
     # light directions: fp64 rounded once in both builds, to an ulp.  BRDF directions start from ggx_point's Np and V,
@@ -95,7 +96,7 @@ def test_kernels_match_host_build(lego, host_so, monkeypatch):
     lin = lin.cpu().double()
     hit = ch["acc"] > 0.5
     with monkeypatch.context() as mp:
-        H.use_host(mp, host_so, H.plane_march())
+        use_host(mp, host_so, H.plane_march())
         for k in range(3):
             want, bound = M.shade_ref(host_so, env_cpu, names, k, ch, dirs, pos, vis, S_l, S_b, resc)
             err = (lin[k] - want).abs()

@@ -58,7 +58,7 @@ import torch
 import torch.nn.functional as F
 
 from test_shade_kernels_fp64 import EPS, LO, PI, SENTINEL, SRGB_T, R, _d, check_fin, f32, ggx_ref, tone
-from test_relighting_cpu import host_lib, host_so  # noqa: F401  (fixtures: the host build of the relighting ABI)
+from helpers import build_host_lib, use_host
 from oracle import tensoir_oracle as O
 from tensoir_b200 import _lib, relighting
 from tensoir_b200.relight import Environment_Light
@@ -382,6 +382,17 @@ def test_reference_matches_oracle_cpu(golden_rotated):
         assert bool(((background_ref(e, d).v - want).abs() <= 1e-6 * (1 + want.abs())).all())
     finally:
         torch.set_default_dtype(old)
+
+
+@pytest.fixture(scope="module")
+def host_so(tmp_path_factory):
+    return build_host_lib(tmp_path_factory.mktemp("host_relight"), "host_relight.cpp")
+
+
+@pytest.fixture
+def host_lib(host_so, monkeypatch):
+    use_host(monkeypatch, host_so)
+    return host_so
 
 
 def host_case(maps_np, n, S, rough_stride, thr, vis_kind, seed, monkeypatch):

@@ -1,39 +1,23 @@
 """tensoir_b200/tail.py end to end on the CPU: the library handle is replaced by a host build of the SAME entry points
-(tests/host_tail.cpp: identical C-ABI signatures and per-item math, loops instead of kernels), so the real ctypes
-marshalling (argument order, TirRayMaps packing, NULL handling) and the autograd wrappers run and are compared with
-torch autograd of the expressions they replace."""
-import ctypes as C
-import os
-import subprocess
-
+(tests/host_tail.cpp: identical C-ABI signatures, argument checks and per-item math, loops instead of kernels), so the
+real ctypes marshalling (argument order, TirRayMaps packing, NULL handling) and the autograd wrappers run and are
+compared with torch autograd of the expressions they replace."""
 import pytest
 import torch
 
-from tensoir_b200 import _lib, tail
+from helpers import build_host_lib, use_host
+from tensoir_b200 import tail
 
-HERE = os.path.dirname(os.path.abspath(__file__))
+
+@pytest.fixture(scope="module")
+def host_so(tmp_path_factory):
+    return build_host_lib(tmp_path_factory.mktemp("host_tail"), "host_tail.cpp")
 
 
 @pytest.fixture
-def host_lib(tmp_path, monkeypatch):
-    so = str(tmp_path / "libhost_tail.so")
-    subprocess.run(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", "-o", so, os.path.join(HERE, "host_tail.cpp")],
-                   check=True)
-    lib = C.CDLL(so)
-    for name in ("tir_tail_fwd", "tir_tail_bwd", "tir_epilogue_fwd", "tir_epilogue_bwd"):
-        res, args = _lib.EXPORTS[name]
-        getattr(lib, name).restype, getattr(lib, name).argtypes = res, args
-    monkeypatch.setattr(_lib, "load", lambda: lib)
-    monkeypatch.setattr(_lib, "stream_ptr", lambda: None)
-
-    def host_dptr(t, dtype=torch.float32, allow_none=False):
-        if t is None:
-            assert allow_none
-            return None
-        assert t.dtype == dtype and t.is_contiguous()
-        return C.c_void_p(t.data_ptr())
-    monkeypatch.setattr(_lib, "dptr", host_dptr)
-    return lib
+def host_lib(host_so, monkeypatch):
+    use_host(monkeypatch, host_so)
+    return host_so
 
 
 def _rel(a, b):
@@ -116,3 +100,13 @@ def test_epilogue_wrapper(host_lib, bg, partial):
             assert torch.allclose(got, want.reshape(got.shape), rtol=2e-5, atol=2e-6)
     for got, want in zip(res[0][1], res[1][1]):
         assert torch.allclose(got, want, rtol=3e-4, atol=3e-5)
+
+
+def test_null_and_empty_arguments(host_so):
+    """The host build runs the library's own argument checks: NULL inputs fail with TIR_ERR_NULL, an empty batch is a
+    no-op (the codes test_abi_cpu.py asserts of the CUDA library)."""
+    for n, want in ((5, -1), (0, 0), (-1, 0)):
+        assert host_so.tir_tail_fwd(n, *[None] * 10) == want
+        assert host_so.tir_tail_bwd(n, *[None] * 16) == want
+        assert host_so.tir_epilogue_fwd(n, None, None, None, None, 0.04, 1, None, None, None, None) == want
+        assert host_so.tir_epilogue_bwd(n, None, None, None, None, 0.04, 1, *[None] * 7) == want
