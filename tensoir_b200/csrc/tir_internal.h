@@ -74,13 +74,23 @@ int launch_valid_samples(const TirField& f, const TirMarchCfg& cfg, const float*
                          float* out_z, float* out_dist, uint64_t* counters, int64_t capacity, cudaStream_t stream);
 int launch_density_bwd(const TirField& f, const float* xn, int64_t n, const int64_t* n_dev, const float* g_feature,
                        const GradPtrs& g, cudaStream_t stream);
-// g0 (+ g1 + g2 when not NULL): heads evaluated at the same points share one scatter
-int launch_app_products_bwd(const TirField& f, const float* xn, int64_t n, const int64_t* n_dev, const float* g0,
-                            const float* g1, const float* g2, const GradPtrs& g, cudaStream_t stream);
+// One scatter of an appearance-list point set into the VM-factor gradients: the appearance products' backward (g[0] +
+// g[1] + g[2] when not NULL: heads evaluated at the same points share one scatter) or, with density_grad, the
+// backward of the density feature and its spatial gradient (g[0] = d L / d feature, g[1] = d L / d (d f / d x_hat),
+// either NULL for zero).  The jobs of one launch write disjoint gradients.
+constexpr int kMaxAppScatterJobs = 3;
+struct AppScatterJob {
+  int density_grad;
+  const float* xn;
+  const float* g[3];
+  GradPtrs out;
+  int ctas;                   // set by launch_app_scatter
+};
+// all jobs over the same list length (n rows, min(*n_dev, n) when n_dev is given), CTAs split in proportion to work
+int launch_app_scatter(const TirField& f, AppScatterJob* jobs, int n_jobs, int64_t n, const int64_t* n_dev,
+                       cudaStream_t stream);
 int launch_density_grad(const TirField& f, const float* xn, int64_t n, const int64_t* n_dev, float* feature,
                         float* dfdx, cudaStream_t stream);
-int launch_density_grad_bwd(const TirField& f, const float* xn, int64_t n, const int64_t* n_dev, const float* g_feature,
-                            const float* g_dfdx, const GradPtrs& g, cudaStream_t stream);
 
 // real row count of a list: min(*n_dev, n) when a device count is given
 __device__ __forceinline__ int64_t list_rows(int64_t n, const int64_t* n_dev) {

@@ -571,30 +571,35 @@ extern "C" int tir_primary_backward(const TirField* field, const TirHeadJob* job
   sh.x0[0] = w->x0[0]; sh.x0[1] = w->x0[1]; sh.g_basis = gr->basis; sh.g_light = gr->light_line;
   rc = launch_heads_backward(*field, hb, n_jobs, sh, cap, n_app, stream);
   if (rc) return rc;
-  // 4. appearance scatters: one per point set, the heads of a set summed on load
+  // 4. appearance scatters, one per point set (the heads of a set summed on load), and 5. the derived normals' double
+  // backward of the density gather (tensorBase:846-853): one launch over the appearance list
   GradPtrs ga{}, gd{};
   for (int k = 0; k < 3; ++k) {
     ga.plane[k] = gr->aplane[k]; ga.line[k] = gr->aline[k];
     gd.plane[k] = gr->dplane[k]; gd.line[k] = gr->dline[k];
     if (!ga.plane[k] || !ga.line[k] || !gd.plane[k] || !gd.line[k]) return TIR_ERR_NULL;
   }
+  AppScatterJob sj[kMaxAppScatterJobs] = {};
+  int n_sj = 0;
   for (int ps = 0; ps < 2; ++ps) {
-    const float* g3[3] = {nullptr, nullptr, nullptr};
+    AppScatterJob& s = sj[n_sj];
     int m = 0;
     for (int j = 0; j < n_jobs; ++j)
       if (jobs[j].point_set == ps) {
         if (m >= 3) return TIR_ERR_CONFIG;
-        g3[m++] = b->gx0[j];
+        s.g[m++] = b->gx0[j];
       }
     if (m == 0) continue;
-    rc = launch_app_products_bwd(*field, ps == 0 ? w->a_xn : w->a_xj, cap, n_app, g3[0], g3[1], g3[2], ga, stream);
-    if (rc) return rc;
+    s.xn = ps == 0 ? w->a_xn : w->a_xj;
+    s.out = ga;
+    ++n_sj;
   }
-  // 5. derived normals: double backward of the density gather (tensorBase:846-853)
   if (normals_kind != TIR_NORMALS_PREDICTED) {
-    rc = launch_density_grad_bwd(*field, w->a_xn, cap, n_app, b->g_dn_feat, b->g_dn_dfdx, gd, stream);
-    if (rc) return rc;
+    AppScatterJob& s = sj[n_sj++];
+    s.density_grad = 1; s.xn = w->a_xn; s.g[0] = b->g_dn_feat; s.g[1] = b->g_dn_dfdx; s.out = gd;
   }
+  rc = launch_app_scatter(*field, sj, n_sj, cap, n_app, stream);
+  if (rc) return rc;
   // 6. compositing (+ feature2density), acc_map / depth_map gradients folded in
   primary_composite_bwd_kernel<<<(unsigned)((n_rays * 32 + 255) / 256), 256, 0, stream>>>(
       *field, w->v_feat, w->v_sigma, w->v_dist, w->v_z, w->offsets, n_rays, field->distance_scale, w->cap_valid,
@@ -697,7 +702,9 @@ extern "C" int tir_primary_radiance_backward(const TirField* field, const TirHea
   rc = launch_heads_backward(*field, &h, 1, sh, cap, n_app, stream);
   if (rc) return rc;
   // 3. appearance scatter (point set 0 only)
-  rc = launch_app_products_bwd(*field, w->a_xn, cap, n_app, b->gx0[0], nullptr, nullptr, ga, stream);
+  AppScatterJob sj{};
+  sj.xn = w->a_xn; sj.g[0] = b->gx0[0]; sj.out = ga;
+  rc = launch_app_scatter(*field, &sj, 1, cap, n_app, stream);
   if (rc) return rc;
   // 4. compositing (+ feature2density) with the acc / depth gradients, 5. density scatter
   primary_composite_bwd_kernel<<<(unsigned)((n_rays * 32 + 255) / 256), 256, 0, stream>>>(

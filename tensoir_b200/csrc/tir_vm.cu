@@ -2,7 +2,8 @@
 //   * tir_vm_app_products         plane*line products of the appearance tensors   (tensoRF_rotated_lights.py:141-153)
 //   * tir_vm_density_grad         density feature + analytic d f / d x_hat with the clamped-index sampler
 //                                 (compute_densityfeature_with_xyz_grad tensoRF:113-129 + relight_utils.py:57-107)
-//   * backward scatters of the three gathers into channel-last gradient shadows (float4 atomics, sm_90+)
+//   * backward scatters of the three gathers into channel-last gradient shadows (float4 atomics, sm_90+, summed over
+//     runs of rows that hit the same texel first)
 //   * ray-sorted valid-sample lists (count / fill) and the sequential compositing scan with its backward
 //     (raw2alpha, tensorBase:21-28)
 #include "tir_device.cuh"
@@ -96,78 +97,6 @@ __global__ void app_products_kernel(TirField f, const float* __restrict__ xn, in
   }
 }
 
-// One thread per (point, orientation, 4-channel chunk): the appearance list is short (~15 k points per step), so the work
-// is spread over C/4 = 12x more threads than a per-(point, orientation) loop, and consecutive threads hit consecutive
-// 16-byte chunks of the same texel (coalesced loads and atomics).
-template <int C>
-__global__ void app_products_bwd_kernel(TirField f, const float* __restrict__ xn, int64_t n_cap,
-                                        const int64_t* __restrict__ n_dev, const float* __restrict__ gout,
-                                        const float* __restrict__ gout1, const float* __restrict__ gout2, GradPtrs g) {
-  constexpr int Q = C / 4;
-  const int64_t n = list_rows(n_cap, n_dev);
-  const int64_t total = n * 3 * Q;
-  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t pk = t / Q;
-    const int c = (int)(t - pk * Q) * 4;
-    const int64_t i = pk / 3;
-    const int k = (int)(pk - i * 3);
-    const float x[3] = {xn[i * 3], xn[i * 3 + 1], xn[i * 3 + 2]};
-    const int m0 = kMat0[k], m1 = kMat1[k], v = kVec[k];
-    const Bilinear b = bilinear_setup(x[m0], x[m1], f.grid[m0], f.grid[m1]);
-    const Linear1 l = linear_setup(x[v], f.grid[v]);
-    const float* P = f.aplane[k];
-    const float* L = f.aline[k];
-    const int64_t go_off = i * (3 * C) + k * C + c;
-    float4 gv = *reinterpret_cast<const float4*>(gout + go_off);
-    if (gout1) gv = f4_add(gv, *reinterpret_cast<const float4*>(gout1 + go_off));   // heads sharing the points
-    if (gout2) gv = f4_add(gv, *reinterpret_cast<const float4*>(gout2 + go_off));
-    const float4 pv = bilerp4(ldg4(P + (size_t)b.o00 * C + c), ldg4(P + (size_t)b.o01 * C + c),
-                              ldg4(P + (size_t)b.o10 * C + c), ldg4(P + (size_t)b.o11 * C + c), b);
-    const float4 lv = lerp4(ldg4(L + (size_t)l.o0 * C + c), ldg4(L + (size_t)l.o1 * C + c), l);
-    const float4 gp = f4_mul(gv, lv);   // d/d plane value
-    const float4 gl = f4_mul(gv, pv);   // d/d line value
-    if (b.nw != 0.f) red4(g.plane[k] + (size_t)b.o00 * C + c, f4_scale(gp, b.nw));
-    if (b.ne != 0.f) red4(g.plane[k] + (size_t)b.o01 * C + c, f4_scale(gp, b.ne));
-    if (b.sw != 0.f) red4(g.plane[k] + (size_t)b.o10 * C + c, f4_scale(gp, b.sw));
-    if (b.se != 0.f) red4(g.plane[k] + (size_t)b.o11 * C + c, f4_scale(gp, b.se));
-    if (l.w0 != 0.f) red4(g.line[k] + (size_t)l.o0 * C + c, f4_scale(gl, l.w0));
-    if (l.w1 != 0.f) red4(g.line[k] + (size_t)l.o1 * C + c, f4_scale(gl, l.w1));
-  }
-}
-
-// density feature backward (zero-padding sampler): d L / d feature[i] = gout[i]
-template <int C>
-__global__ void density_bwd_kernel(TirField f, const float* __restrict__ xn, int64_t n_cap,
-                                   const int64_t* __restrict__ n_dev, const float* __restrict__ gout, GradPtrs g) {
-  const int64_t total = list_rows(n_cap, n_dev) * 3;
-  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t i = t / 3;
-    const int k = (int)(t - i * 3);
-    const float gi = gout[i];
-    if (gi == 0.f) continue;
-    const float x[3] = {xn[i * 3], xn[i * 3 + 1], xn[i * 3 + 2]};
-    const int m0 = kMat0[k], m1 = kMat1[k], v = kVec[k];
-    const Bilinear b = bilinear_setup(x[m0], x[m1], f.grid[m0], f.grid[m1]);
-    const Linear1 l = linear_setup(x[v], f.grid[v]);
-    const float* P = f.dplane[k];
-    const float* L = f.dline[k];
-#pragma unroll
-    for (int c = 0; c < C; c += 4) {
-      const float4 pv = bilerp4(ldg4(P + (size_t)b.o00 * C + c), ldg4(P + (size_t)b.o01 * C + c),
-                                ldg4(P + (size_t)b.o10 * C + c), ldg4(P + (size_t)b.o11 * C + c), b);
-      const float4 lv = lerp4(ldg4(L + (size_t)l.o0 * C + c), ldg4(L + (size_t)l.o1 * C + c), l);
-      const float4 gp = f4_scale(lv, gi);
-      const float4 gl = f4_scale(pv, gi);
-      if (b.nw != 0.f) red4(g.plane[k] + (size_t)b.o00 * C + c, f4_scale(gp, b.nw));
-      if (b.ne != 0.f) red4(g.plane[k] + (size_t)b.o01 * C + c, f4_scale(gp, b.ne));
-      if (b.sw != 0.f) red4(g.plane[k] + (size_t)b.o10 * C + c, f4_scale(gp, b.sw));
-      if (b.se != 0.f) red4(g.plane[k] + (size_t)b.o11 * C + c, f4_scale(gp, b.se));
-      if (l.w0 != 0.f) red4(g.line[k] + (size_t)l.o0 * C + c, f4_scale(gl, l.w0));
-      if (l.w1 != 0.f) red4(g.line[k] + (size_t)l.o1 * C + c, f4_scale(gl, l.w1));
-    }
-  }
-}
-
 // ------------------------------------------------------------------------------------------------------------------
 // density feature + spatial gradient (clamped sampler), forward / backward
 // ------------------------------------------------------------------------------------------------------------------
@@ -213,23 +142,116 @@ __global__ void density_grad_kernel(TirField f, const float* __restrict__ xn, in
   }
 }
 
-// one thread per (point, orientation, 4-channel chunk), like app_products_bwd_kernel
-template <int C>
-__global__ void density_grad_bwd_kernel(TirField f, const float* __restrict__ xn, int64_t n_cap,
-                                        const int64_t* __restrict__ n_dev, const float* __restrict__ g_feat,
-                                        const float* __restrict__ g_dfdx, GradPtrs g) {
-  constexpr int Q = C / 4;
-  const int64_t total = list_rows(n_cap, n_dev) * 3 * Q;
-  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t pk = t / Q;
-    const int c = (int)(t - pk * Q) * 4;
-    const int64_t i = pk / 3;
-    const int k = (int)(pk - i * 3);
-    const float x[3] = {xn[i * 3], xn[i * 3 + 1], xn[i * 3 + 2]};
+// ------------------------------------------------------------------------------------------------------------------
+// gradient scatters of the three gathers: float4 atomics into channel-last gradient shadows, summed per run first
+// ------------------------------------------------------------------------------------------------------------------
+// A group of C/4 consecutive threads (one 4-channel chunk each, so a group covers whole texels and a warp's atomics fill
+// whole 32-byte sectors) walks kScatterRows consecutive rows of a list for one orientation.  The valid and appearance
+// lists are sorted by ray and a ray's samples are half a voxel apart, so consecutive rows often hit the same tap texel:
+// each of the 6 taps keeps its open run (texel, sum so far) in registers and issues one atomic when its texel changes
+// or the block ends.  The merge compares texels, not rays, so it is exact for any row order (an unsorted list only
+// merges less), and a run adds as many terms into an entry as its rows would one by one.
+constexpr int kScatterRows = 8;
+
+struct TapRun {
+  int key;       // texel of the open run, -1: none
+  float4 acc;
+};
+
+// what one row adds to its 4 plane taps and 2 line taps; key -1: nothing (zero tap weight)
+struct RowTaps {
+  int key[6];
+  float4 v[6];
+};
+
+__device__ __forceinline__ void run_add(TapRun& r, float* g, int C, int key, float4 v) {
+  if (key < 0) return;
+  if (key == r.key) {
+    r.acc = f4_add(r.acc, v);
+    return;
+  }
+  if (r.key >= 0) red4(g + (size_t)r.key * C, r.acc);
+  r.key = key;
+  r.acc = v;
+}
+
+// zero-padding sampler: taps with a zero weight add nothing
+__device__ __forceinline__ void zero_padded_taps(const Bilinear& b, const Linear1& l, float4 gp, float4 gl, RowTaps& r) {
+  r.key[0] = b.nw != 0.f ? b.o00 : -1; r.v[0] = f4_scale(gp, b.nw);
+  r.key[1] = b.ne != 0.f ? b.o01 : -1; r.v[1] = f4_scale(gp, b.ne);
+  r.key[2] = b.sw != 0.f ? b.o10 : -1; r.v[2] = f4_scale(gp, b.sw);
+  r.key[3] = b.se != 0.f ? b.o11 : -1; r.v[3] = f4_scale(gp, b.se);
+  r.key[4] = l.w0 != 0.f ? l.o0 : -1; r.v[4] = f4_scale(gl, l.w0);
+  r.key[5] = l.w1 != 0.f ? l.o1 : -1; r.v[5] = f4_scale(gl, l.w1);
+}
+
+// coordinates of a point on plane k's two axes and line k's axis (kMat0 / kMat1 / kVec without an indexed local array)
+struct Orient {
+  float a, b, v;
+};
+__device__ __forceinline__ Orient orient(const float* xn, int64_t i, int k) {
+  const float x0 = xn[i * 3], x1 = xn[i * 3 + 1], x2 = xn[i * 3 + 2];
+  return Orient{k == 2 ? x1 : x0, k == 0 ? x1 : x2, k == 0 ? x2 : (k == 1 ? x1 : x0)};
+}
+
+// density feature backward (zero-padding sampler): d L / d feature[i] = g[i]; rows with g[i] == 0 are skipped
+struct DensityRows {
+  static constexpr int C = 16;
+  const float* xn;
+  const float* g;
+  __device__ __forceinline__ bool row(const TirField& f, int64_t i, int k, int c, RowTaps& r) const {
+    const float gi = g[i];
+    if (gi == 0.f) return false;
+    const Orient x = orient(xn, i, k);
+    const Bilinear b = bilinear_setup(x.a, x.b, f.grid[kMat0[k]], f.grid[kMat1[k]]);
+    const Linear1 l = linear_setup(x.v, f.grid[kVec[k]]);
+    const float* P = f.dplane[k];
+    const float* L = f.dline[k];
+    const float4 pv = bilerp4(ldg4(P + (size_t)b.o00 * C + c), ldg4(P + (size_t)b.o01 * C + c),
+                              ldg4(P + (size_t)b.o10 * C + c), ldg4(P + (size_t)b.o11 * C + c), b);
+    const float4 lv = lerp4(ldg4(L + (size_t)l.o0 * C + c), ldg4(L + (size_t)l.o1 * C + c), l);
+    zero_padded_taps(b, l, f4_scale(lv, gi), f4_scale(pv, gi), r);
+    return true;
+  }
+};
+
+// appearance products backward (zero-padding sampler): d L / d product = g0 (+ g1 + g2, heads sharing the points)
+struct AppRows {
+  static constexpr int C = 48;
+  const float* xn;
+  const float* g0;
+  const float* g1;
+  const float* g2;
+  __device__ __forceinline__ bool row(const TirField& f, int64_t i, int k, int c, RowTaps& r) const {
+    const Orient x = orient(xn, i, k);
+    const Bilinear b = bilinear_setup(x.a, x.b, f.grid[kMat0[k]], f.grid[kMat1[k]]);
+    const Linear1 l = linear_setup(x.v, f.grid[kVec[k]]);
+    const float* P = f.aplane[k];
+    const float* L = f.aline[k];
+    const int64_t go_off = i * (3 * C) + k * C + c;
+    float4 gv = *reinterpret_cast<const float4*>(g0 + go_off);
+    if (g1) gv = f4_add(gv, *reinterpret_cast<const float4*>(g1 + go_off));
+    if (g2) gv = f4_add(gv, *reinterpret_cast<const float4*>(g2 + go_off));
+    const float4 pv = bilerp4(ldg4(P + (size_t)b.o00 * C + c), ldg4(P + (size_t)b.o01 * C + c),
+                              ldg4(P + (size_t)b.o10 * C + c), ldg4(P + (size_t)b.o11 * C + c), b);
+    const float4 lv = lerp4(ldg4(L + (size_t)l.o0 * C + c), ldg4(L + (size_t)l.o1 * C + c), l);
+    zero_padded_taps(b, l, f4_mul(gv, lv), f4_mul(gv, pv), r);   // d/d plane value, d/d line value
+    return true;
+  }
+};
+
+// backward of density_grad_kernel (clamped sampler) from g_feat and / or g_dfdx (NULL: zero); every tap adds
+struct DensityGradRows {
+  static constexpr int C = 16;
+  const float* xn;
+  const float* g_feat;
+  const float* g_dfdx;
+  __device__ __forceinline__ bool row(const TirField& f, int64_t i, int k, int c, RowTaps& r) const {
+    const Orient x = orient(xn, i, k);
     const int m0 = kMat0[k], m1 = kMat1[k], v = kVec[k];
     const int W = f.grid[m0], H = f.grid[m1], D = f.grid[v];
-    const BilinearD b = bilinear_clamped(x[m0], x[m1], W, H);
-    const LinearD l = linear_clamped(x[v], D);
+    const BilinearD b = bilinear_clamped(x.a, x.b, W, H);
+    const LinearD l = linear_clamped(x.v, D);
     const float sx = 0.5f * (W - 1), sy = 0.5f * (H - 1), sl = 0.5f * (D - 1);
     const float gf = g_feat ? g_feat[i] : 0.f;
     const float g0 = g_dfdx ? g_dfdx[i * 3 + m0] * sx : 0.f;
@@ -248,15 +270,75 @@ __global__ void density_grad_bwd_kernel(TirField f, const float* __restrict__ xn
     const float4 py = f4_comb4(a, bb, cc, d, b.dy_nw, b.dy_ne, b.dy_sw, b.dy_se);
     const float4 lv = f4_add(f4_scale(l0, l.w0), f4_scale(l1, l.w1));
     const float4 dl = f4_sub(l1, l0);
-    red4(g.plane[k] + (size_t)b.o00 * C + c, f4_add(f4_scale(lv, a_nw), f4_scale(dl, gv * b.nw)));
-    red4(g.plane[k] + (size_t)b.o01 * C + c, f4_add(f4_scale(lv, a_ne), f4_scale(dl, gv * b.ne)));
-    red4(g.plane[k] + (size_t)b.o10 * C + c, f4_add(f4_scale(lv, a_sw), f4_scale(dl, gv * b.sw)));
-    red4(g.plane[k] + (size_t)b.o11 * C + c, f4_add(f4_scale(lv, a_se), f4_scale(dl, gv * b.se)));
+    r.key[0] = b.o00; r.v[0] = f4_add(f4_scale(lv, a_nw), f4_scale(dl, gv * b.nw));
+    r.key[1] = b.o01; r.v[1] = f4_add(f4_scale(lv, a_ne), f4_scale(dl, gv * b.ne));
+    r.key[2] = b.o10; r.v[2] = f4_add(f4_scale(lv, a_sw), f4_scale(dl, gv * b.sw));
+    r.key[3] = b.o11; r.v[3] = f4_add(f4_scale(lv, a_se), f4_scale(dl, gv * b.se));
     // coefficient of L_u: pv*(gf*wl_u -/+ gv) + wl_u*(g0*px + g1*py)
     const float4 q = f4_add(f4_scale(px, g0), f4_scale(py, g1));
-    red4(g.line[k] + (size_t)l.o0 * C + c, f4_add(f4_scale(pv, gf * l.w0 - gv), f4_scale(q, l.w0)));
-    red4(g.line[k] + (size_t)l.o1 * C + c, f4_add(f4_scale(pv, gf * l.w1 + gv), f4_scale(q, l.w1)));
+    r.key[4] = l.o0; r.v[4] = f4_add(f4_scale(pv, gf * l.w0 - gv), f4_scale(q, l.w0));
+    r.key[5] = l.o1; r.v[5] = f4_add(f4_scale(pv, gf * l.w1 + gv), f4_scale(q, l.w1));
+    return true;
   }
+};
+
+// threads of a scatter over n rows: one group of C/4 per (orientation, block of kScatterRows rows)
+inline int64_t scatter_threads(int64_t n, int C) { return 3 * ((n + kScatterRows - 1) / kScatterRows) * (C / 4); }
+
+// grid-stride over the (orientation, row block, chunk) threads t0, t0 + stride, ... of a list of n rows
+template <class Rows>
+__device__ __forceinline__ void scatter_rows(const TirField& f, const Rows& rows, const GradPtrs& g, int64_t n,
+                                             int64_t t0, int64_t stride) {
+  constexpr int C = Rows::C, Q = C / 4;
+  const int64_t blocks = (n + kScatterRows - 1) / kScatterRows;
+  const int64_t total = blocks * 3 * Q;
+  for (int64_t t = t0; t < total; t += stride) {
+    const int64_t grp = t / Q;
+    const int c = (int)(t - grp * Q) * 4;
+    const int k = (int)(grp / blocks);
+    const int64_t i0 = (grp - k * blocks) * kScatterRows;
+    const int64_t i1 = i0 + kScatterRows < n ? i0 + kScatterRows : n;
+    float* gp = (k == 0 ? g.plane[0] : k == 1 ? g.plane[1] : g.plane[2]) + c;   // no indexed copy of g
+    float* gl = (k == 0 ? g.line[0] : k == 1 ? g.line[1] : g.line[2]) + c;
+    TapRun run[6];
+#pragma unroll
+    for (int u = 0; u < 6; ++u) run[u] = TapRun{-1, make_float4(0.f, 0.f, 0.f, 0.f)};
+    for (int64_t i = i0; i < i1; ++i) {
+      RowTaps r;
+      if (!rows.row(f, i, k, c, r)) continue;
+#pragma unroll
+      for (int u = 0; u < 6; ++u) run_add(run[u], u < 4 ? gp : gl, C, r.key[u], r.v[u]);
+    }
+#pragma unroll
+    for (int u = 0; u < 6; ++u)
+      if (run[u].key >= 0) red4((u < 4 ? gp : gl) + (size_t)run[u].key * C, run[u].acc);
+  }
+}
+
+__global__ void __launch_bounds__(128, 4) density_bwd_kernel(TirField f, DensityRows rows, int64_t n_cap,
+                                                          const int64_t* __restrict__ n_dev, GradPtrs g) {
+  scatter_rows(f, rows, g, list_rows(n_cap, n_dev), blockIdx.x * (int64_t)blockDim.x + threadIdx.x,
+               (int64_t)gridDim.x * blockDim.x);
+}
+
+// the scatters of one appearance list (AppScatterJob) in one launch: job j runs on its own range of job[j].ctas CTAs
+struct AppScatterLaunch {
+  AppScatterJob job[kMaxAppScatterJobs];
+  int n_jobs;
+  int64_t n_cap;
+  const int64_t* n_dev;
+};
+
+__global__ void __launch_bounds__(128, 4) app_scatter_kernel(TirField f, AppScatterLaunch p) {
+  int b = blockIdx.x, j = 0;
+  while (j + 1 < p.n_jobs && b >= p.job[j].ctas) b -= p.job[j].ctas, ++j;
+  const AppScatterJob& J = p.job[j];
+  const int64_t n = list_rows(p.n_cap, p.n_dev);
+  const int64_t t0 = b * (int64_t)blockDim.x + threadIdx.x, stride = (int64_t)J.ctas * blockDim.x;
+  if (J.density_grad)
+    scatter_rows(f, DensityGradRows{J.xn, J.g[0], J.g[1]}, J.out, n, t0, stride);
+  else
+    scatter_rows(f, AppRows{J.xn, J.g[0], J.g[1], J.g[2]}, J.out, n, t0, stride);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -409,14 +491,31 @@ int launch_density_bwd(const TirField& f, const float* xn, int64_t n, const int6
                        const GradPtrs& g, cudaStream_t stream) {
   if (n <= 0) return TIR_OK;
   if (f.dC != 16) return TIR_ERR_SHAPE;
-  density_bwd_kernel<16><<<blocks_for(n * 3, 128), 128, 0, stream>>>(f, xn, n, n_dev, g_feature, g);
+  density_bwd_kernel<<<blocks_for(scatter_threads(n, 16), 128), 128, 0, stream>>>(f, DensityRows{xn, g_feature}, n,
+                                                                                  n_dev, g);
   return (int)cudaGetLastError();
 }
-int launch_app_products_bwd(const TirField& f, const float* xn, int64_t n, const int64_t* n_dev, const float* g0,
-                            const float* g1, const float* g2, const GradPtrs& g, cudaStream_t stream) {
-  if (n <= 0) return TIR_OK;
-  if (f.aC != 48) return TIR_ERR_SHAPE;
-  app_products_bwd_kernel<48><<<blocks_for(n * 3 * 12, 128), 128, 0, stream>>>(f, xn, n, n_dev, g0, g1, g2, g);
+int launch_app_scatter(const TirField& f, AppScatterJob* jobs, int n_jobs, int64_t n, const int64_t* n_dev,
+                       cudaStream_t stream) {
+  if (n <= 0 || n_jobs <= 0) return TIR_OK;
+  if (n_jobs > kMaxAppScatterJobs) return TIR_ERR_CONFIG;
+  AppScatterLaunch p{};
+  int64_t threads[kMaxAppScatterJobs], sum = 0;
+  for (int j = 0; j < n_jobs; ++j) {
+    if (jobs[j].density_grad ? f.dC != 16 : f.aC != 48) return TIR_ERR_SHAPE;
+    threads[j] = scatter_threads(n, jobs[j].density_grad ? 16 : 48);
+    sum += threads[j];
+  }
+  const int total = blocks_for(sum, 128);
+  int ctas = 0;
+  for (int j = 0; j < n_jobs; ++j) {
+    jobs[j].ctas = (int)((double)total * threads[j] / sum + 0.5);
+    if (jobs[j].ctas < 1) jobs[j].ctas = 1;
+    p.job[j] = jobs[j];
+    ctas += jobs[j].ctas;
+  }
+  p.n_jobs = n_jobs; p.n_cap = n; p.n_dev = n_dev;
+  app_scatter_kernel<<<ctas, 128, 0, stream>>>(f, p);
   return (int)cudaGetLastError();
 }
 int launch_density_grad(const TirField& f, const float* xn, int64_t n, const int64_t* n_dev, float* feature,
@@ -424,13 +523,6 @@ int launch_density_grad(const TirField& f, const float* xn, int64_t n, const int
   if (n <= 0) return TIR_OK;
   if (f.dC != 16) return TIR_ERR_SHAPE;
   density_grad_kernel<16><<<blocks_for(n, 128), 128, 0, stream>>>(f, xn, n, n_dev, feature, dfdx);
-  return (int)cudaGetLastError();
-}
-int launch_density_grad_bwd(const TirField& f, const float* xn, int64_t n, const int64_t* n_dev, const float* g_feature,
-                            const float* g_dfdx, const GradPtrs& g, cudaStream_t stream) {
-  if (n <= 0) return TIR_OK;
-  if (f.dC != 16) return TIR_ERR_SHAPE;
-  density_grad_bwd_kernel<16><<<blocks_for(n * 3 * 4, 128), 128, 0, stream>>>(f, xn, n, n_dev, g_feature, g_dfdx, g);
   return (int)cudaGetLastError();
 }
 }  // namespace tir
@@ -448,11 +540,10 @@ extern "C" int tir_vm_app_products_bwd(const TirField* field, const float* xn, i
   if (n <= 0) return TIR_OK;   // empty input: nothing to do (pointers of empty tensors are NULL)
   if (!field || !xn || !g_out || !g_plane || !g_line) return TIR_ERR_NULL;
   if (field->aC != 48) return TIR_ERR_SHAPE;
-  GradPtrs g;
-  for (int k = 0; k < 3; ++k) { g.plane[k] = g_plane[k]; g.line[k] = g_line[k]; }
-  app_products_bwd_kernel<48><<<blocks_for(n * 3 * 12, 128), 128, 0, (cudaStream_t)stream>>>(*field, xn, n, nullptr, g_out,
-                                                                                       nullptr, nullptr, g);
-  return (int)cudaGetLastError();
+  AppScatterJob j{};
+  j.xn = xn; j.g[0] = g_out;
+  for (int k = 0; k < 3; ++k) { j.out.plane[k] = g_plane[k]; j.out.line[k] = g_line[k]; }
+  return launch_app_scatter(*field, &j, 1, n, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int tir_vm_density_bwd(const TirField* field, const float* xn, int64_t n, const float* g_feature,
@@ -462,8 +553,7 @@ extern "C" int tir_vm_density_bwd(const TirField* field, const float* xn, int64_
   if (field->dC != 16) return TIR_ERR_SHAPE;
   GradPtrs g;
   for (int k = 0; k < 3; ++k) { g.plane[k] = g_plane[k]; g.line[k] = g_line[k]; }
-  density_bwd_kernel<16><<<blocks_for(n * 3, 128), 128, 0, (cudaStream_t)stream>>>(*field, xn, n, nullptr, g_feature, g);
-  return (int)cudaGetLastError();
+  return launch_density_bwd(*field, xn, n, nullptr, g_feature, g, (cudaStream_t)stream);
 }
 
 extern "C" int tir_vm_density_grad(const TirField* field, const float* xn, int64_t n, float* feature, float* dfdx,
@@ -481,11 +571,10 @@ extern "C" int tir_vm_density_grad_bwd(const TirField* field, const float* xn, i
   if (n <= 0) return TIR_OK;   // empty input: nothing to do (pointers of empty tensors are NULL)
   if (!field || !xn || !g_plane || !g_line) return TIR_ERR_NULL;
   if (field->dC != 16) return TIR_ERR_SHAPE;
-  GradPtrs g;
-  for (int k = 0; k < 3; ++k) { g.plane[k] = g_plane[k]; g.line[k] = g_line[k]; }
-  density_grad_bwd_kernel<16><<<blocks_for(n * 3 * 4, 128), 128, 0, (cudaStream_t)stream>>>(*field, xn, n, nullptr,
-                                                                                       g_feature, g_dfdx, g);
-  return (int)cudaGetLastError();
+  AppScatterJob j{};
+  j.density_grad = 1; j.xn = xn; j.g[0] = g_feature; j.g[1] = g_dfdx;
+  for (int k = 0; k < 3; ++k) { j.out.plane[k] = g_plane[k]; j.out.line[k] = g_line[k]; }
+  return launch_app_scatter(*field, &j, 1, n, nullptr, (cudaStream_t)stream);
 }
 
 extern "C" int tir_valid_samples_count(const TirField* field, const float* rays_o, const float* rays_d,
