@@ -45,6 +45,13 @@ an exact fp32 input (the ReLU of dn_feat, the softplus branch of v_feat) has no 
 within 4 eps32 (G - 1) of a texel index take a one-sided d feature / d x_hat (test_vm_kernels_fp64); they are counted,
 and their dfdx is not compared.
 
+``launch`` drives the entry points and returns a Dump; ``check_stages`` checks a Dump, whichever launch or training
+step left it (tests/test_train_step_primary_fp64.py passes it the dumps and captured upstream gradients of real steps).
+The radiance-only entry points tir_primary_radiance / _backward have the same pair (``launch_radiance``,
+``check_radiance_stages``): march, compositing and the appearance list as above, the head through
+test_heads_kernels_fp64, radiance_ray_fwd_kernel's rgb_map / depth_map and radiance_ray_bwd_kernel's g_out, g_weight
+(through a_src), g_acc and g_depth in R arithmetic, then the compositing backward and the density scatter.
+
 ``test_tail_and_epilogue_backward_match_autograd_cpu`` pins the hand-written tail and epilogue backward to float64
 autograd of their forward, away from kinks, to 1e-10, and ``test_chained_references_reproduce_the_oracle_cpu`` pins
 the chained references to the oracle's relight-phase maps, losses and parameter gradients."""
@@ -69,6 +76,7 @@ DS_A, DS_E = float(torch.tensor(1.055) / torch.tensor(2.4)), float(torch.tensor(
 C09, C009 = f32(0.9), f32(0.09)
 F0_FP32 = True                 # fixed_fresnel as the kernel gets it (a float argument)
 STATS = {}
+MAP_NAMES = ("rgb", "depth", "normal", "albedo", "rough", "fresnel", "nd", "no")
 
 
 # ------------------------------------------------------------------------------------------------------------------
@@ -350,6 +358,40 @@ def epilogue_backward(P, acc, dz, f0, bg, g, g_ac, g_rc, gates):
 
 
 # ------------------------------------------------------------------------------------------------------------------
+# the radiance-only tail (radiance_ray_fwd_kernel / radiance_ray_bwd_kernel) in float64 with error bounds
+# ------------------------------------------------------------------------------------------------------------------
+def radiance_forward(w, out, ray, acc, depth, dz, bg):
+    """rgb_map [R n,3] = sum over the ray's rows of w out (+ 1 - acc) and depth_map [R n] = depth (+ (1 - acc) dz):
+    w [m], out [m,3] the rows, ray [m] their ray; acc, depth, dz [n] exact.  The sequential sum carries (count) eps32 of
+    sum|w out| besides its terms' own errors."""
+    n = acc.shape[0]
+    wo = R(w[:, None]) * R(out)
+    cnt = torch.bincount(ray, minlength=n).to(acc.dtype)[:, None]
+    sv = torch.zeros(n, 3, dtype=acc.dtype, device=acc.device).index_add(0, ray, wo.v)
+    se = torch.zeros_like(sv).index_add(0, ray, wo.e) + EPS32 * cnt * torch.zeros_like(sv).index_add(
+        0, ray, _d(wo.v).abs())
+    rgb, dm = R(sv, se), rc(depth)
+    if bg:
+        om = 1.0 - rc(acc)
+        rgb = rgb + R(om.v[:, None], om.e[:, None])
+        dm = dm + om * rc(dz)
+    return rgb, dm
+
+
+def radiance_backward(w, out, ray, dz, g, gd, bg):
+    """-> (g_out [R m,3], g_weight [R m], g_acc [R n], g_depth [R n]) of radiance_forward for the map gradients g [n,3]
+    and gd [n]"""
+    gr = g[ray]
+    g_out = R(w[:, None]) * rc(gr)
+    g_w = rc(out[:, 0]) * rc(gr[:, 0]) + rc(out[:, 1]) * rc(gr[:, 1]) + rc(out[:, 2]) * rc(gr[:, 2])
+    if bg:
+        g_acc = -(rc(g[:, 0]) + rc(g[:, 1]) + rc(g[:, 2])) - rc(gd) * rc(dz)
+    else:
+        g_acc = rc(torch.zeros_like(gd))
+    return g_out, g_w, g_acc, rc(gd)
+
+
+# ------------------------------------------------------------------------------------------------------------------
 # CPU: the hand-written backward equals autograd
 # ------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("kind", [0, 1, 2])
@@ -409,6 +451,28 @@ def test_tail_and_epilogue_backward_match_autograd_cpu(kind, monkeypatch):
                                              dtype=d)), R(torch.full((n,), g_rc, dtype=d)), Gates())
         for a, b, what in ((gP_a, gP.v, "g_packed"), (gacc_a, gacc.v, "g_acc"), (gd_a, gd.v, "g_depth")):
             assert torch.allclose(a, b, rtol=1e-10, atol=1e-12), (bg, what, float((a - b).abs().max()))
+
+
+@pytest.mark.parametrize("bg", [1, 0])
+def test_radiance_backward_matches_autograd_cpu(bg):
+    """radiance_backward against float64 autograd of radiance_forward (rows of rays with 0 to 5 rows), to 1e-10."""
+    g = torch.Generator().manual_seed(21 + bg)
+    d = torch.float64
+    n = 40
+    ray = torch.repeat_interleave(torch.arange(n), torch.randint(0, 6, (n,), generator=g))
+    m_ = ray.numel()
+    w = torch.rand(m_, generator=g, dtype=d).requires_grad_(True)
+    out = torch.rand(m_, 3, generator=g, dtype=d).requires_grad_(True)
+    acc = torch.rand(n, generator=g, dtype=d).requires_grad_(True)
+    depth = (torch.rand(n, generator=g, dtype=d) * 4).requires_grad_(True)
+    dz = torch.randn(n, generator=g, dtype=d)
+    gm, gd = torch.randn(n, 3, generator=g, dtype=d), torch.randn(n, generator=g, dtype=d)
+    rgb, dm = radiance_forward(w, out, ray, acc, depth, dz, bg)
+    got = torch.autograd.grad((rgb.v * gm).sum() + (dm.v * gd).sum(), [out, w, acc, depth], allow_unused=True)
+    got = [torch.zeros_like(x) if y is None else y for x, y in zip((out, w, acc, depth), got)]
+    want = radiance_backward(w.detach(), out.detach(), ray, dz, gm, gd, bg)
+    for a, b, what in zip(got, want, ("g_out", "g_weight", "g_acc", "g_depth")):
+        assert torch.allclose(a, b.v, rtol=1e-10, atol=1e-12), (bg, what, float((a - b.v).abs().max()))
 
 
 def test_chained_references_reproduce_the_oracle_cpu(monkeypatch):
@@ -522,28 +586,42 @@ def _oracle_density(m):
     return ps, ls
 
 
+class Dump:
+    """What check_stages reads: the workspace ``ws`` a forward/backward left its dumps in, the inputs of that launch
+    (model, rays, light ids, jitter or z table, noise, background flag) and the upstream gradients of its backward
+    (``gm``: map gradients by name, None for a map that got none; ``g_acc_map``, ``g_la``, ``g_lr``: None or tensors),
+    and the parameter gradients it produced: ``vmg`` (channel-last density planes, density lines, app planes, app
+    lines), ``g_basis``, ``g_ll``, ``mod`` (head module -> its six tensors), each prefilled with ``pre``."""
+
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+
 def run_case(cs, ws=None, n_rays=None, cap_valid=None, cap_app=None, bg=1, stats_key=""):
     """Drive the four entry points once on ``cs`` and check every stage.  -> dict with the totals.  With ``ws``
     given, its integer arrays keep what the launch before left in them."""
-    from tensoir_b200 import _lib, ops, vm_autograd as vm
+    return check_stages(launch(cs, ws, n_rays, cap_valid, cap_app, bg), stats_key)
+
+
+def launch(cs, ws=None, n_rays=None, cap_valid=None, cap_app=None, bg=1):
+    """tir_primary_march / _app_list / _heads / _backward once on ``cs``, seeded with random map gradients (fresnel
+    and roughness None), a non-NULL g_acc_map and both loss gradients, every parameter gradient prefilled with PRE
+    -> Dump"""
+    from tensoir_b200 import _lib, ops
     from tensoir_b200.primary_fused import Workspace, _jobs
-    import test_vm_kernels_fp64 as V
     lib = _lib.load()
     m = cs.m
     n_rays = n_rays or cs.rays.shape[0]
     rays, li = cs.rays[:n_rays].contiguous(), cs.li.reshape(-1)[:n_rays].to(torch.int32).contiguous()
     jitter = cs.jitter[:n_rays].contiguous()
     g = cs.g
-    what0 = f"{stats_key} n_rays {n_rays}"
     f = ops.device_field(m).refresh(m, force=True)
     keep = []
     jobs, n_jobs, heads, kind = _jobs(m, keep)
     if cs.table is not None:
         jitter = None
     cfg = ops.march_cfg(m, table=cs.table, n_samples=cs.n_samples, jitter=jitter, keep=keep)
-    # --- the march's reference: the modular valid-sample list (pinned to the oracle elsewhere)
-    ref = vm.valid_samples(m, rays[:, :3], rays[:, 3:6], n_samples=cs.n_samples, jitter=jitter, table=cs.table)
-    total = int(ref["offsets"][-1])
+    total = int(march_reference(m, rays, cs.n_samples, jitter, cs.table)["offsets"][-1])
     cv = cap_valid if cap_valid is not None else total
     ca = cap_app if cap_app is not None else total
     fresh = ws is None
@@ -561,14 +639,12 @@ def run_case(cs, ws=None, n_rays=None, cap_valid=None, cap_app=None, bg=1, stats
     w = ws.work_struct(noise, n_jobs, True)
     w.cap_valid, w.cap_app = cv, ca
     stream = _lib.stream_ptr()
-    t = ws.t
     _lib.check(lib.tir_primary_march(C.byref(f), _lib.dptr(rays), n_rays, C.byref(cfg), C.byref(w), None, stream),
                "tir_primary_march")
     _lib.check(lib.tir_primary_app_list(C.byref(f), n_rays, C.byref(w), stream), "tir_primary_app_list")
     maps_t = [torch.full((n_rays, c), SENT, device=DEV) for c in (3, 1, 3, 3, 1, 3, 1, 1)]
-    names = ("rgb", "depth", "normal", "albedo", "rough", "fresnel", "nd", "no")
     maps = _lib.TirRayMaps()
-    for k, x in zip(names, maps_t):
+    for k, x in zip(MAP_NAMES, maps_t):
         setattr(maps, k, x.data_ptr())
     mask = torch.empty(n_rays, dtype=torch.bool, device=DEV)
     losses = torch.full((2,), SENT, device=DEV)
@@ -578,10 +654,10 @@ def run_case(cs, ws=None, n_rays=None, cap_valid=None, cap_app=None, bg=1, stats
                                      _lib.dptr(losses), None, stream), "tir_primary_heads")
     # --- backward
     gm = {}
-    for k, x in zip(names, maps_t):
+    for k, x in zip(MAP_NAMES, maps_t):
         gm[k] = None if k in ("fresnel", "rough") else torch.randn(x.shape, generator=g).to(DEV)
     gmaps = _lib.TirRayMaps()
-    for k in names:
+    for k in MAP_NAMES:
         setattr(gmaps, k, None if gm[k] is None else gm[k].data_ptr())
     g_acc_map = torch.randn(n_rays, generator=g).to(DEV)
     g_la, g_lr = torch.randn(1, generator=g).to(DEV), torch.randn(1, generator=g).to(DEV)
@@ -607,8 +683,31 @@ def run_case(cs, ws=None, n_rays=None, cap_valid=None, cap_app=None, bg=1, stats
                                         n_rays, C.byref(w), C.byref(b), f0, bg, C.byref(gmaps), _lib.dptr(g_acc_map),
                                         _lib.dptr(g_la), _lib.dptr(g_lr), C.byref(gr), stream), "tir_primary_backward")
     torch.cuda.synchronize()
-    gates = Gates()
+    return Dump(m=m, ws=ws, rays=rays, li=li, jitter=jitter, table=cs.table, n_samples=cs.n_samples, cv=cv, ca=ca,
+                noise=noise, bg=bg, maps=maps_t, mask=mask, losses=losses, gm=gm, g_acc_map=g_acc_map, g_la=g_la,
+                g_lr=g_lr, vmg=vmg, g_basis=g_basis, g_ll=g_ll, mod=mod, pre=PRE, guards=True, fresh=fresh)
 
+
+def _scalar(g):
+    return 0.0 if g is None else float(g.reshape(-1)[0])
+
+
+def march_reference(m, rays, n_samples, jitter, table):
+    """the modular valid-sample list (pinned to the oracle elsewhere) of the same march"""
+    from tensoir_b200 import vm_autograd as vm
+    return vm.valid_samples(m, rays[:, :3], rays[:, 3:6], n_samples=n_samples, jitter=jitter, table=table)
+
+
+def front(d, what0):
+    """march, density, compositing and the appearance list of the launch in ``d`` against their references (the
+    module docstring's first three items) -> dict of what the later stages need"""
+    import test_vm_kernels_fp64 as V
+    m, ws, rays, t = d.m, d.ws, d.rays, d.ws.t
+    n_rays = rays.shape[0]
+    grid = [int(x) for x in m.gridSize]
+    cv, ca = d.cv, d.ca
+    ref = march_reference(m, rays, d.n_samples, d.jitter, d.table)
+    total = int(ref["offsets"][-1])
     # ================= 1. march
     status = t["status"].tolist()
     nv = min(total, cv)
@@ -618,7 +717,7 @@ def run_case(cs, ws=None, n_rays=None, cap_valid=None, cap_app=None, bg=1, stats
     assert torch.equal(t["offsets"][:n_rays + 1], want_off), what0
     for k, kr in (("v_ray", "ray"), ("v_sample", "sample"), ("v_xn", "xn"), ("v_z", "z"), ("v_dist", "dist")):
         assert torch.equal(t[k][:nv], ref[kr][:nv]), (what0, k)
-        if fresh or t[k].is_floating_point():
+        if d.guards and (d.fresh or t[k].is_floating_point()):
             assert bool((t[k][nv:] == (SENT if t[k].is_floating_point() else 0)).all()), (what0, k, "guard")
     # ================= 2. density and compositing
     softplus = m.fea2denseAct == "softplus"
@@ -626,13 +725,13 @@ def run_case(cs, ws=None, n_rays=None, cap_valid=None, cap_app=None, bg=1, stats
     dps, dls = _oracle_density(m)
     xv = t["v_xn"][:nv].double()
     with V.f64():
-        fo = O.OracleField(aabb=torch.tensor([[-1.0] * 3, [1.0] * 3]), grid_size=cs.grid, density_plane=dps,
+        fo = O.OracleField(aabb=torch.tensor([[-1.0] * 3, [1.0] * 3]), grid_size=grid, density_plane=dps,
                            density_line=dls, app_plane=dps, app_line=dls, basis_w=None, mlp_rgb=None)
         feat64 = O.density_feature(fo, xv)
-    ts = V.tap_sums(dps, dls, xv, False, False, cs.grid)
-    tu = V.tap_sums(dps, dls, xv, False, True, cs.grid)
+    ts = V.tap_sums(dps, dls, xv, False, False, grid)
+    tu = V.tap_sums(dps, dls, xv, False, True, grid)
     efeat = V.bound(sum((q["AP"] * q["AL"]).sum(1) for q in ts), sum((q["AP"] * q["AL"]).sum(1) for q in tu),
-                    grid=cs.grid)
+                    grid=grid)
     chk(t["v_feat"][:nv], feat64, efeat, f"{what0}: v_feat", "v_feat")
     featk = t["v_feat"][:nv].double()
     if softplus:
@@ -706,11 +805,39 @@ def run_case(cs, ws=None, n_rays=None, cap_valid=None, cap_app=None, bg=1, stats
     assert torch.equal(t["a_ray"][:na], t["v_ray"][src]), what0
     assert torch.equal(t["a_w"][:na], t["v_weight"][src]), what0
     assert torch.equal(t["a_xn"][:na], t["v_xn"][src]), what0
-    for k in ("a_w", "a_xn", "a_xj", "dn_feat", "dn_dfdx", "g_dn_feat", "g_dn_dfdx") + tuple(
-            f"{p}{j}" for j in range(n_jobs) for p in ("out", "g_out", "inp", "h2_", "gx0_")):
-        assert bool((t[k][na:] == SENT).all()), (what0, k, "guard")
-    if fresh:
-        assert bool((t["a_src"][na:] == 0).all()), (what0, "a_src guard")
+    return dict(gates=Gates(), total=total, total_app=total_app, nv=nv, na=na, src=src, sel=sel, cv=cv, ca=ca, grid=grid,
+                softplus=softplus, shift=shift, dps=dps, dls=dls, xv=xv, fo=fo, ts=ts, tu=tu, ray_v=ray_v, pos=pos, S=S,
+                valid=valid, pad=pad, r64=r64, fp64_ok=fp64_ok, z=z, bw=bw, bT=bT)
+
+
+def check_stages(d, stats_key=""):
+    """Every stage of a relight-phase forward/backward against float64, from the dumps and inputs in ``d`` (Dump).
+    With ``d.guards`` the rows past the lists' capacities must hold the sentinel (a launch of ``launch``).
+    -> dict with the totals"""
+    from tensoir_b200.primary_fused import _jobs
+    import test_vm_kernels_fp64 as V
+    m, ws, rays, li, bg, noise, PRE = d.m, d.ws, d.rays, d.li, d.bg, d.noise, d.pre
+    fresh = d.fresh
+    t = ws.t
+    n_rays = rays.shape[0]
+    jobs, n_jobs, heads, kind = _jobs(m, [])
+    ll = getattr(m, "light_line", None)
+    f0 = float(m.fixed_fresnel)
+    maps_t, mask, losses, gm = d.maps, d.mask, d.losses, d.gm
+    names = MAP_NAMES
+    vmg, g_basis, g_ll, mod = d.vmg, d.g_basis, d.g_ll, d.mod
+    what0 = f"{stats_key} n_rays {n_rays}"
+    c = front(d, what0)
+    gates = c["gates"]
+    total, total_app, nv, na, src, sel = c["total"], c["total_app"], c["nv"], c["na"], c["src"], c["sel"]
+    softplus, shift, grid, fo, dps, dls = c["softplus"], c["shift"], c["grid"], c["fo"], c["dps"], c["dls"]
+    # ================= 3. appearance list (guard rows)
+    if d.guards:
+        for k in ("a_w", "a_xn", "a_xj", "dn_feat", "dn_dfdx", "g_dn_feat", "g_dn_dfdx") + tuple(
+                f"{p}{j}" for j in range(n_jobs) for p in ("out", "g_out", "inp", "h2_", "gx0_")):
+            assert bool((t[k][na:] == SENT).all()), (what0, k, "guard")
+        if fresh:
+            assert bool((t["a_src"][na:] == 0).all()), (what0, "a_src guard")
     if na == 0:
         return dict(total=total, total_app=total_app, ws=ws, gates=gates)
     # ================= 4. heads forward
@@ -721,7 +848,7 @@ def run_case(cs, ws=None, n_rays=None, cap_valid=None, cap_app=None, bg=1, stats
     pts = [T["a_xn"], T["a_xj"]]
     aps, als = [p.detach() for p in m.app_plane], [p.detach() for p in m.app_line]
     for ps in (0, 1):
-        check_gather(aps, als, cs.grid, pts[ps], T[f"x0_{ps}"], f"{what0}: x0 of point set {ps}")
+        check_gather(aps, als, grid, pts[ps], T[f"x0_{ps}"], f"{what0}: x0 of point set {ps}")
     basis = m.basis_mat.weight.detach().double()
     ll64 = ll.weight.detach().double() if ll is not None else None
     L = ll64.shape[0] if ll is not None else 1
@@ -745,16 +872,16 @@ def run_case(cs, ws=None, n_rays=None, cap_valid=None, cap_app=None, bg=1, stats
             xs = xa.clone().requires_grad_(True)
             ftc = O.density_feature_with_xyz_grad(fo, xs)
             (dfd,) = torch.autograd.grad(ftc.sum(), xs)
-        tsc = V.tap_sums(dps, dls, xa, True, False, cs.grid)
-        tuc = V.tap_sums(dps, dls, xa, True, True, cs.grid)
+        tsc = V.tap_sums(dps, dls, xa, True, False, grid)
+        tuc = V.tap_sums(dps, dls, xa, True, True, grid)
         mf, md = V._grad_mags(tsc, xa)
         uf, ud = V._grad_mags(tuc, xa)
-        chk(T["dn_feat"], ftc.detach(), V.bound(mf, uf, grid=cs.grid), f"{what0}: dn_feat", "dn_feat")
-        gi = torch.stack([(xa[:, a] + 1) / 2 * (cs.grid[a] - 1) for a in range(3)], 1)
-        near = ((gi - gi.round()).abs() <= 4 * EPS32 * (max(cs.grid) - 1)).any(1)
+        chk(T["dn_feat"], ftc.detach(), V.bound(mf, uf, grid=grid), f"{what0}: dn_feat", "dn_feat")
+        gi = torch.stack([(xa[:, a] + 1) / 2 * (grid[a] - 1) for a in range(3)], 1)
+        near = ((gi - gi.round()).abs() <= 4 * EPS32 * (max(grid) - 1)).any(1)
         STATS["texel-centre rows"] = STATS.get("texel-centre rows", 0) + int(near.sum())
         assert int(near.sum()) <= 0.01 * na + 2, (what0, int(near.sum()))
-        chk(T["dn_dfdx"][~near], dfd[~near], V.bound(md, ud, grid=cs.grid)[~near], f"{what0}: dn_dfdx", "dn_dfdx")
+        chk(T["dn_dfdx"][~near], dfd[~near], V.bound(md, ud, grid=grid)[~near], f"{what0}: dn_dfdx", "dn_dfdx")
     # ================= 5. tail forward
     j_of = {jobs[j].role: j for j in range(n_jobs)}
     o_rgb, o_b, o_bj = T[f"out{j_of[0]}"], T[f"out{j_of[1]}"], T[f"out{j_of[2]}"]
@@ -781,16 +908,16 @@ def run_case(cs, ws=None, n_rays=None, cap_valid=None, cap_app=None, bg=1, stats
         chk_r(x.reshape(eo[k].v.shape), eo[k], f"{what0}: map {k}", f"map {k}")
     chk_r(maps_t[5], eo["fresnel"], f"{what0}: map fresnel", "map fresnel")
     assert torch.equal(mask, t["acc"][:n_rays] > 0.5), what0
-    for i, c in enumerate((10, 11)):
-        want = Pk[:, c].sum() / n_rays
-        bnd = sum_bound(Pk[:, c].abs().sum(), n_rays) / n_rays + 2 * EPS32 * Pk[:, c].abs().sum() / n_rays
+    for i, col in enumerate((10, 11)):
+        want = Pk[:, col].sum() / n_rays
+        bnd = sum_bound(Pk[:, col].abs().sum(), n_rays) / n_rays + 2 * EPS32 * Pk[:, col].abs().sum() / n_rays
         chk(losses[i:i + 1], want.reshape(1), bnd.reshape(1) + 1e-30, f"{what0}: loss {i}", "losses")
     # ================= 7. backward: epilogue
     gz = {k: (gm[k].double() if gm[k] is not None else torch.zeros(x.shape, dtype=torch.float64, device=DEV))
           for k, x in zip(names, maps_t)}
     gz = {k: (v_.reshape(-1) if v_.shape[1] == 1 else v_) for k, v_ in gz.items()}
-    g_ac = R(torch.full((n_rays,), float(g_la), dtype=torch.float64, device=DEV)) / float(n_rays)
-    g_rc = R(torch.full((n_rays,), float(g_lr), dtype=torch.float64, device=DEV)) / float(n_rays)
+    g_ac = R(torch.full((n_rays,), _scalar(d.g_la), dtype=torch.float64, device=DEV)) / float(n_rays)
+    g_rc = R(torch.full((n_rays,), _scalar(d.g_lr), dtype=torch.float64, device=DEV)) / float(n_rays)
     gP, gacc, gdep = epilogue_backward(Pk, acck, dz, f0, bg, gz, g_ac, g_rc, gates)
     chk_r(t["g_packed"][:n_rays], gP, f"{what0}: g_packed", "g_packed")
     chk_r(t["g_acc"][:n_rays], gacc, f"{what0}: g_acc", "g_acc")
@@ -843,10 +970,29 @@ def run_case(cs, ws=None, n_rays=None, cap_valid=None, cap_app=None, bg=1, stats
         chk(g_ll - PRE, wsum["light"], bsum["light"] + sum_bound(PRE, na * n_jobs), f"{what0}: d light_line",
             "light_line")
     # the appearance factors: both point sets through one float64 scatter of the summed d x0
-    check_factor_grads(aps, als, cs.grid, torch.cat(pts), torch.cat(a_ps), vmg[2], vmg[3],
+    check_factor_grads(aps, als, grid, torch.cat(pts), torch.cat(a_ps), vmg[2], vmg[3],
                        f"{what0}: appearance factors", prefill=PRE)
+    back(d, c, what0, (T["a_xn"], T["g_dn_feat"], T["g_dn_dfdx"], tsc, tuc) if has_dn else None)
+    return dict(total=total, total_app=total_app, ws=ws, gates=gates, lengths=t["counts"][:n_rays].clone(),
+                flat_rows=int((dn["norm"].v <= LO).sum()) if has_dn else 0, weights=t["v_weight"][:nv].clone(),
+                t_zero=int((t["v_trans"][:nv] == 0).sum()), t_last_zero=int((t["t_last"][:n_rays] == 0).sum()))
+
+
+def back(d, c, what0, dgrad):
+    """compositing backward and density scatter of the launch in ``d`` (``c``: front's dict), from the kernel's own
+    g_weight, g_acc (+ the caller's g_acc_map) and g_depth; ``dgrad``: None, or (a_xn, g_dn_feat, g_dn_dfdx, tap sums
+    of the gradient gather, their unit sums) of the derived normals' double backward"""
+    import test_vm_kernels_fp64 as V
+    t, PRE, vmg = d.ws.t, d.pre, d.vmg
+    n_rays = d.rays.shape[0]
+    nv, cv, grid, pad, r64, z = c["nv"], c["cv"], c["grid"], c["pad"], c["r64"], c["z"]
+    bw, bT, fp64_ok, valid, softplus, shift = c["bw"], c["bT"], c["fp64_ok"], c["valid"], c["softplus"], c["shift"]
+    dps, dls, xv, ts, tu = c["dps"], c["dls"], c["xv"], c["ts"], c["tu"]
+    if dgrad is not None:
+        xa, g_dn_feat, g_dn_dfdx, tsc, tuc = dgrad
+    g_ext = d.g_acc_map.double() if d.g_acc_map is not None else torch.zeros(n_rays, dtype=torch.float64, device=DEV)
     # ================= compositing backward (from the kernel's own g_weight, g_acc + g_acc_map, g_depth)
-    ga_tot = t["g_acc"][:n_rays].double() + g_acc_map.double()
+    ga_tot = t["g_acc"][:n_rays].double() + g_ext
     gdk = t["g_depth"][:n_rays].double()
     gw_pad = pad(t["g_weight"])
     loss = (r64["w"] * gw_pad).sum() + (r64["w"].sum(1) * ga_tot).sum() + ((r64["w"] * z).sum(1) * gdk).sum()
@@ -858,7 +1004,7 @@ def run_case(cs, ws=None, n_rays=None, cap_valid=None, cap_app=None, bg=1, stats
     else:
         ds = (featp > 0).double()
     gfeat64 = gsig64 * ds
-    bnd, bwd_ok = composite_bwd_bound(r64, bw, bT, gw_pad, ga_tot, gdk, z, g_acc_map.double(), t["g_acc"][:n_rays].double(),
+    bnd, bwd_ok = composite_bwd_bound(r64, bw, bT, gw_pad, ga_tot, gdk, z, g_ext, t["g_acc"][:n_rays].double(),
                               gsig64, ds, gfeat64)
     gf = pad(t["g_feat"])
     assert bool(torch.isfinite(t["g_feat"][:nv]).all()), what0
@@ -870,36 +1016,164 @@ def run_case(cs, ws=None, n_rays=None, cap_valid=None, cap_app=None, bg=1, stats
     # that fp32 knows to no relative precision, so neither float64 nor the fp32 autograd of the reference's
     # expression (which differentiates cumprod, not the kernel's suffix sum) bounds it; only finiteness is checked
     STATS["g_feat rows with om unresolved"] = STATS.get("g_feat rows with om unresolved", 0) + int(bwd_32.sum())
-    assert bool((t["g_feat"][cv:] == SENT).all()) and bool((t["g_weight"][cv:] == SENT).all()), (what0, "guard")
+    if d.guards:
+        assert bool((t["g_feat"][cv:] == SENT).all()) and bool((t["g_weight"][cv:] == SENT).all()), (what0, "guard")
     # ================= density factors: g_feat at v_xn (zero padding) + the double backward at a_xn (clamped)
     gfk = t["g_feat"][:nv].double()
     with V.f64():
         dps_ = [p.clone().requires_grad_(True) for p in dps]
         dls_ = [p.clone().requires_grad_(True) for p in dls]
-        fg = O.OracleField(aabb=torch.tensor([[-1.0] * 3, [1.0] * 3]), grid_size=cs.grid, density_plane=dps_,
+        fg = O.OracleField(aabb=torch.tensor([[-1.0] * 3, [1.0] * 3]), grid_size=grid, density_plane=dps_,
                            density_line=dls_, app_plane=dps_, app_line=dls_, basis_w=None, mlp_rgb=None)
         loss = (O.density_feature(fg, xv) * gfk).sum()
-        if has_dn:
-            xs = T["a_xn"].clone().requires_grad_(True)
+        if dgrad is not None:
+            xs = xa.clone().requires_grad_(True)
             ftc = O.density_feature_with_xyz_grad(fg, xs)
             (dfd,) = torch.autograd.grad(ftc.sum(), xs, create_graph=True)
-            loss = loss + (ftc * T["g_dn_feat"]).sum() + (dfd * T["g_dn_dfdx"]).sum()
+            loss = loss + (ftc * g_dn_feat).sum() + (dfd * g_dn_dfdx).sum()
         loss.backward()
     agf = gfk.abs()[:, None]
     mv = V.scatter(ts, lambda k, q, j: agf * q["ptaps"][j][1][:, None] * q["AL"],
                    lambda k, q, j: agf * q["ltaps"][j][1][:, None] * q["AP"], 16)
     uv = V.scatter(tu, lambda k, q, j: agf * q["ptaps"][j][1][:, None] * q["AL"],
                    lambda k, q, j: agf * q["ltaps"][j][1][:, None] * q["AP"], 16)
-    if has_dn:
-        mc, uc = _dgrad_scatter(tsc, tuc, T["g_dn_feat"].abs(), T["g_dn_dfdx"].abs())
+    if dgrad is not None:
+        mc, uc = _dgrad_scatter(tsc, tuc, g_dn_feat.abs(), g_dn_dfdx.abs())
         mv = [tuple(a + b_ for a, b_ in zip(x, y)) for x, y in zip(mv, mc)]
         uv = [tuple(a + b_ for a, b_ in zip(x, y)) for x, y in zip(uv, uc)]
     mv = [(mp + PRE, ml + PRE, cp, cl) for mp, ml, cp, cl in mv]
     V.check_scatter([x - PRE for x in vmg[0]], [x - PRE for x in vmg[1]], [p.grad for p in dps_],
-                    [p.grad for p in dls_], mv, uv, f"{what0}: density factors", cs.grid)
-    return dict(total=total, total_app=total_app, ws=ws, gates=gates, lengths=t["counts"][:n_rays].clone(),
-                flat_rows=int((dn["norm"].v <= LO).sum()) if has_dn else 0, weights=t["v_weight"][:nv].clone(),
-                t_zero=int((t["v_trans"][:nv] == 0).sum()), t_last_zero=int((t["t_last"][:n_rays] == 0).sum()))
+                    [p.grad for p in dls_], mv, uv, f"{what0}: density factors", grid)
+
+
+def launch_radiance(cs, bg=1):
+    """tir_primary_march / _app_list / _radiance / _radiance_backward once on ``cs`` with random rgb, depth and acc map
+    gradients, every parameter gradient prefilled with PRE -> Dump"""
+    from tensoir_b200 import _lib, ops
+    from tensoir_b200.primary_fused import Workspace, _radiance_job
+    lib = _lib.load()
+    m, g = cs.m, cs.g
+    n_rays = cs.rays.shape[0]
+    rays, li = cs.rays, cs.li.reshape(-1).to(torch.int32).contiguous()
+    jitter = None if cs.table is not None else cs.jitter
+    f = ops.device_field(m).refresh(m, force=True)
+    keep = []
+    job = _radiance_job(m, keep)
+    cfg = ops.march_cfg(m, table=cs.table, n_samples=cs.n_samples, jitter=jitter, keep=keep)
+    total = int(march_reference(m, rays, cs.n_samples, jitter, cs.table)["offsets"][-1])
+    ws = Workspace(DEV, point_sets=1)
+    ws.ensure(n_rays, total + 257, total + 257, 1, True)
+    fill_sentinel(ws)
+    w = ws.work_struct(None, 1, True)
+    w.cap_valid, w.cap_app = total, total
+    stream = _lib.stream_ptr()
+    _lib.check(lib.tir_primary_march(C.byref(f), _lib.dptr(rays), n_rays, C.byref(cfg), C.byref(w), None, stream),
+               "tir_primary_march")
+    _lib.check(lib.tir_primary_app_list(C.byref(f), n_rays, C.byref(w), stream), "tir_primary_app_list")
+    rgb, depth = torch.full((n_rays, 3), SENT, device=DEV), torch.full((n_rays, 1), SENT, device=DEV)
+    _lib.check(lib.tir_primary_radiance(C.byref(f), C.byref(job), _lib.dptr(rays), _lib.dptr(li, torch.int32), n_rays,
+                                        C.byref(w), bg, _lib.dptr(rgb), _lib.dptr(depth), stream),
+               "tir_primary_radiance")
+    gm = dict(rgb=torch.randn(n_rays, 3, generator=g).to(DEV), depth=torch.randn(n_rays, 1, generator=g).to(DEV))
+    g_acc_map = torch.randn(n_rays, generator=g).to(DEV)
+    b = ws.bwd_struct(1)
+    gr = _lib.TirPrimaryGrads()
+    vmg = grad_bufs(m, DEV)
+    for k in range(3):
+        gr.dplane[k], gr.dline[k] = vmg[0][k].data_ptr(), vmg[1][k].data_ptr()
+        gr.aplane[k], gr.aline[k] = vmg[2][k].data_ptr(), vmg[3][k].data_ptr()
+    g_basis = torch.full_like(m.basis_mat.weight, PRE)
+    gr.basis = g_basis.data_ptr()
+    ll = getattr(m, "light_line", None)
+    g_ll = torch.full_like(ll.weight, PRE) if ll is not None else None
+    gr.light_line = None if ll is None else g_ll.data_ptr()
+    mlp = m.renderModule.mlp
+    mod = {"renderModule": [torch.full_like(x, PRE) for x in (mlp[0].weight, mlp[0].bias, mlp[2].weight, mlp[2].bias,
+                                                               mlp[4].weight, mlp[4].bias)]}
+    gr.w0[0], gr.b0[0], gr.w1[0], gr.b1[0], gr.w2[0], gr.b2[0] = [x.data_ptr() for x in mod["renderModule"]]
+    _lib.check(lib.tir_primary_radiance_backward(C.byref(f), C.byref(job), _lib.dptr(rays), _lib.dptr(li, torch.int32),
+                                                 n_rays, C.byref(w), C.byref(b), bg, _lib.dptr(gm["rgb"]),
+                                                 _lib.dptr(gm["depth"]), _lib.dptr(g_acc_map), C.byref(gr), stream),
+               "tir_primary_radiance_backward")
+    torch.cuda.synchronize()
+    return Dump(m=m, ws=ws, rays=rays, li=li, jitter=jitter, table=cs.table, n_samples=cs.n_samples, cv=total,
+                ca=total, noise=None, bg=bg, maps=[rgb, depth], mask=None, losses=None, gm=gm, g_acc_map=g_acc_map,
+                g_la=None, g_lr=None, vmg=vmg, g_basis=g_basis, g_ll=g_ll, mod=mod, pre=PRE, guards=True, fresh=True)
+
+
+def check_radiance_stages(d, stats_key=""):
+    """Every stage of a radiance-only forward/backward (tir_primary_radiance / _backward) against float64, from the
+    dumps and inputs in ``d`` (Dump; ``d.maps`` = [rgb_map, depth_map], ``d.gm`` holds "rgb" and "depth"):
+      * march, density, compositing and the appearance list as in check_stages;
+      * the head (test_heads_kernels_fp64: gather, Stages.forward, data_grads, param_grads, check_factor_grads);
+      * radiance_ray_fwd_kernel: rgb_map = sum_rows w out (+ 1 - acc) and depth_map = depth (+ (1 - acc) rays[..., 5])
+        from the kernel's own rows, acc and depth, in R arithmetic with (count) eps32 of sum|w out| for the sum;
+      * radiance_ray_bwd_kernel: g_out = w g_rgb (4th column 0), g_weight[a_src] = out . g_rgb (0 on every other
+        valid row), g_acc = -(sum g_rgb) - g_depth rays[..., 5] under a background (else 0), g_depth = g_depth_map;
+      * compositing backward and the density scatter (back), with no double backward.
+    -> dict with the totals"""
+    from tensoir_b200.primary_fused import _radiance_job
+    from test_heads_kernels_fp64 import P_W
+    m, ws, rays, li, bg, PRE = d.m, d.ws, d.rays, d.li, d.bg, d.pre
+    t = ws.t
+    n_rays = rays.shape[0]
+    what0 = f"{stats_key} radiance n_rays {n_rays}"
+    c = front(d, what0)
+    grid, nv, na, src = c["grid"], c["nv"], c["na"], c["src"]
+    if d.guards:
+        for k in ("a_w", "a_xn", "out0", "g_out0", "inp0", "h2_0", "gx0_0"):
+            assert bool((t[k][na:] == SENT).all()), (what0, k, "guard")
+    if na == 0:
+        return dict(total=c["total"], total_app=c["total_app"], ws=ws, gates=c["gates"])
+    T = {k: v[:na].double() for k, v in t.items() if v.shape[0] == ws.cap_app and v.is_floating_point()}
+    ray = t["a_ray"][:na].long()
+    aps, als = [p.detach() for p in m.app_plane], [p.detach() for p in m.app_line]
+    check_gather(aps, als, grid, T["a_xn"], T["x0_0"], f"{what0}: x0")
+    job = _radiance_job(m, [])
+    ll = getattr(m, "light_line", None)
+    ll64 = ll.weight.detach().double() if ll is not None else None
+    mlp = m.renderModule.mlp
+    W = [mlp[i].weight.detach().double() for i in (0, 2, 4)]
+    B = [mlp[i].bias.detach().double() for i in (0, 2, 4)]
+    vd = rays[ray, 3:6].double()
+    st = Stages(na, job.light_mode if ll is not None else 0, 0, ll64.shape[0] if ll is not None else 1, W, B,
+                m.basis_mat.weight.detach().double(), ll64, li.long()[ray], vd, T["x0_0"], T["inp0"], T["h1_0"],
+                T["h2_0"], T["out0"][:, :3])
+    st.forward(f"{what0}: head")
+    # ================= radiance_ray_fwd_kernel, from the kernel's own rows, acc and depth
+    o, aw = T["out0"][:, :3], T["a_w"]
+    dz = rays[:, 5].double()
+    rgb, depth = radiance_forward(aw, o, ray, t["acc"][:n_rays].double(), t["depth"][:n_rays].double(), dz, bg)
+    chk_r(d.maps[0], rgb, f"{what0}: rgb_map", "radiance rgb_map")
+    chk_r(d.maps[1].reshape(-1), depth, f"{what0}: depth_map", "radiance depth_map")
+    # ================= radiance_ray_bwd_kernel
+    zero3 = torch.zeros(n_rays, 3, dtype=torch.float64, device=DEV)
+    g = d.gm["rgb"].double().reshape(n_rays, 3) if d.gm.get("rgb") is not None else zero3
+    gd = d.gm["depth"].double().reshape(-1) if d.gm.get("depth") is not None else zero3[:, 0]
+    g_out, gw, g_acc, g_depth = radiance_backward(aw, o, ray, dz, g, gd, bg)
+    chk_r(t["g_acc"][:n_rays], g_acc, f"{what0}: g_acc", "radiance g_acc")
+    chk_r(t["g_depth"][:n_rays], g_depth, f"{what0}: g_depth", "radiance g_depth")
+    chk_r(T["g_out0"][:, :3], g_out, f"{what0}: g_out", "radiance g_out")
+    assert bool((t["g_out0"][:na, 3] == 0).all()), what0
+    chk_r(t["g_weight"][:nv].double()[src], gw, f"{what0}: g_weight", "radiance g_weight")
+    other = torch.ones(nv, dtype=torch.bool, device=DEV)
+    other[src] = False
+    assert bool((t["g_weight"][:nv][other] == 0).all()), what0
+    # ================= head backward and the appearance factors
+    a = st.data_grads(f"{what0}: head", T["g_out0"], T["gz2_0"], T["gz1_0"], T["gfeat0"][:, :NF], T["gx0_0"])
+    want, bnds = st.param_grads(T["g_out0"], T["gz2_0"], T["gz1_0"], T["gfeat0"][:, :NF], a)
+    for k, buf in zip(("w0", "b0", "w1", "b1", "w2", "b2"), d.mod["renderModule"]):
+        chk(buf - PRE, want[k], bnds[k] + sum_bound(PRE, P_W) + 1e-30, f"{what0}: d renderModule.{k}", "head weights")
+    chk(d.g_basis - PRE, want["basis"], bnds["basis"] + sum_bound(PRE, P_W) + 1e-30, f"{what0}: d basis_mat",
+        "basis_mat")
+    if "light" in want:
+        chk(d.g_ll - PRE, want["light"], bnds["light"] + sum_bound(PRE, na) + 1e-30, f"{what0}: d light_line",
+            "light_line")
+    check_factor_grads(aps, als, grid, T["a_xn"], T["gx0_0"], d.vmg[2], d.vmg[3], f"{what0}: appearance factors",
+                       prefill=PRE)
+    back(d, c, what0, None)
+    return dict(total=c["total"], total_app=c["total_app"], ws=ws, gates=c["gates"],
+                lengths=t["counts"][:n_rays].clone())
 
 
 def composite_bwd_bound(r64, bw, bT, gw_pad, ga_tot, gdk, z, g_ext, g_acc_k, gsig64, ds, gfeat64):
@@ -1041,6 +1315,17 @@ def test_lego_bench_batch_stages():
     assert max(lens) > 64 and 0 in lens, max(lens)
     assert_gates(res["gates"], res["total_app"], "lego")
     report("lego 128")
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("bg", [1, 0], ids=["bg", "no_bg"])
+def test_radiance_stages(bg):
+    """tir_primary_radiance / _backward on rotated_g24 (a light_line model: the head reads each ray's own light) with
+    random rgb, depth and acc map gradients, with and without the background term."""
+    m, rays, li = rotated("derived_plus_predicted")
+    res = check_radiance_stages(launch_radiance(Case(m, rays, li, -1, 8), bg=bg), stats_key=f"rotated bg {bg}")
+    assert res["total_app"] > 100
+    report(f"radiance bg {bg}")
 
 
 @pytest.mark.gpu
