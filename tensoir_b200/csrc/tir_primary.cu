@@ -411,6 +411,70 @@ TailPtrs tail_ptrs(const TirField* field, const TirPrimaryWork* w, const float* 
   return t;
 }
 
+int check_radiance_job(const TirHeadJob* job) {
+  if (!job) return TIR_ERR_NULL;
+  if (job->role != TIR_HEAD_RGB || job->point_set != 0 || job->x_in != 0) return TIR_ERR_CONFIG;
+  if (job->light_mode < 0 || job->light_mode > 2) return TIR_ERR_CONFIG;
+  return TIR_OK;
+}
+
+// an MLP without a light_line reads no light, whatever the job asks for
+int job_light_mode(const TirHeadJob& job) { return job.mlp.light_line ? job.light_mode : 0; }
+
+// the forward of job slot j over the appearance list of w (save_x0 is left to the caller: one dump per point set)
+HeadJobDev head_job_dev(const TirHeadJob& job, int j, const float* rays, const int32_t* light_idx,
+                        const TirPrimaryWork* w) {
+  HeadJobDev d{};
+  d.mlp = job.mlp;
+  d.xn = job.point_set == 0 ? w->a_xn : w->a_xj;
+  if (job.x_in == 0) { d.x_in = rays + 3; d.x_in_stride = 6; d.x_index = w->a_ray; }
+  else { d.x_in = d.xn; d.x_in_stride = 3; d.x_index = nullptr; }
+  d.light_mode = job_light_mode(job);
+  if (d.light_mode == 1) { d.light_idx = light_idx; d.x_index = w->a_ray; }
+  d.act = job.act;
+  d.out = w->out[j]; d.out_stride = 4;
+  d.save_in = w->inp[j]; d.save_h1 = w->h1[j]; d.save_h2 = w->h2[j];
+  return d;
+}
+
+// the backward of job slot j: its forward dumps, its scratch and its parameter gradients
+HeadBwdJob head_bwd_job(const TirHeadJob& job, int j, const int32_t* light_idx, const TirPrimaryWork* w,
+                        const TirPrimaryBwdWork* b, const TirPrimaryGrads* gr) {
+  HeadBwdJob h{};
+  h.mlp = job.mlp;
+  h.light_mode = job_light_mode(job);
+  h.x_index = h.light_mode == 1 ? w->a_ray : nullptr;
+  h.light_idx = h.light_mode == 1 ? light_idx : nullptr;
+  h.act = job.act; h.point_set = job.point_set;
+  h.out = w->out[j]; h.out_stride = 4; h.g_out = b->g_out[j];
+  h.inp = w->inp[j]; h.h1 = w->h1[j]; h.h2 = w->h2[j];
+  h.gz1 = b->gz1[j]; h.gz2 = b->gz2[j]; h.gfeat = b->gfeat[j]; h.gx0 = b->gx0[j];
+  h.g_w0 = gr->w0[j]; h.g_b0 = gr->b0[j]; h.g_w1 = gr->w1[j]; h.g_b1 = gr->b1[j]; h.g_w2 = gr->w2[j]; h.g_b2 = gr->b2[j];
+  return h;
+}
+
+// the VM-factor gradient buffers of gr, appearance and density; every one must be given
+int vm_grad_ptrs(const TirPrimaryGrads* gr, GradPtrs* app, GradPtrs* density) {
+  for (int k = 0; k < 3; ++k) {
+    app->plane[k] = gr->aplane[k]; app->line[k] = gr->aline[k];
+    density->plane[k] = gr->dplane[k]; density->line[k] = gr->dline[k];
+    if (!app->plane[k] || !app->line[k] || !density->plane[k] || !density->line[k]) return TIR_ERR_NULL;
+  }
+  return TIR_OK;
+}
+
+// the last two stages of both backwards: compositing (+ feature2density) with the acc_map / depth_map gradients folded
+// in, then the density scatter
+int composite_density_bwd(const TirField* field, int64_t n_rays, const TirPrimaryWork* w, const TirPrimaryBwdWork* b,
+                          const float* g_acc_map, const GradPtrs& gd, cudaStream_t stream) {
+  primary_composite_bwd_kernel<<<(unsigned)((n_rays * 32 + 255) / 256), 256, 0, stream>>>(
+      *field, w->v_feat, w->v_sigma, w->v_dist, w->v_z, w->offsets, n_rays, field->distance_scale, w->cap_valid,
+      w->v_weight, w->v_trans, b->g_weight, b->g_acc, g_acc_map, b->g_depth, b->g_feat);
+  const int rc = launch_density_bwd(*field, w->v_xn, w->cap_valid, w->offsets + n_rays, b->g_feat, gd, stream);
+  if (rc) return rc;
+  return (int)cudaGetLastError();
+}
+
 }  // namespace
 
 extern "C" int tir_epilogue_fwd(int64_t n, const float* packed, const float* acc, const float* depth, const float* rays,
@@ -481,18 +545,9 @@ extern "C" int tir_primary_heads(const TirField* field, const TirHeadJob* jobs, 
   HeadJobDev dev[kMaxHeadJobs];
   for (int j = 0; j < n_jobs; ++j) {
     if (!w->out[j]) return TIR_ERR_NULL;
-    HeadJobDev& d = dev[j];
-    d = HeadJobDev{};
-    d.mlp = jobs[j].mlp;
-    d.xn = jobs[j].point_set == 0 ? w->a_xn : w->a_xj;
-    if (jobs[j].x_in == 0) { d.x_in = rays + 3; d.x_in_stride = 6; d.x_index = w->a_ray; }
-    else { d.x_in = d.xn; d.x_in_stride = 3; d.x_index = nullptr; }
-    d.light_mode = jobs[j].mlp.light_line ? jobs[j].light_mode : 0;
-    if (d.light_mode == 1) { d.light_idx = light_idx; d.x_index = w->a_ray; }
-    if (d.light_mode == 1 && jobs[j].x_in != 0) return TIR_ERR_CONFIG;   // an indexed light needs the ray index table
-    d.act = jobs[j].act;
-    d.out = w->out[j]; d.out_stride = 4;
-    d.save_in = w->inp[j]; d.save_h1 = w->h1[j]; d.save_h2 = w->h2[j];
+    // an indexed light needs the ray index table
+    if (job_light_mode(jobs[j]) == 1 && jobs[j].x_in != 0) return TIR_ERR_CONFIG;
+    dev[j] = head_job_dev(jobs[j], j, rays, light_idx, w);
   }
   // the raw products are dumped once per point set (by the first head that visits it)
   bool saved[2] = {false, false};
@@ -536,7 +591,6 @@ extern "C" int tir_primary_backward(const TirField* field, const TirHeadJob* job
   cudaStream_t stream = (cudaStream_t)stream_;
   const int64_t cap = w->cap_app;
   const int64_t* n_app = w->a_offsets + n_rays;
-  const int64_t* n_valid = w->offsets + n_rays;
 
   // 1. per-ray epilogue
   rc = tir_epilogue_bwd(n_rays, w->packed, w->acc, w->depth, rays, fresnel0, white_bg, g_maps, g_loss_albedo,
@@ -554,19 +608,7 @@ extern "C" int tir_primary_backward(const TirField* field, const TirHeadJob* job
   primary_tail_bwd_kernel<<<blocks_for(cap, 256), 256, 0, stream>>>(t, q, cap, n_app, b->g_packed);
   // 3. heads: data gradient + weight gradients
   HeadBwdJob hb[kMaxHeadJobs];
-  for (int j = 0; j < n_jobs; ++j) {
-    HeadBwdJob& h = hb[j];
-    h = HeadBwdJob{};
-    h.mlp = jobs[j].mlp;
-    h.light_mode = jobs[j].mlp.light_line ? jobs[j].light_mode : 0;
-    h.x_index = h.light_mode == 1 ? w->a_ray : nullptr;
-    h.light_idx = h.light_mode == 1 ? light_idx : nullptr;
-    h.act = jobs[j].act; h.point_set = jobs[j].point_set;
-    h.out = w->out[j]; h.out_stride = 4; h.g_out = b->g_out[j];
-    h.inp = w->inp[j]; h.h1 = w->h1[j]; h.h2 = w->h2[j];
-    h.gz1 = b->gz1[j]; h.gz2 = b->gz2[j]; h.gfeat = b->gfeat[j]; h.gx0 = b->gx0[j];
-    h.g_w0 = gr->w0[j]; h.g_b0 = gr->b0[j]; h.g_w1 = gr->w1[j]; h.g_b1 = gr->b1[j]; h.g_w2 = gr->w2[j]; h.g_b2 = gr->b2[j];
-  }
+  for (int j = 0; j < n_jobs; ++j) hb[j] = head_bwd_job(jobs[j], j, light_idx, w, b, gr);
   HeadsBwdShared sh{};
   sh.x0[0] = w->x0[0]; sh.x0[1] = w->x0[1]; sh.g_basis = gr->basis; sh.g_light = gr->light_line;
   rc = launch_heads_backward(*field, hb, n_jobs, sh, cap, n_app, stream);
@@ -574,11 +616,8 @@ extern "C" int tir_primary_backward(const TirField* field, const TirHeadJob* job
   // 4. appearance scatters, one per point set (the heads of a set summed on load), and 5. the derived normals' double
   // backward of the density gather (tensorBase:846-853): one launch over the appearance list
   GradPtrs ga{}, gd{};
-  for (int k = 0; k < 3; ++k) {
-    ga.plane[k] = gr->aplane[k]; ga.line[k] = gr->aline[k];
-    gd.plane[k] = gr->dplane[k]; gd.line[k] = gr->dline[k];
-    if (!ga.plane[k] || !ga.line[k] || !gd.plane[k] || !gd.line[k]) return TIR_ERR_NULL;
-  }
+  rc = vm_grad_ptrs(gr, &ga, &gd);
+  if (rc) return rc;
   AppScatterJob sj[kMaxAppScatterJobs] = {};
   int n_sj = 0;
   for (int ps = 0; ps < 2; ++ps) {
@@ -600,30 +639,11 @@ extern "C" int tir_primary_backward(const TirField* field, const TirHeadJob* job
   }
   rc = launch_app_scatter(*field, sj, n_sj, cap, n_app, stream);
   if (rc) return rc;
-  // 6. compositing (+ feature2density), acc_map / depth_map gradients folded in
-  primary_composite_bwd_kernel<<<(unsigned)((n_rays * 32 + 255) / 256), 256, 0, stream>>>(
-      *field, w->v_feat, w->v_sigma, w->v_dist, w->v_z, w->offsets, n_rays, field->distance_scale, w->cap_valid,
-      w->v_weight, w->v_trans, b->g_weight, b->g_acc, g_acc_map, b->g_depth, b->g_feat);
-  // 7. density scatter
-  rc = launch_density_bwd(*field, w->v_xn, w->cap_valid, n_valid, b->g_feat, gd, stream);
-  if (rc) return rc;
-  return (int)cudaGetLastError();
+  // 6. compositing and 7. density scatter
+  return composite_density_bwd(field, n_rays, w, b, g_acc_map, gd, stream);
 }
 
 // ---- radiance-only primary: TensorBase.forward with is_relight=False -------------------------------------------------
-namespace {
-
-int check_radiance_job(const TirHeadJob* job) {
-  if (!job) return TIR_ERR_NULL;
-  if (job->role != TIR_HEAD_RGB || job->point_set != 0 || job->x_in != 0) return TIR_ERR_CONFIG;
-  if (job->light_mode < 0 || job->light_mode > 2) return TIR_ERR_CONFIG;
-  return TIR_OK;
-}
-
-int radiance_light_mode(const TirHeadJob* job) { return job->mlp.light_line ? job->light_mode : 0; }
-
-}  // namespace
-
 extern "C" int tir_primary_radiance(const TirField* field, const TirHeadJob* job, const float* rays,
                                     const int32_t* light_idx, int64_t n_rays, const TirPrimaryWork* w, int32_t white_bg,
                                     float* rgb_map, float* depth_map, void* stream_) {
@@ -632,20 +652,12 @@ extern "C" int tir_primary_radiance(const TirField* field, const TirHeadJob* job
   int rc = check_radiance_job(job);
   if (rc) return rc;
   if (!w->a_offsets || !w->a_ray || !w->a_w || !w->a_xn || !w->acc || !w->depth || !w->out[0]) return TIR_ERR_NULL;
-  const int mode = radiance_light_mode(job);
-  if (mode == 1 && !light_idx) return TIR_ERR_NULL;
+  if (job_light_mode(*job) == 1 && !light_idx) return TIR_ERR_NULL;
   cudaStream_t stream = (cudaStream_t)stream_;
   const int64_t cap = w->cap_app;
   const int64_t* n_app = w->a_offsets + n_rays;
-  HeadJobDev d{};
-  d.mlp = job->mlp;
-  d.xn = w->a_xn;
-  d.x_in = rays + 3; d.x_in_stride = 6; d.x_index = w->a_ray;
-  d.light_mode = mode;
-  d.light_idx = mode == 1 ? light_idx : nullptr;
-  d.act = job->act;
-  d.out = w->out[0]; d.out_stride = 4;
-  d.save_x0 = w->x0[0]; d.save_in = w->inp[0]; d.save_h1 = w->h1[0]; d.save_h2 = w->h2[0];
+  HeadJobDev d = head_job_dev(*job, 0, rays, light_idx, w);
+  d.save_x0 = w->x0[0];
   rc = launch_heads_forward(*field, &d, 1, cap, n_app, stream);
   if (rc) return rc;
   radiance_ray_fwd_kernel<<<(unsigned)((n_rays + 127) / 128), 128, 0, stream>>>(
@@ -667,18 +679,13 @@ extern "C" int tir_primary_radiance_backward(const TirField* field, const TirHea
     return TIR_ERR_NULL;
   if (!w->x0[0] || !w->inp[0] || !w->h1[0] || !w->h2[0] || !w->out[0] || !w->a_src || !w->a_w || !w->a_xn)
     return TIR_ERR_NULL;
-  const int mode = radiance_light_mode(job);
-  if (mode == 1 && !light_idx) return TIR_ERR_NULL;
+  if (job_light_mode(*job) == 1 && !light_idx) return TIR_ERR_NULL;
   GradPtrs ga{}, gd{};
-  for (int k = 0; k < 3; ++k) {
-    ga.plane[k] = gr->aplane[k]; ga.line[k] = gr->aline[k];
-    gd.plane[k] = gr->dplane[k]; gd.line[k] = gr->dline[k];
-    if (!ga.plane[k] || !ga.line[k] || !gd.plane[k] || !gd.line[k]) return TIR_ERR_NULL;
-  }
+  rc = vm_grad_ptrs(gr, &ga, &gd);
+  if (rc) return rc;
   cudaStream_t stream = (cudaStream_t)stream_;
   const int64_t cap = w->cap_app;
   const int64_t* n_app = w->a_offsets + n_rays;
-  const int64_t* n_valid = w->offsets + n_rays;
 
   // 1. epilogue + per-sample tail: d out of the head, d weight onto the valid list, d acc / d depth per ray
   cudaError_t e = cudaMemsetAsync(b->g_weight, 0, (size_t)w->cap_valid * sizeof(float), stream);
@@ -687,16 +694,7 @@ extern "C" int tir_primary_radiance_backward(const TirField* field, const TirHea
       w->out[0], w->a_w, w->a_offsets, w->a_src, n_rays, cap, rays, white_bg, g_rgb_map, g_depth_map, b->g_out[0],
       b->g_weight, b->g_acc, b->g_depth);
   // 2. head: data gradient + weight gradients
-  HeadBwdJob h{};
-  h.mlp = job->mlp;
-  h.light_mode = mode;
-  h.x_index = mode == 1 ? w->a_ray : nullptr;
-  h.light_idx = mode == 1 ? light_idx : nullptr;
-  h.act = job->act; h.point_set = 0;
-  h.out = w->out[0]; h.out_stride = 4; h.g_out = b->g_out[0];
-  h.inp = w->inp[0]; h.h1 = w->h1[0]; h.h2 = w->h2[0];
-  h.gz1 = b->gz1[0]; h.gz2 = b->gz2[0]; h.gfeat = b->gfeat[0]; h.gx0 = b->gx0[0];
-  h.g_w0 = gr->w0[0]; h.g_b0 = gr->b0[0]; h.g_w1 = gr->w1[0]; h.g_b1 = gr->b1[0]; h.g_w2 = gr->w2[0]; h.g_b2 = gr->b2[0];
+  const HeadBwdJob h = head_bwd_job(*job, 0, light_idx, w, b, gr);
   HeadsBwdShared sh{};
   sh.x0[0] = w->x0[0]; sh.x0[1] = nullptr; sh.g_basis = gr->basis; sh.g_light = gr->light_line;
   rc = launch_heads_backward(*field, &h, 1, sh, cap, n_app, stream);
@@ -706,11 +704,6 @@ extern "C" int tir_primary_radiance_backward(const TirField* field, const TirHea
   sj.xn = w->a_xn; sj.g[0] = b->gx0[0]; sj.out = ga;
   rc = launch_app_scatter(*field, &sj, 1, cap, n_app, stream);
   if (rc) return rc;
-  // 4. compositing (+ feature2density) with the acc / depth gradients, 5. density scatter
-  primary_composite_bwd_kernel<<<(unsigned)((n_rays * 32 + 255) / 256), 256, 0, stream>>>(
-      *field, w->v_feat, w->v_sigma, w->v_dist, w->v_z, w->offsets, n_rays, field->distance_scale, w->cap_valid,
-      w->v_weight, w->v_trans, b->g_weight, b->g_acc, g_acc_map, b->g_depth, b->g_feat);
-  rc = launch_density_bwd(*field, w->v_xn, w->cap_valid, n_valid, b->g_feat, gd, stream);
-  if (rc) return rc;
-  return (int)cudaGetLastError();
+  // 4. compositing and 5. density scatter
+  return composite_density_bwd(field, n_rays, w, b, g_acc_map, gd, stream);
 }

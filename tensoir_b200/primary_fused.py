@@ -11,6 +11,7 @@ device-side flag instead.
 from __future__ import annotations
 
 import ctypes as C
+from collections import namedtuple
 
 import torch
 
@@ -19,7 +20,6 @@ from .device_field import mlp_struct
 
 HEAD_RGB, HEAD_BRDF, HEAD_BRDF_JITTER, HEAD_NORMAL = 0, 1, 2, 3
 NORMALS = {"derived_plus_predicted": 0, "purely_predicted": 1, "purely_derived": 2}
-MAXH = _lib.MAX_HEADS
 
 
 TirHeadJob, TirPrimaryWork, TirPrimaryBwdWork, TirPrimaryGrads = (_lib.TirHeadJob, _lib.TirPrimaryWork,
@@ -106,30 +106,36 @@ class Workspace:
         return b
 
 
-def _jobs(model, keep):
-    """(TirHeadJob array, n_jobs, module name of every job)."""
+# Every head job of the primary march: (module, role, point set, x_in, light mode when the model has a light_line, act).
+# The relight phase (tensorBase:930-1004) runs all of them, renderModule_normal only when the normals are predicted; the
+# radiance-only phase runs the renderModule row alone: the view direction in, light_line[light_idx] if the model has one.
+_JOB_SPEC = (("renderModule", HEAD_RGB, 0, 0, 1, 0),
+             ("renderModule_brdf", HEAD_BRDF, 0, 1, 2, 0),
+             ("renderModule_brdf", HEAD_BRDF_JITTER, 1, 1, 2, 0),
+             ("renderModule_normal", HEAD_NORMAL, 0, 1, 2, 1))
+HEADS = ("renderModule", "renderModule_brdf", "renderModule_normal")
+
+
+def _jobs(model, keep, heads=HEADS):
+    """The job table of a node over the head modules ``heads`` -> (TirHeadJob array, n_jobs, module of every job,
+    normals kind)."""
     kind = NORMALS[model.normals_kind]
     has_light = getattr(model, "light_line", None) is not None
-    spec = [("renderModule", HEAD_RGB, 0, 0, 1 if has_light else 0, 0),
-            ("renderModule_brdf", HEAD_BRDF, 0, 1, 2 if has_light else 0, 0),
-            ("renderModule_brdf", HEAD_BRDF_JITTER, 1, 1, 2 if has_light else 0, 0)]
-    if kind != 2:
-        spec.append(("renderModule_normal", HEAD_NORMAL, 0, 1, 2 if has_light else 0, 1))
+    spec = [s for s in _JOB_SPEC if s[0] in heads and not (s[1] == HEAD_NORMAL and kind == 2)]
     arr = (TirHeadJob * len(spec))()
     for j, (head, role, ps, x_in, lm, act) in enumerate(spec):
         arr[j].mlp = mlp_struct(model, head, keep, light="index" if has_light else "none")
-        arr[j].point_set, arr[j].x_in, arr[j].light_mode, arr[j].act, arr[j].role = ps, x_in, lm, act, role
+        arr[j].point_set, arr[j].x_in, arr[j].act, arr[j].role = ps, x_in, act, role
+        arr[j].light_mode = lm if has_light else 0
     return arr, len(spec), [s[0] for s in spec], kind
 
 
-def _cl_zeros(p):
-    """Zeroed gradient buffer in the kernels' channel-last layout + its view in the parameter's shape."""
-    _, Cc, H, W = p.shape
-    buf = torch.zeros((H, W, Cc), device=p.device, dtype=torch.float32)
-    return buf, buf.permute(2, 0, 1).unsqueeze(0)
+def _radiance_job(model, keep):
+    """The one job of the radiance-only node: the renderModule row of the job table."""
+    return _jobs(model, keep, HEADS[:1])[0][0]
 
 
-def _workspace(model, key, dev, need, point_sets=2):
+def _workspace(model, key, dev, need, point_sets):
     """The cached workspace of ``model.__dict__[key]``, marked busy until the backward when ``need``."""
     ws = model.__dict__.get(key)
     if ws is None or ws.dev != dev:
@@ -175,33 +181,39 @@ def _march(lib, f, rays, cfg, ws, n_jobs, need, counters, st):
     return w, n_app
 
 
-def _vm_grad_buffers(model):
-    """Gradient buffers of the VM factors (17-31 M floats), in the order density planes, density lines, app planes, app
-    lines -> (buffers the kernels accumulate into, what autograd gets for each factor).  When a parameter already HAS
-    a dense channel-last .grad (kept zeroed in place by tensoir_b200.optim.FusedAdam, or the views of a dp.GradBucket)
-    the kernels accumulate straight into it and autograd gets None for that input: no 70 MB allocation + memset +
-    AccumulateGrad pass per step.  Otherwise a zeroed buffer in the kernels' layout is returned the usual way."""
-    vm = list(model.density_plane) + list(model.density_line) + list(model.app_plane) + list(model.app_line)
-    bufs, views = [], []
-    for p in vm:
-        g = p.grad
-        if (g is not None and g.dtype == torch.float32 and g.shape == p.shape and p.shape[0] == 1
-                and all(a == b for a, b, n in zip(g.stride(), p.stride(), p.shape) if n > 1)
-                and p.is_contiguous(memory_format=torch.channels_last)
-                and model.__dict__.get("_tir_grad_inplace", True)):
-            bufs.append(g)
-            views.append(None)
-        else:
-            b_, v_ = _cl_zeros(p)
-            bufs.append(b_)
-            views.append(v_)
-    return bufs, views
+def _vm_factors(model):
+    """The VM factors in the order density planes, density lines, app planes, app lines."""
+    return list(model.density_plane) + list(model.density_line) + list(model.app_plane) + list(model.app_line)
 
 
-def _set_vm_grads(gr, bufs):
-    for k in range(3):
-        gr.dplane[k], gr.dline[k] = bufs[k].data_ptr(), bufs[3 + k].data_ptr()
-        gr.aplane[k], gr.aline[k] = bufs[6 + k].data_ptr(), bufs[9 + k].data_ptr()
+def _head_params(model, head):
+    m = getattr(model, head).mlp
+    return [m[0].weight, m[0].bias, m[2].weight, m[2].bias, m[4].weight, m[4].bias]
+
+
+def _params(model, heads):
+    """Autograd inputs of a primary node: VM factors, basis, [light_line], 6 tensors per head."""
+    params = _vm_factors(model) + [model.basis_mat.weight]
+    ll = getattr(model, "light_line", None)
+    if ll is not None:
+        params.append(ll.weight)
+    for head in heads:
+        params += _head_params(model, head)
+    return params
+
+
+def _vm_target(p, inplace):
+    """(buffer the kernels accumulate into, what autograd gets) for a VM factor: its own .grad when that is dense in
+    the parameter's channel-last layout, else a zeroed buffer in the kernels' layout and its view in the parameter's
+    shape."""
+    g = p.grad
+    if (inplace and g is not None and g.dtype == torch.float32 and g.shape == p.shape and p.shape[0] == 1
+            and all(a == b for a, b, n in zip(g.stride(), p.stride(), p.shape) if n > 1)
+            and p.is_contiguous(memory_format=torch.channels_last)):
+        return g, None
+    _, Cc, H, W = p.shape
+    buf = torch.zeros((H, W, Cc), device=p.device, dtype=torch.float32)
+    return buf, buf.permute(2, 0, 1).unsqueeze(0)
 
 
 def _grad_target(p, inplace):
@@ -215,133 +227,178 @@ def _grad_target(p, inplace):
     return z, z
 
 
+def _grad_targets(model, heads, job_heads):
+    """The parameter gradients of a node over the head modules ``heads`` whose job j runs ``job_heads[j]`` ->
+    (TirPrimaryGrads, the gradients autograd gets in the order of _params(model, heads): None for a head without a job).
+
+    When a parameter already HAS a dense .grad (kept zeroed in place by tensoir_b200.optim.FusedAdam, or the views of a
+    dp.GradBucket) the kernels accumulate straight into it and autograd gets None for that input: for the VM factors
+    (17-31 M floats) no 70 MB allocation + memset + AccumulateGrad pass per step.  With ``model._tir_grad_inplace``
+    off, or without such a .grad, a zeroed buffer is returned the usual way."""
+    inplace = model.__dict__.get("_tir_grad_inplace", True)
+    gr = TirPrimaryGrads()
+    grads = []
+    for k, p in enumerate(_vm_factors(model)):
+        buf, ret = _vm_target(p, inplace)
+        (gr.dplane, gr.dline, gr.aplane, gr.aline)[k // 3][k % 3] = buf.data_ptr()
+        grads.append(ret)
+    buf, ret = _grad_target(model.basis_mat.weight, inplace)
+    gr.basis = buf.data_ptr()
+    grads.append(ret)
+    ll = getattr(model, "light_line", None)
+    if ll is not None:
+        buf, ret = _grad_target(ll.weight, inplace)
+        gr.light_line = buf.data_ptr()
+        grads.append(ret)
+    for head in heads:
+        slots = [j for j, h in enumerate(job_heads) if h == head]
+        if not slots:
+            grads += [None] * 6
+            continue
+        ts = [_grad_target(t, inplace) for t in _head_params(model, head)]
+        for j in slots:
+            gr.w0[j], gr.b0[j], gr.w1[j], gr.b1[j], gr.w2[j], gr.b2[j] = [t[0].data_ptr() for t in ts]
+        grads += [t[1] for t in ts]
+    return gr, tuple(grads)
+
+
+# ctx.keep of the two nodes: what their backwards read, and the host tensors (keep) their job tables and march configs
+# point into.  cfg: the TirMarchCfg of the march, noise: the smoothness term's xyz noise, li: int32 light index per ray,
+# bg: the background flag.
+_RelightKeep = namedtuple("_RelightKeep", "keep jobs n_jobs kind cfg noise li rays ws jitter")
+_RadianceKeep = namedtuple("_RadianceKeep", "keep jobs li rays ws jitter bg")
+
+
+def _forward_common(ctx, model, rays, light_idx, is_train, n_samples, jitter, heads, ws_key):
+    """What both nodes' forwards do before their own C call: field refresh, job table, march config, workspace, march
+    and appearance list; ``ctx`` gets the model and the heads its backward hands gradients to -> (library, field,
+    work struct, appearance rows (None in shape-static mode), keep, jobs, normals kind, march config, int32 light
+    indices, workspace)."""
+    lib = _lib.load()
+    need = any(ctx.needs_input_grad)
+    f = ops.device_field(model).refresh(model, force=bool(is_train))
+    keep = []
+    jobs, n_jobs, job_heads, kind = _jobs(model, keep, heads)
+    cfg = ops.march_cfg(model, n_samples=n_samples, jitter=jitter, keep=keep)
+    point_sets = 1 + max(jobs[j].point_set for j in range(n_jobs))
+    ws = _workspace(model, ws_key, rays.device, need, point_sets)
+    li = light_idx.reshape(-1).to(torch.int32).contiguous()
+    w, n_app = _march(lib, f, rays, cfg, ws, n_jobs, need, model.__dict__.get("_tir_counters"),
+                      model.__dict__.get("_tir_static"))
+    ctx.model, ctx.heads, ctx.job_heads = model, heads, job_heads
+    return lib, f, w, n_app, keep, jobs, kind, cfg, li, ws
+
+
+def _f32(t):
+    return None if t is None else t.contiguous().float()
+
+
+def _ptr(t):
+    return None if t is None else _lib.dptr(t)
+
+
+# per-ray shape of the maps of TensorBase.forward's 12-tuple: rgb, depth, normal, albedo, roughness, fresnel, acc,
+# normals_diff, normals_orientation, acc_mask; the albedo and roughness smoothness losses follow
+_MAP_SHAPES = ((3,), (), (3,), (3,), (1,), (3,), (), (1,), (1,), ())
+_RAY_MAPS = (0, 1, 2, 3, 4, 5, 7, 8)        # the entries TirRayMaps holds, in its field order
+
+
+def _ray_maps(ts):
+    maps = _lib.TirRayMaps()
+    for k, t in zip(("rgb", "depth", "normal", "albedo", "rough", "fresnel", "nd", "no"), ts):
+        setattr(maps, k, None if t is None else t.data_ptr())
+    return maps
+
+
 class _PrimaryRelight(torch.autograd.Function):
     @staticmethod
     def forward(ctx, model, rays, light_idx, white_bg, is_train, n_samples, bg_flag, jitter, *params):
-        lib = _lib.load()
-        cd = lib
-        dev = rays.device
-        st = model.__dict__.get("_tir_static")
-        need = any(ctx.needs_input_grad)
-        n_rays = rays.shape[0]
-        df = ops.device_field(model)
-        f = df.refresh(model, force=bool(is_train))
-        keep = []
-        jobs, n_jobs, heads, kind = _jobs(model, keep)
-        cfg = ops.march_cfg(model, n_samples=n_samples, jitter=jitter, keep=keep)
-        counters = model.__dict__.get("_tir_counters")
-        cptr = None if counters is None else _lib.dptr(counters, torch.int64)
-        ws = _workspace(model, "_tir_primary_ws", dev, need)
-        li = light_idx.reshape(-1).to(torch.int32).contiguous()
-        stream = _lib.stream_ptr()
-        w, n_app = _march(cd, f, rays, cfg, ws, n_jobs, need, counters, st)
+        lib, f, w, n_app, keep, jobs, kind, cfg, li, ws = _forward_common(ctx, model, rays, light_idx, is_train,
+                                                                          n_samples, jitter, HEADS, "_tir_primary_ws")
+        dev, n_rays = rays.device, rays.shape[0]
         # xyz noise of the smoothness term: randn_like(xyz_sampled[app_mask]) (tensorBase:937), drawn on the device in
         # list order; the eager path draws exactly n_app rows like the reference
         draw = model.__dict__.get("_tir_randn_like")       # test hook: replay the oracle's stream / deterministic noise
-        rows = ws.cap_app if st is not None else int(n_app)
+        rows = ws.cap_app if model.__dict__.get("_tir_static") is not None else int(n_app)
         noise = torch.zeros(ws.cap_app, 3, device=dev)
         if rows > 0:
             x_a = ws.t["a_xn"][:rows]
             noise[:rows] = draw(x_a) if draw is not None else torch.randn_like(x_a)
         w.noise = noise.data_ptr()
-        outs = [torch.empty(n_rays, 3, device=dev), torch.empty(n_rays, device=dev), torch.empty(n_rays, 3, device=dev),
-                torch.empty(n_rays, 3, device=dev), torch.empty(n_rays, 1, device=dev), torch.empty(n_rays, 3, device=dev),
-                torch.empty(n_rays, 1, device=dev), torch.empty(n_rays, 1, device=dev)]
-        maps = _lib.TirRayMaps()
-        for k, t in zip(("rgb", "depth", "normal", "albedo", "rough", "fresnel", "nd", "no"), outs):
-            setattr(maps, k, t.data_ptr())
+        outs = [torch.empty((n_rays,) + _MAP_SHAPES[k], device=dev) for k in _RAY_MAPS]
         mask = torch.empty(n_rays, dtype=torch.bool, device=dev)
         losses = torch.empty(2, device=dev)
-        _lib.check(cd.tir_primary_heads(C.byref(f), jobs, n_jobs, kind, _lib.dptr(rays), _lib.dptr(li, torch.int32),
-                                        n_rays, C.byref(w), float(model.fixed_fresnel), int(bool(bg_flag)),
-                                        C.byref(maps), _lib.dptr(mask, torch.bool), _lib.dptr(losses), cptr, stream),
-                   "tir_primary_heads")
+        counters = model.__dict__.get("_tir_counters")
+        _lib.check(lib.tir_primary_heads(C.byref(f), jobs, len(jobs), kind, _lib.dptr(rays), _lib.dptr(li, torch.int32),
+                                         n_rays, C.byref(w), float(model.fixed_fresnel), int(bool(bg_flag)),
+                                         C.byref(_ray_maps(outs)), _lib.dptr(mask, torch.bool), _lib.dptr(losses),
+                                         None if counters is None else _lib.dptr(counters, torch.int64),
+                                         _lib.stream_ptr()), "tir_primary_heads")
         if kind == 1:
             _lib.launch_count -= 1          # no derived-normal gather
         acc = ws.t["acc"].clone()
-        ctx.model, ctx.need, ctx.heads = model, need, heads
-        ctx.cfg_args = (white_bg, bool(bg_flag), n_samples, bool(is_train))
-        ctx.keep = (keep, jobs, n_jobs, kind, cfg, noise, li, rays, ws, jitter)
+        ctx.bg = int(bool(bg_flag))
+        ctx.keep = _RelightKeep(keep, jobs, len(jobs), kind, cfg, noise, li, rays, ws, jitter)
         ctx.mark_non_differentiable(mask)
         rgb, depth, normal, albedo, rough, fresnel, nd, no = outs
         return rgb, depth, normal, albedo, rough, fresnel, acc, nd, no, mask, losses[0], losses[1]
 
     @staticmethod
     def backward(ctx, g_rgb, g_depth, g_normal, g_albedo, g_rough, g_fresnel, g_acc, g_nd, g_no, _g_mask, g_la, g_lr):
-        model = ctx.model
-        keep, jobs, n_jobs, kind, cfg, noise, li, rays, ws, jitter = ctx.keep
+        k, model = ctx.keep, ctx.model
         lib = _lib.load()
-        cd = lib
-        df = ops.device_field(model)
-        f = df.refresh(model)
-        dev = rays.device
-        n_rays = rays.shape[0]
-
-        def c(t):
-            return None if t is None else t.contiguous().float()
-        gs = [c(t) for t in (g_rgb, g_depth, g_normal, g_albedo, g_rough, g_fresnel, g_nd, g_no)]
-        gmaps = _lib.TirRayMaps()
-        for k, t in zip(("rgb", "depth", "normal", "albedo", "rough", "fresnel", "nd", "no"), gs):
-            setattr(gmaps, k, None if t is None else t.data_ptr())
-        g_acc, g_la, g_lr = c(g_acc), (None if g_la is None else c(g_la.reshape(1))), (None if g_lr is None else
-                                                                                       c(g_lr.reshape(1)))
-        w = ws.work_struct(noise, n_jobs, True)
-        b = ws.bwd_struct(n_jobs)
-        gr = TirPrimaryGrads()
-        bufs, views = _vm_grad_buffers(model)
-        _set_vm_grads(gr, bufs)
-        inplace = model.__dict__.get("_tir_grad_inplace", True)
-
-        def target(p):
-            return _grad_target(p, inplace)
-        g_basis, r_basis = target(model.basis_mat.weight)
-        gr.basis = g_basis.data_ptr()
-        ll = getattr(model, "light_line", None)
-        g_light, r_light = target(ll.weight) if ll is not None else (None, None)
-        gr.light_line = None if g_light is None else g_light.data_ptr()
-        mod_grads = {}
-        for j, head in enumerate(ctx.heads):
-            if head not in mod_grads:
-                m = getattr(model, head).mlp
-                mod_grads[head] = [target(t) for t in (m[0].weight, m[0].bias, m[2].weight, m[2].bias, m[4].weight,
-                                                       m[4].bias)]
-            g = mod_grads[head]
-            gr.w0[j], gr.b0[j], gr.w1[j], gr.b1[j], gr.w2[j], gr.b2[j] = [t[0].data_ptr() for t in g]
-        white_bg, bg_flag, n_samples, is_train = ctx.cfg_args
-        _lib.check(cd.tir_primary_backward(C.byref(f), jobs, n_jobs, kind, _lib.dptr(rays), _lib.dptr(li, torch.int32),
-                                           n_rays, C.byref(w), C.byref(b), float(model.fixed_fresnel), int(bg_flag),
-                                           C.byref(gmaps), None if g_acc is None else _lib.dptr(g_acc),
-                                           None if g_la is None else _lib.dptr(g_la),
-                                           None if g_lr is None else _lib.dptr(g_lr), C.byref(gr), _lib.stream_ptr()),
+        f = ops.device_field(model).refresh(model)
+        gs = [_f32(t) for t in (g_rgb, g_depth, g_normal, g_albedo, g_rough, g_fresnel, g_nd, g_no)]
+        g_acc = _f32(g_acc)
+        g_la, g_lr = [None if t is None else _f32(t.reshape(1)) for t in (g_la, g_lr)]
+        w, b = k.ws.work_struct(k.noise, k.n_jobs, True), k.ws.bwd_struct(k.n_jobs)
+        gr, grads = _grad_targets(model, ctx.heads, ctx.job_heads)
+        _lib.check(lib.tir_primary_backward(C.byref(f), k.jobs, k.n_jobs, k.kind, _lib.dptr(k.rays),
+                                            _lib.dptr(k.li, torch.int32), k.rays.shape[0], C.byref(w), C.byref(b),
+                                            float(model.fixed_fresnel), ctx.bg, C.byref(_ray_maps(gs)), _ptr(g_acc),
+                                            _ptr(g_la), _ptr(g_lr), C.byref(gr), _lib.stream_ptr()),
                    "tir_primary_backward")
-        if kind == 1:
+        if k.kind == 1:
             _lib.launch_count -= 1          # no derived-normal scatter
-        ws.busy = False
-        # gradients in the order of `params` (see forward_relight): VM factors, basis, [light_line], 3 x 6 MLP tensors
-        out = list(views) + [r_basis] + ([r_light] if ll is not None else [])
-        for head in ("renderModule", "renderModule_brdf", "renderModule_normal"):
-            out += [t[1] for t in mod_grads[head]] if head in mod_grads else [None] * 6
-        return (None, None, None, None, None, None, None, None, *out)
+        k.ws.busy = False
+        return (None,) * 8 + grads
+
+
+class _PrimaryRadiance(torch.autograd.Function):
+    """TensorBase.forward with is_relight=False (training's warm-up phase) around tir_primary_march / _app_list /
+    _radiance (9 launches) and tir_primary_radiance_backward (6 launches) -> (rgb_map, depth_map, acc_map)."""
+
+    @staticmethod
+    def forward(ctx, model, rays, light_idx, is_train, n_samples, bg_flag, jitter, *params):
+        lib, f, w, _, keep, jobs, _, _, li, ws = _forward_common(ctx, model, rays, light_idx, is_train, n_samples,
+                                                                 jitter, HEADS[:1], "_tir_radiance_ws")
+        n_rays, dev = rays.shape[0], rays.device
+        rgb, depth = torch.empty(n_rays, 3, device=dev), torch.empty(n_rays, device=dev)
+        _lib.check(lib.tir_primary_radiance(C.byref(f), jobs, _lib.dptr(rays), _lib.dptr(li, torch.int32), n_rays,
+                                            C.byref(w), int(bool(bg_flag)), _lib.dptr(rgb), _lib.dptr(depth),
+                                            _lib.stream_ptr()), "tir_primary_radiance")
+        ctx.keep = _RadianceKeep(keep, jobs, li, rays, ws, jitter, int(bool(bg_flag)))
+        return rgb, depth, ws.t["acc"].clone()
+
+    @staticmethod
+    def backward(ctx, g_rgb, g_depth, g_acc):
+        k, model = ctx.keep, ctx.model
+        lib = _lib.load()
+        f = ops.device_field(model).refresh(model)
+        g_rgb, g_depth, g_acc = _f32(g_rgb), _f32(g_depth), _f32(g_acc)
+        w, b = k.ws.work_struct(None, 1, True), k.ws.bwd_struct(1)
+        gr, grads = _grad_targets(model, ctx.heads, ctx.job_heads)
+        _lib.check(lib.tir_primary_radiance_backward(C.byref(f), k.jobs, _lib.dptr(k.rays),
+                                                     _lib.dptr(k.li, torch.int32), k.rays.shape[0], C.byref(w),
+                                                     C.byref(b), k.bg, _ptr(g_rgb), _ptr(g_depth), _ptr(g_acc),
+                                                     C.byref(gr), _lib.stream_ptr()), "tir_primary_radiance_backward")
+        k.ws.busy = False
+        return (None,) * 7 + grads
 
 
 def supported(model) -> bool:
     return (getattr(model, "shadingMode", None) == "MLP_Fea" and model.normals_kind in NORMALS
             and int(model.app_dim) == 27 and not model.__dict__.get("_tir_modular", False))
-
-
-def forward_relight(model, rays_chunk, light_idx, white_bg=True, is_train=False, N_samples=-1):
-    """-> the 12-tuple of TensorBase.forward (is_relight=True)."""
-    rays = rays_chunk.float().contiguous()
-    n_rays = rays.shape[0]
-    dev = rays.device
-    if n_rays == 0:        # torch.mean over zero rays is NaN in the reference; keep that contract on the empty batch
-        z3, z1, z = torch.zeros(0, 3, device=dev), torch.zeros(0, 1, device=dev), torch.zeros(0, device=dev)
-        nan = torch.full((), float("nan"), device=dev)
-        return (z3, z, z3.clone(), z3.clone(), z1, z3.clone(), z.clone(), z1.clone(), z1.clone(), z > 0.5, nan,
-                nan.clone())
-    jitter, bg = _host_draws(model, n_rays, dev, white_bg, is_train)
-    params = _params(model, ("renderModule", "renderModule_brdf", "renderModule_normal"))
-    return _PrimaryRelight.apply(model, rays, light_idx, white_bg, is_train, N_samples, bg, jitter, *params)
 
 
 def _host_draws(model, n_rays, dev, white_bg, is_train):
@@ -354,105 +411,31 @@ def _host_draws(model, n_rays, dev, white_bg, is_train):
     return jitter, white_bg or (is_train and bool(torch.rand((1,)) < 0.5))
 
 
-def _params(model, heads):
-    """Autograd inputs of a primary node: VM factors, basis, [light_line], 6 tensors per head."""
-    params = list(model.density_plane) + list(model.density_line) + list(model.app_plane) + list(model.app_line)
-    params.append(model.basis_mat.weight)
-    ll = getattr(model, "light_line", None)
-    if ll is not None:
-        params.append(ll.weight)
-    for head in heads:
-        m = getattr(model, head).mlp
-        params += [m[0].weight, m[0].bias, m[2].weight, m[2].bias, m[4].weight, m[4].bias]
-    return params
+def _forward(model, rays_chunk, white_bg, is_train, slots, run):
+    """TensorBase.forward's 12-tuple with the outputs of ``run(rays, background flag, jitter)`` (a node's apply) at
+    ``slots``, the rest None.  An empty batch runs no node: its maps are empty and its losses NaN, as torch.mean over
+    zero rays is in the reference."""
+    rays = rays_chunk.float().contiguous()
+    n_rays, dev = rays.shape[0], rays.device
+    if n_rays == 0:
+        outs = [torch.full((), float("nan"), device=dev) if k >= len(_MAP_SHAPES) else
+                torch.zeros((0,) + _MAP_SHAPES[k], device=dev, dtype=torch.bool if k == 9 else None) for k in slots]
+    else:
+        jitter, bg = _host_draws(model, n_rays, dev, white_bg, is_train)
+        outs = run(rays, bg, jitter)
+    ret = [None] * 12
+    for k, t in zip(slots, outs):
+        ret[k] = t
+    return tuple(ret)
 
 
-# ---- radiance-only primary (is_relight=False): training's warm-up phase -------------------------------------------------
-def _radiance_job(model, keep):
-    """The one head of the radiance branch: renderModule on the view direction, light_line[light_idx] if the model has
-    one (tensorBase:930-946, is_relight=False)."""
-    has_light = getattr(model, "light_line", None) is not None
-    job = TirHeadJob()
-    job.mlp = mlp_struct(model, "renderModule", keep, light="index" if has_light else "none")
-    job.point_set, job.x_in, job.light_mode, job.act, job.role = 0, 0, 1 if has_light else 0, 0, HEAD_RGB
-    return job
-
-
-class _PrimaryRadiance(torch.autograd.Function):
-    """TensorBase.forward with is_relight=False around tir_primary_march / _app_list / _radiance (9 launches) and
-    tir_primary_radiance_backward (6 launches) -> (rgb_map, depth_map, acc_map)."""
-
-    @staticmethod
-    def forward(ctx, model, rays, light_idx, is_train, n_samples, bg_flag, jitter, *params):
-        lib = _lib.load()
-        dev = rays.device
-        need = any(ctx.needs_input_grad)
-        n_rays = rays.shape[0]
-        f = ops.device_field(model).refresh(model, force=bool(is_train))
-        keep = []
-        job = _radiance_job(model, keep)
-        cfg = ops.march_cfg(model, n_samples=n_samples, jitter=jitter, keep=keep)
-        ws = _workspace(model, "_tir_radiance_ws", dev, need, point_sets=1)
-        w, _ = _march(lib, f, rays, cfg, ws, 1, need, model.__dict__.get("_tir_counters"),
-                      model.__dict__.get("_tir_static"))
-        li = light_idx.reshape(-1).to(torch.int32).contiguous()
-        rgb, depth = torch.empty(n_rays, 3, device=dev), torch.empty(n_rays, device=dev)
-        _lib.check(lib.tir_primary_radiance(C.byref(f), C.byref(job), _lib.dptr(rays), _lib.dptr(li, torch.int32),
-                                            n_rays, C.byref(w), int(bool(bg_flag)), _lib.dptr(rgb), _lib.dptr(depth),
-                                            _lib.stream_ptr()), "tir_primary_radiance")
-        acc = ws.t["acc"].clone()
-        ctx.model = model
-        ctx.keep = (keep, job, li, rays, ws, jitter, int(bool(bg_flag)))
-        return rgb, depth, acc
-
-    @staticmethod
-    def backward(ctx, g_rgb, g_depth, g_acc):
-        model = ctx.model
-        keep, job, li, rays, ws, jitter, bg = ctx.keep
-        lib = _lib.load()
-        f = ops.device_field(model).refresh(model)
-
-        def c(t):
-            return None if t is None else t.contiguous().float()
-        g_rgb, g_depth, g_acc = c(g_rgb), c(g_depth), c(g_acc)
-        w = ws.work_struct(None, 1, True)
-        b = ws.bwd_struct(1)
-        gr = TirPrimaryGrads()
-        bufs, views = _vm_grad_buffers(model)
-        _set_vm_grads(gr, bufs)
-        inplace = model.__dict__.get("_tir_grad_inplace", True)
-        g_basis, r_basis = _grad_target(model.basis_mat.weight, inplace)
-        gr.basis = g_basis.data_ptr()
-        ll = getattr(model, "light_line", None)
-        g_light, r_light = _grad_target(ll.weight, inplace) if ll is not None else (None, None)
-        gr.light_line = None if g_light is None else g_light.data_ptr()
-        m = model.renderModule.mlp
-        mg = [_grad_target(t, inplace) for t in (m[0].weight, m[0].bias, m[2].weight, m[2].bias, m[4].weight,
-                                                  m[4].bias)]
-        gr.w0[0], gr.b0[0], gr.w1[0], gr.b1[0], gr.w2[0], gr.b2[0] = [t[0].data_ptr() for t in mg]
-
-        def ptr(t):
-            return None if t is None else _lib.dptr(t)
-        _lib.check(lib.tir_primary_radiance_backward(C.byref(f), C.byref(job), _lib.dptr(rays),
-                                                     _lib.dptr(li, torch.int32), rays.shape[0], C.byref(w), C.byref(b),
-                                                     bg, ptr(g_rgb), ptr(g_depth), ptr(g_acc), C.byref(gr),
-                                                     _lib.stream_ptr()), "tir_primary_radiance_backward")
-        ws.busy = False
-        # gradients in the order of `params` (see forward_radiance): VM factors, basis, [light_line], renderModule
-        out = list(views) + [r_basis] + ([r_light] if ll is not None else []) + [t[1] for t in mg]
-        return (None,) * 7 + tuple(out)
+def forward_relight(model, rays_chunk, light_idx, white_bg=True, is_train=False, N_samples=-1):
+    """-> the 12-tuple of TensorBase.forward (is_relight=True)."""
+    return _forward(model, rays_chunk, white_bg, is_train, range(12), lambda rays, bg, jitter: _PrimaryRelight.apply(
+        model, rays, light_idx, white_bg, is_train, N_samples, bg, jitter, *_params(model, HEADS)))
 
 
 def forward_radiance(model, rays_chunk, light_idx, white_bg=True, is_train=False, N_samples=-1):
     """-> the 12-tuple of TensorBase.forward (is_relight=False): rgb_map, depth_map, acc_map, the rest None."""
-    rays = rays_chunk.float().contiguous()
-    n_rays = rays.shape[0]
-    dev = rays.device
-    if n_rays == 0:
-        z = torch.zeros(0, device=dev)
-        rgb, depth, acc = torch.zeros(0, 3, device=dev), z, z.clone()
-    else:
-        jitter, bg = _host_draws(model, n_rays, dev, white_bg, is_train)
-        params = _params(model, ("renderModule",))
-        rgb, depth, acc = _PrimaryRadiance.apply(model, rays, light_idx, is_train, N_samples, bg, jitter, *params)
-    return rgb, depth, None, None, None, None, acc, None, None, None, None, None
+    return _forward(model, rays_chunk, white_bg, is_train, (0, 1, 6), lambda rays, bg, jitter: _PrimaryRadiance.apply(
+        model, rays, light_idx, is_train, N_samples, bg, jitter, *_params(model, HEADS[:1])))

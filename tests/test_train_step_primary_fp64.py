@@ -94,6 +94,37 @@ def test_node_gradient_unpacking_cpu(golden_general, is_relight, kind):
             assert t.shape == p.shape and bool((t == idx[id(p)]).all()), head
 
 
+@pytest.mark.parametrize("is_relight", [True, False], ids=["relight", "phase1"])
+@pytest.mark.parametrize("kind", ["derived_plus_predicted", "purely_derived"])
+def test_grad_targets_follow_params_cpu(golden_general, is_relight, kind):
+    """primary_fused._grad_targets (``_tir_grad_inplace`` off): every kernel gradient buffer is the one returned for
+    its parameter in the order of primary_fused._params, job slot j writes into the head of job j, and a head without
+    a job gets None"""
+    from tensoir_b200 import primary_fused as F
+    m = model_from_fixture(golden_general, "cpu")
+    m.normals_kind = kind
+    m.__dict__["_tir_grad_inplace"] = False
+    heads = HEADS if is_relight else HEADS[:1]
+    _, n_jobs, job_heads, _ = F._jobs(m, [], heads)
+    gr, grads = F._grad_targets(m, heads, job_heads)
+    params = F._params(m, heads)
+    assert len(grads) == len(params) and n_jobs == len(job_heads)
+    vm = [gr.dplane[k] for k in range(3)] + [gr.dline[k] for k in range(3)] + [gr.aplane[k] for k in range(3)] + \
+        [gr.aline[k] for k in range(3)]
+    for k in range(12):
+        assert vm[k] == grads[k].data_ptr() and grads[k].shape == params[k].shape
+    assert gr.basis == grads[12].data_ptr() and gr.light_line == grads[13].data_ptr()
+    for j, head in enumerate(job_heads):
+        g = grads[14 + 6 * heads.index(head):20 + 6 * heads.index(head)]
+        assert [gr.w0[j], gr.b0[j], gr.w1[j], gr.b1[j], gr.w2[j], gr.b2[j]] == [t.data_ptr() for t in g]
+    for i, head in enumerate(heads):
+        g = grads[14 + 6 * i:20 + 6 * i]
+        if head in job_heads:
+            assert all(t.shape == p.shape and not t.any() for t, p in zip(g, params[14 + 6 * i:20 + 6 * i]))
+        else:
+            assert head == "renderModule_normal" and kind == "purely_derived" and list(g) == [None] * 6
+
+
 def captured_step(monkeypatch, m, rays, li, seed, is_relight, n_samples, args, white_bg=True):
     """One eager training step of train_loss with the fused primary node wrapped -> P.Dump of its forward/backward"""
     from tensoir_b200 import Renderer_TensoIR_train
