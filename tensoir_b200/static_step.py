@@ -9,15 +9,20 @@ forward + loss + backward + (optional gradient all-reduce) + Adam is captured on
 Anything the host changes from step to step must live in device memory to reach a replay: ray batch / light indices
 (copied in by ``run``), the host-drawn randoms (staged by ``run``), learning rates (``lr_tensors`` + ``scale_lr``), and
 any loss weight that ``loss_fn`` varies over the iterations (the reference decays its TV weights,
-train_tensoIR.py:277-282) — keep those in 0-dim device tensors and update them in place between replays; Python floats
-are baked in at capture.  Grid maintenance (updateAlphaMask / shrink / upsample) needs a new capture (``run`` checks).
+train_tensoIR.py:277-282) — keep those in 0-dim device tensors; Python floats are baked in at capture.  Values that
+change every iteration are best handed to ``run(..., scalars=(device_vector, host_values))``, which stages them with the
+step, so that a redone step reads its own.  Grid maintenance (updateAlphaMask / shrink / upsample) needs a new capture
+(``run`` checks).
 
-Capacities can never silently change the computation: every list records its real length on the device, a step whose
-lists did not fit raises a device-side flag that (i) turns the optimizer update of that very step into an exact no-op
-(``found_inf`` of the fused Adam: parameters, moments and step counters untouched) and (ii) is read back by the host a
-step later, which then re-captures the graph with larger lists and REDOES the same batch.  The host also watches the
-high-water marks and grows the lists before they fill up (``grow_at``), so an overflow needs a >20 % jump from one batch to
-the next.  ``redone`` / ``recaptures`` count what happened; bench.py fails if a timed step had to be redone.
+Capacities can never silently change the computation: every list records its real length on the device, and a step
+whose lists did not fit raises a device-side flag.  The flag is ``found_inf`` of the fused Adam and it is sticky: the
+overflowed step and every step replayed after it are exact no-ops (parameters, moments and step counters untouched)
+until the host has re-captured.  The host reads the flag ``lag`` steps later, re-captures the graph with larger lists
+and REDOES the overflowed step and every step launched after it, in launch order, each with its own batch, host randoms,
+scalars and ``after`` callback.  So the optimizer sees the same steps in the same order as without the overflow.  The
+host also watches the high-water marks and grows the lists before they fill up (``grow_at``), so an overflow needs a
+>20 % jump from one batch to the next.  ``redone`` / ``recaptures`` count what happened; bench.py fails if a timed step
+had to be redone.
 
 Numerics are those of the eager path except for (i) the device-side xyz-noise draw, which has the padded shape and
 therefore a different random stream, and (ii) atomics ordering.  Parity tests run the eager path.
@@ -74,20 +79,22 @@ class StaticTrainStep:
                        "overflow_step": torch.zeros((), dtype=torch.int64, device=dev),
                        "overflow": torch.zeros((), dtype=torch.int64, device=dev)}
         # found_inf of torch's fused / capturable Adam: 1.0 -> the whole update (parameters, moments, step counters)
-        # is skipped.  Raised by a list overflow, so an overflowed step leaves the model exactly as it was.
+        # is skipped.  Raised by a list overflow and kept by every later replay until capture() clears it, so an
+        # overflowed step and the steps behind it leave the model exactly as it was.  capture() also holds it at 1.0
+        # while it warms up: those eager executions must not train on whatever the input buffers hold.
         self.found_inf = torch.zeros((), dtype=torch.float32, device=dev)
-        # 1.0 while capture() warms up: those eager executions must not train on whatever the input buffers hold
-        self.force_skip = torch.zeros((), dtype=torch.float32, device=dev)
         self.graph = None
         self.loss = None
         self.launches_per_replay = 0
         self.redone = 0            # steps that overflowed (no-op on the device) and were executed again
         self.recaptures = 0        # graph re-captures with larger lists (overflow or high-water mark)
         self._step = 0
+        self._seq = 0              # launch order of the slots, redos included
         ring = self.lag + 1
         # ring of pinned staging slots: the host never rewrites a slot whose copies may still be in flight
         self._slots = [{"jitter": torch.zeros(n_rays, 1).pin_memory(), "dirs": torch.zeros(n_dirs, 3).pin_memory(),
-                        "stats": torch.zeros(5, dtype=torch.int64).pin_memory(), "event": None, "batch": None}
+                        "stats": torch.zeros(5, dtype=torch.int64).pin_memory(), "scalars": None, "event": None,
+                        "batch": None, "seq": 0}
                        for _ in range(ring)]
 
     # ------------------------------------------------------------------------------------------------ capacities
@@ -135,7 +142,7 @@ class StaticTrainStep:
         loss = self.loss_fn(ret, self.model)
         self.ret = ret                    # the captured forward's outputs: after a replay they hold that step's values
         loss.backward()
-        flag = torch.maximum((st["overflow_step"] > 0).to(torch.float32), self.force_skip)
+        flag = torch.maximum((st["overflow_step"] > 0).to(torch.float32), self.found_inf)
         if self.bucket is not None:
             # the flag rides in the bucket's spare slot: one rank's overflow makes every rank skip the same step
             self.bucket.extra[0].copy_(flag)
@@ -156,7 +163,7 @@ class StaticTrainStep:
         # during capture
         s = getattr(self, "_stream", None) or torch.cuda.Stream()
         self._stream = s
-        self.force_skip.fill_(1.0)
+        self.found_inf.fill_(1.0)
         s.wait_stream(torch.cuda.current_stream())
         # FusedAdam(clear_grad=True) keeps every gradient zeroed IN PLACE: the buffers created by the first warm-up step
         # are the ones the captured kernels accumulate into (no per-step allocation / memset / AccumulateGrad pass)
@@ -175,7 +182,7 @@ class StaticTrainStep:
         with torch.cuda.graph(self.graph, stream=s, capture_error_mode=capture_error_mode):
             self.loss = self._body()
         self.launches_per_replay = _lib.launch_count - l0
-        self.force_skip.zero_()
+        self.found_inf.zero_()
         self.static["overflow"].zero_()
         torch.cuda.synchronize()
         for slot in self._slots:
@@ -198,7 +205,13 @@ class StaticTrainStep:
         return (id(m.alphaMask), tuple((p.data_ptr(), tuple(p.shape)) for p in vm))
 
     # ------------------------------------------------------------------------------------------------ replay
-    def _launch(self, rays, light_idx, slot, target=None, seed=None):
+    def _launch(self, slot, rays, light_idx, target=None, seed=None, scalars=None, after=None):
+        if scalars is not None:
+            dst, values = scalars
+            if slot["scalars"] is None or slot["scalars"].shape != dst.shape:
+                slot["scalars"] = torch.zeros(dst.shape, dtype=dst.dtype).pin_memory()
+            slot["scalars"].copy_(values)
+            dst.copy_(slot["scalars"], non_blocking=True)
         self.rays.copy_(rays, non_blocking=True)
         self.light_idx.copy_(light_idx.reshape(-1, 1), non_blocking=True)
         if target is not None:
@@ -207,11 +220,14 @@ class StaticTrainStep:
             torch.manual_seed(seed)
         self._stage_host_randoms(slot)
         self.graph.replay()
+        if after is not None:
+            after()
         slot["stats"][:4].copy_(self.static["stats"], non_blocking=True)
         slot["stats"][4:5].copy_(self.static["overflow_step"].reshape(1), non_blocking=True)
         ev = torch.cuda.Event()
         ev.record()
-        slot["event"], slot["batch"] = ev, (rays, light_idx, target, seed)
+        self._seq += 1
+        slot["event"], slot["batch"], slot["seq"] = ev, (rays, light_idx, target, seed, scalars, after), self._seq
         mark_parameters_updated()        # the replayed optimizer step is invisible to the host-side bookkeeping
         _lib.launch_count += self.launches_per_replay
 
@@ -253,7 +269,8 @@ class StaticTrainStep:
 
     def _settle(self, slot):
         """Host-side follow-up of one finished step (read ``lag`` steps late): grow the lists when a high-water mark
-        came close to its capacity; an overflowed step (a no-op on the device) is redone after the re-capture."""
+        came close to its capacity.  After an overflow every later replay was a no-op too (the flag is sticky): the
+        overflowed step and all steps launched after it are redone in launch order after the re-capture."""
         if slot["event"] is None:
             return
         batch = slot["batch"]
@@ -262,27 +279,32 @@ class StaticTrainStep:
             grow = tuple(int(self.headroom * c) + 64 for c in self.capacities())
         if grow is not None:
             torch.cuda.synchronize()
-            pending = [s for s in self._slots if s["event"] is not None]
+            # steps launched after the inspected one, already finished, oldest first
+            pending = sorted((s for s in self._slots if s["event"] is not None), key=lambda s: s["seq"])
             redo = [batch] if over else []
-            for s in pending:                        # steps launched after the inspected one, already finished
+            for s in pending:
                 o, _ = self._inspect(s)
-                if o:
+                if o or redo:
                     redo.append(s["batch"])
             self._recapture(grow)
-            for rays, li, target, seed in redo:
+            for b in redo:
                 self.redone += 1
-                self._launch(rays, li, self._slots[0], target, seed)
+                self._launch(self._slots[0], *b)
                 self._settle_now(self._slots[0])
 
     def _settle_now(self, slot):
         torch.cuda.synchronize()
         self._settle(slot)
 
-    def run(self, rays, light_idx, target=None, seed=None):
+    def run(self, rays, light_idx, target=None, seed=None, scalars=None, after=None):
         """One training step.  ``rays`` / ``light_idx`` / ``target`` (copied into :attr:`target` for ``loss_fn``;
         None leaves it as it is) may live on the host (pinned) or on the device; they must stay unchanged for
         ``lag + 1`` further calls, since an overflowed step is redone from them.  With ``seed``, the step's host randoms
-        are drawn right after ``torch.manual_seed(seed)`` (a redo draws the same ones), whatever re-capture runs first."""
+        are drawn right after ``torch.manual_seed(seed)`` (a redo draws the same ones), whatever re-capture runs first.
+        ``scalars = (device_tensor, host_values)``: the step's per-iteration values (learning rates, loss weights),
+        copied into ``device_tensor`` through a pinned buffer of the step's own right before its replay, and again
+        before a redo.  ``after()`` is called right after every replay of this step, the redos included (e.g. to copy
+        the step's loss out of the graph's output buffers)."""
         if self.graph is None:
             raise RuntimeError("StaticTrainStep.run() before capture()")
         if self._model_signature() != self._captured_for:
@@ -291,7 +313,7 @@ class StaticTrainStep:
         slot = self._slots[self._step % len(self._slots)]
         self._settle(slot)                          # the step that used this slot `lag + 1` calls ago
         self._step += 1
-        self._launch(rays, light_idx, slot, target, seed)
+        self._launch(slot, rays, light_idx, target, seed, scalars, after)
         return self.loss
 
     def reserve(self, factor=2.0):
@@ -311,11 +333,11 @@ class StaticTrainStep:
         return self.capacities()
 
     def flush(self):
-        """Settle every step still in flight (end of training / before reading results that must be exact)."""
-        for _ in range(len(self._slots)):
-            for slot in self._slots:
-                if slot["event"] is not None:
-                    self._settle_now(slot)
+        """Settle every step still in flight, oldest first (end of training / before reading results that must be
+        exact)."""
+        n = len(self._slots)
+        for k in range(n):                          # the slot run() reuses next holds the oldest step
+            self._settle_now(self._slots[(self._step + k) % n])
 
     def scale_lr(self, factor: float):
         """The train loop's per-iteration decay ``param_group['lr'] = param_group['lr'] * lr_factor``
@@ -330,8 +352,8 @@ class StaticTrainStep:
             lr.mul_(factor)
 
     def overflowed(self) -> int:
-        """Number of replays whose lists exceeded the static capacities (each was a no-op and has been, or will be,
-        redone by ``run`` / ``flush``).  Host sync."""
+        """Number of replays whose own lists exceeded the static capacities (each was a no-op and has been, or will
+        be, redone by ``run`` / ``flush``, with the steps behind it).  Host sync."""
         return int(self.static["overflow"].item())
 
     def release(self):

@@ -6,8 +6,9 @@ are :class:`static_step.StaticTrainStep` captures: the radiance-only step (``is_
 iteration is one graph replay plus its input copies; nothing on the per-step path reads a device value back.
 
 * Every value the schedule changes between replays lives in device memory: the param groups' learning rates and the
-  TV / normal / BRDF weights are 0-dim views of one device vector, written from the schedule's float64 host values with
-  one host-to-device copy per iteration.  The L1 term is folded into :class:`optim.FusedAdam` (``density_l1``).
+  TV / normal / BRDF weights are 0-dim views of one device vector.  The step stages each iteration's float64 host
+  values into it with one host-to-device copy (``run(..., scalars=...)``), again when it redoes the iteration.  The L1
+  term is folded into :class:`optim.FusedAdam` (``density_l1``).
 * Batches come from the reference's :class:`schedule.SimpleSampler` on numpy's global stream, gathered on the host
   into a ring of pinned buffers.
 * The host randoms of iteration ``it`` (per-ray jitter, stratified light directions) are drawn right after
@@ -15,10 +16,10 @@ iteration is one graph replay plus its input copies; nothing on the per-step pat
   the graphed one.  The graphed step draws the xyz noise of the smoothness terms on the device with the padded list
   shape (static_step.py), so the two runs are not one random trajectory, and neither reproduces the reference run's
   random stream.
-* The loss terms of each step are copied into a device ring; the host reads the ring once per
-  ``progress_refresh_rate`` iterations for the progress line and the TensorBoard scalars.  A step that overflowed its
-  static lists is a no-op replay and is redone on the same batch (static_step.py); its ring row holds the values of the
-  overflowed attempt.
+* The loss terms of each step are copied into a device ring after each of its replays; the host flushes the step and
+  reads the ring once per ``progress_refresh_rate`` iterations for the progress line and the TensorBoard scalars.  A
+  step that overflowed its static lists, and every step launched after it, is a no-op replay and is redone in order on
+  the same batch (static_step.py); the redo rewrites the step's ring row, so the log holds the applied replay.
 * At a grid event: ``flush``, ``release``, the grid operation, a new optimizer when the reference makes one (only at an
   upsample; a mask update keeps it, :385-422), then a newly calibrated and captured step.  An evaluation or a
   checkpoint first flushes; an evaluation runs eager forwards on the model, so the step is captured again after it.
@@ -310,7 +311,6 @@ def reconstruction(args, train_dataset, test_dataset, logfolder, *, variant="ful
 
     # per-iteration host values -> one device vector: [lr of each group, tv_density, tv_app, normal, brdf factor]
     scal = torch.zeros(n_groups + 4, device=dev)
-    scal_host = [torch.zeros(n_groups + 4, dtype=torch.float32).pin_memory() for _ in range(RING)]
     w_dev = tuple(scal[n_groups + k] for k in range(4))
     ring = torch.zeros(args.progress_refresh_rate, len(TERMS), device=dev)
     losses = torch.zeros(args.n_iters, len(TERMS))
@@ -359,6 +359,8 @@ def reconstruction(args, train_dataset, test_dataset, logfolder, *, variant="ful
 
     def read_ring(upto):
         nonlocal read
+        if st is not None:
+            st.flush()                           # a redo rewrites its step's row
         rows = ring.cpu()                        # the one host sync of the logging path
         for i in range(read, upto + 1):
             losses[i] = rows[i % rate]
@@ -391,12 +393,11 @@ def reconstruction(args, train_dataset, test_dataset, logfolder, *, variant="ful
                 st = new_step(opt, w)
                 timer.add("capture", sync_time() - t0)
                 phase_t0 += time.perf_counter() - t0
-            host = scal_host[it % RING]
-            host.copy_(torch.tensor(list(w.lrs) + [w.tv_density, w.tv_app, w.normal_factor, w.brdf_factor],
-                                    dtype=torch.float64))
-            scal.copy_(host, non_blocking=True)
-            st.run(batch_rays, batch_li, batch_rgb, seed=SEED + it)
-            ring[it % rate].copy_(terms[0])        # the vector of the graph captured last (re-captures included)
+            host = torch.tensor(list(w.lrs) + [w.tv_density, w.tv_app, w.normal_factor, w.brdf_factor],
+                                dtype=torch.float64)
+            # terms[0]: the vector of the graph captured last (re-captures included)
+            st.run(batch_rays, batch_li, batch_rgb, seed=SEED + it, scalars=(scal, host),
+                   after=lambda row=ring[it % rate]: row.copy_(terms[0]))
         else:
             for g, lr in zip(opt.param_groups, w.lrs):
                 g['lr'] = lr
