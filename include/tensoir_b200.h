@@ -807,6 +807,54 @@ int tir_indirect_shade(const TirEnvMap* envs, int32_t n_lights, const float* ray
                        const float* Lo, int64_t m_h, float* with_bg, float* without_bg, float* indirect,
                        int64_t out_rows, int64_t row0, void* stream);
 
+/* ---- camera-path frames: rotated environment maps and a shadow-catching ground plane ---------------------------------
+ * Conventions.  Cameras are camera-to-world matrices in the OpenCV convention (x right, y down, z forward), as the
+ * datasets (transform_matrix @ blender2opencv) and tir_generate_rays use.  A map rotated by angle a turns about world +z
+ * with R(a) = [[cos a, -sin a, 0], [sin a, cos a, 0], [0, 0, 1]] (the reference's light_rotation matrix): the radiance
+ * arriving from world direction w is E(w @ R(a)), w a row vector, as the reference lights with
+ * init_light_directions @ rotation_matrix.  The object under a rotated map is shaded by tir_relight_sample and
+ * tir_relight_shade with the map's dir table replaced by dir @ R(a)^T (bins, rgb, pdf_return and cdf unchanged), which
+ * rotates their estimator exactly.
+ *
+ * The ground is the plane z = ground_z with normal +z, a shadow catcher: it receives the object's shadow but does not
+ * occlude or light the object.  Primary ray i has a ground point p = o + t d when d.z < 0 and t > 0 (never for a NaN
+ * ground_z); p.z is ground_z.
+ *   tir_ground_sample   per (map, ray, slot) of a ray with a ground point, u [L,n,S] fp64: bin = rl_bin of u in the
+ *                       map's CDF (as tir_relight_sample), w = dir[bin] of the (rotated) table, and
+ *                         pos = -1          when w.z <= 1e-6: the slot counts nowhere;
+ *                         pos = -2          when the shadow ray p + t w (t >= 0) misses the box [box_lo, box_hi]
+ *                                           (host [3] each; lo > hi on an axis: empty): unoccluded, not marched;
+ *                         pos = list row    otherwise: (p + max(t_enter - TIR_PATH_SHADOW_NEAR, 0) w, w) is appended,
+ *                                           so a march whose first sample is at TIR_PATH_SHADOW_NEAR starts at the box
+ *                                           entry.
+ *                       Rays without a ground point get bin 0, pos -1 in every slot.  count and capacity as in
+ *                       tir_relight_sample.  The box is the model's occupied-cell box (TirField.occ_lo/occ_hi, where
+ *                       the march finds every valid sample), or its aabb without an alpha mask: a shadow ray that misses
+ *                       it would march through no valid sample and see t_last 1, acc 0.
+ *   tir_march_density   on the list, by the caller, with a table from TIR_PATH_SHADOW_NEAR out past the box diagonal.
+ *   tir_path_composite  one warp per (map, pixel): r_c = sum E_c cos V / pdf / sum E_c cos / pdf over the ray's slots
+ *                       with pos != -1 (fixed lane order), E = rgb[bin], cos = w.z, pdf = pdf_return[bin], V = 1 for
+ *                       pos -2 and the march's visibility as tir_relight_shade reads it for pos >= 0; r clamped to
+ *                       [0, 1], 1 when the denominator is 0 and on rays without a ground point.  bg = get_light at
+ *                       d @ rot (rot = R(a), host [9] row-major, shared by the call's maps) times r per channel;
+ *                       with_bg = acc_t*without_bg + (1-acc_t)*sRGB(clamp(bg)), acc_t = acc > 0.9 ? acc : 0, with
+ *                       without_bg read from the same rows (tir_relight_shade's output).  shadow (NULL allowed) gets r.
+ *                       Rows are [l, row0 + i] of [L, out_rows, 3] maps.  With a NaN ground_z and rot the identity,
+ *                       with_bg has tir_relight_shade's bits; bin, pos and vis_list are then not read and may be NULL.
+ * The ratio is differential rendering with a diffuse receiver: both sums use the same samples, so an unoccluded point
+ * gets exactly 1.  Repeated calls on the same list give identical bits.  TIR_ERR_SHAPE for n < 0, S < 0 (S < 1 for the
+ * composite with a ground), more than TIR_RELIGHT_MAX_LIGHTS maps, capacity outside [0, INT32_MAX] or output rows out of
+ * range; TIR_ERR_CONFIG for an unknown vis_kind; TIR_ERR_NULL for a missing input. */
+#define TIR_PATH_SHADOW_NEAR 0.05f
+int tir_ground_sample(const TirEnvMap* envs /* host array [n_lights] */, int32_t n_lights, const float* rays, int64_t n,
+                      float ground_z, const float* box_lo /* host [3] */, const float* box_hi /* host [3] */,
+                      int32_t n_samples, const double* u /* [L,n,S] */, int32_t* bin, int32_t* pos, float* list_o,
+                      float* list_d /* [capacity,3] */, int64_t capacity, int64_t* count, void* stream);
+int tir_path_composite(const TirEnvMap* envs, int32_t n_lights, const float* rays, const float* acc, int64_t n,
+                       const float* rot /* host [9] */, float ground_z, const int32_t* bin, const int32_t* pos,
+                       const float* vis_list, int32_t vis_kind, int32_t n_samples, const float* without_bg,
+                       float* with_bg, float* shadow /* or NULL */, int64_t out_rows, int64_t row0, void* stream);
+
 /* ---- mesh export: marching cubes over a dense volume (utils.py:165-225, skimage.measure.marching_cubes on
  * TensorBase.getDenseAlpha(), tensorBase_rotated_lights.py:737-753) ---------------------------------------------------
  * volume [X,Y,Z] fp32 C-contiguous, X, Y, Z >= 2 and X*Y*Z <= INT32_MAX (TIR_ERR_SHAPE otherwise).  A point is inside

@@ -148,6 +148,8 @@ LIGHTS_MAX = 16           # TIR_LIGHTS_MAX
 LIGHT_SAMPLES_MAX = 1024  # TIR_LIGHT_SAMPLES_MAX
 LIGHT_DIRECTIONAL, LIGHT_POINT, LIGHT_SPOT = 0, 1, 2
 
+PATH_SHADOW_NEAR = 0.05     # TIR_PATH_SHADOW_NEAR (csrc/tir_path.cu)
+
 TRANSPORT_MAX_TEXELS = 2048  # TIR_TRANSPORT_MAX_TEXELS (csrc/tir_transport.cu)
 
 EXPORTS = {
@@ -280,6 +282,12 @@ EXPORTS = {
                                      C.c_int64, C.c_int32, C.c_float, f32p, C.c_void_p, C.c_void_p, f32p, C.c_int32,
                                      C.c_int32, f32p, C.c_void_p, f32p, f32p, C.c_int64, f32p, f32p, f32p, C.c_int64,
                                      C.c_int64, C.c_void_p]),
+    "tir_ground_sample": (C.c_int, [C.POINTER(TirEnvMap), C.c_int32, f32p, C.c_int64, C.c_float, C.POINTER(C.c_float),
+                                    C.POINTER(C.c_float), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, f32p, f32p,
+                                    C.c_int64, C.c_void_p, C.c_void_p]),
+    "tir_path_composite": (C.c_int, [C.POINTER(TirEnvMap), C.c_int32, f32p, f32p, C.c_int64, C.POINTER(C.c_float),
+                                     C.c_float, C.c_void_p, C.c_void_p, f32p, C.c_int32, C.c_int32, f32p, f32p, f32p,
+                                     C.c_int64, C.c_int64, C.c_void_p]),
     "tir_marching_cubes_work_size": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int64)]),
     "tir_marching_cubes_count": (C.c_int, [f32p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_int64,
                                            C.c_void_p, C.c_void_p]),
@@ -311,7 +319,8 @@ KERNELS_PER_CALL = {"tir_pack_channels_last": 1, "tir_unpack_channels_last_add":
                     "tir_transport_sample": 1, "tir_transport_build": 1,
                     "tir_indirect_sample": 1, "tir_indirect_hits": 3, "tir_indirect_radiance": 1,
                     "tir_indirect_shade": 1, "tir_marching_cubes_count": 7, "tir_marching_cubes_emit": 2,
-                    "tir_atlas_texels": 1, "tir_atlas_encode": 1, "tir_atlas_corners": 1}
+                    "tir_atlas_texels": 1, "tir_atlas_encode": 1, "tir_atlas_corners": 1,
+                    "tir_ground_sample": 1, "tir_path_composite": 1}
 launch_count = 0
 
 _lib = None
