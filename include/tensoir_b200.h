@@ -855,6 +855,48 @@ int tir_path_composite(const TirEnvMap* envs, int32_t n_lights, const float* ray
                        const float* vis_list, int32_t vis_kind, int32_t n_samples, const float* without_bg,
                        float* with_bg, float* shadow /* or NULL */, int64_t out_rows, int64_t row0, void* stream);
 
+/* The same ground under one setup of analytic lights (the TirLight table of tir_lights_sample; the object shaded by
+ * tir_lights_sample / tir_lights_shade).  Slots are laid out light-major as tir_lights_sample's, slot(j, i, s) =
+ * n * (K_0 + ... + K_{j-1}) + i * K_j + s, and read their uniforms under the same rule.
+ *   tir_ground_lights_sample   per slot of a ray with a ground point p: L and falloff of the light sample seen from p
+ *                              (as tir_lights_sample, spot cone and 1/d^2 included), g = falloff * L.z (the slot's
+ *                              unshadowed irradiance weight on the +z receiver), and
+ *                                pos = -1        when L.z <= 1e-6 or g <= 0: the slot counts nowhere;
+ *                                pos = -2        when the shadow ray p + t L misses the box, or, for a point or spot
+ *                                                light, enters it at t_enter >= |q - p|, the distance to the light
+ *                                                sample q: unoccluded, not marched;
+ *                                pos = list row  otherwise, appended as by tir_ground_sample.
+ *                              Rays without a ground point get g 0, pos -1 in every slot.  The box must lie inside the
+ *                              model's aabb (the occupied-cell box clipped to it) and every point or spot light sample
+ *                              outside the aabb: then a shadow ray that enters the box before the light also leaves it
+ *                              before the light, every valid march sample lies between p and the light, and the distance
+ *                              cull is exact.
+ *   tir_march_density          on the list, by the caller, as for tir_ground_sample.
+ *   tir_path_lights_composite  one warp per pixel: r_c = sum_j power_jc / K_j * sum_s g V  /  sum_j power_jc / K_j *
+ *                              sum_s g over the slots with pos != -1 (per light, lanes in a fixed order and the xor
+ *                              butterfly; lights in order), V as for tir_path_composite; r clamped to [0, 1], 1 when
+ *                              the denominator is 0 and on rays without a ground point.  bg_c = background_c where
+ *                              r_c == 1, else sRGB(clamp(background_linear_c * r_c)): background is the setup's display
+ *                              colour (host [3]), background_linear its linear value (host [3]), so the shadow darkens
+ *                              linear light.  with_bg = acc_t*without_bg + (1-acc_t)*bg, acc_t as in tir_lights_shade,
+ *                              without_bg read from the same rows (tir_lights_shade's output).  shadow (NULL allowed)
+ *                              gets r.  Rows are [row0 + i] of [out_rows, 3] maps.  With a NaN ground_z, with_bg has
+ *                              tir_lights_shade's bits; g, pos and vis_list are then not read and may be NULL.
+ * Both sums of the ratio use the same expressions in the same order, so an unoccluded point gets exactly 1.  Repeated
+ * calls on the same list give identical bits.  TIR_ERR_SHAPE for n < 0, more than TIR_LIGHTS_MAX lights, K outside
+ * [1, TIR_LIGHT_SAMPLES_MAX], more than INT32_MAX slots, capacity outside [0, INT32_MAX] or output rows out of range;
+ * TIR_ERR_CONFIG for an unknown light type or vis_kind; TIR_ERR_NULL for a missing input. */
+int tir_ground_lights_sample(const TirLight* lights /* host array [n_lights] */, int32_t n_lights, const float* rays,
+                             int64_t n, float ground_z, const float* box_lo /* host [3] */,
+                             const float* box_hi /* host [3] */, const double* u /* [slots,2] */, float* g /* [slots] */,
+                             int32_t* pos /* [slots] */, float* list_o, float* list_d /* [capacity,3] */,
+                             int64_t capacity, int64_t* count, void* stream);
+int tir_path_lights_composite(const TirLight* lights, int32_t n_lights, const float* rays, const float* acc, int64_t n,
+                              float ground_z, const float* background /* host [3] */,
+                              const float* background_linear /* host [3] */, const float* g, const int32_t* pos,
+                              const float* vis_list, int32_t vis_kind, const float* without_bg, float* with_bg,
+                              float* shadow /* or NULL */, int64_t out_rows, int64_t row0, void* stream);
+
 /* ---- mesh export: marching cubes over a dense volume (utils.py:165-225, skimage.measure.marching_cubes on
  * TensorBase.getDenseAlpha(), tensorBase_rotated_lights.py:737-753) ---------------------------------------------------
  * volume [X,Y,Z] fp32 C-contiguous, X, Y, Z >= 2 and X*Y*Z <= INT32_MAX (TIR_ERR_SHAPE otherwise).  A point is inside

@@ -288,6 +288,12 @@ EXPORTS = {
     "tir_path_composite": (C.c_int, [C.POINTER(TirEnvMap), C.c_int32, f32p, f32p, C.c_int64, C.POINTER(C.c_float),
                                      C.c_float, C.c_void_p, C.c_void_p, f32p, C.c_int32, C.c_int32, f32p, f32p, f32p,
                                      C.c_int64, C.c_int64, C.c_void_p]),
+    "tir_ground_lights_sample": (C.c_int, [C.POINTER(TirLight), C.c_int32, f32p, C.c_int64, C.c_float,
+                                           C.POINTER(C.c_float), C.POINTER(C.c_float), C.c_void_p, f32p, C.c_void_p,
+                                           f32p, f32p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "tir_path_lights_composite": (C.c_int, [C.POINTER(TirLight), C.c_int32, f32p, f32p, C.c_int64, C.c_float,
+                                            C.POINTER(C.c_float), C.POINTER(C.c_float), f32p, C.c_void_p, f32p,
+                                            C.c_int32, f32p, f32p, f32p, C.c_int64, C.c_int64, C.c_void_p]),
     "tir_marching_cubes_work_size": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_int64)]),
     "tir_marching_cubes_count": (C.c_int, [f32p, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_int64,
                                            C.c_void_p, C.c_void_p]),
@@ -320,7 +326,8 @@ KERNELS_PER_CALL = {"tir_pack_channels_last": 1, "tir_unpack_channels_last_add":
                     "tir_indirect_sample": 1, "tir_indirect_hits": 3, "tir_indirect_radiance": 1,
                     "tir_indirect_shade": 1, "tir_marching_cubes_count": 7, "tir_marching_cubes_emit": 2,
                     "tir_atlas_texels": 1, "tir_atlas_encode": 1, "tir_atlas_corners": 1,
-                    "tir_ground_sample": 1, "tir_path_composite": 1}
+                    "tir_ground_sample": 1, "tir_path_composite": 1,
+                    "tir_ground_lights_sample": 1, "tir_path_lights_composite": 1}
 launch_count = 0
 
 _lib = None

@@ -14,10 +14,17 @@ ground, tir_ground_sample turns each ground pixel's light samples into shadow ra
 the density march gives their visibility, and tir_path_composite writes the frame: the rotated background, darkened by
 the ground's shadow ratio, under the object.  The estimators that look texels up by direction (MIS and the indirect
 bounce) are not rotated by a direction table and are rejected.
+
+Under a rig of analytic lights (lighting.load_rig) instead of maps, each setup is turned per frame (``rotated_setup``:
+a light authored at direction d or position p ends up at R(a) d, R(a) p, as a map's texel does), the object is shaded
+by lighting.rig_visibility in slot order and lighting.rig_shade, and with a ground tir_ground_lights_sample and
+tir_path_lights_composite do for the lights' samples what the two map entries do for texels, over the setup's
+background colour (``render_rig_frame``).
 """
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
 import json
 import math
 import os
@@ -27,7 +34,10 @@ import torch
 
 from . import _lib, ops
 from . import relighting as R
-from .lighting import SEED, SHADOW_NEAR, SHADOW_STEP, shadow_table
+from .light_fit import srgb_to_linear
+from .lighting import (SEED, SHADOW_NEAR, SHADOW_STEP, check_outside, default_shadow_far, light_table, load_rig,
+                       rig_shade, rig_visibility, shadow_table, slots_per_ray)
+from .lighting import _uniforms as rig_uniforms
 
 NUM_SAMPLES = R.NUM_SAMPLES
 
@@ -145,6 +155,38 @@ def rotated_env_tables(envir_light, light_names, angle):
     return arr, keep
 
 
+# ---- rotated light rigs ---------------------------------------------------------------------------------------------
+
+def rotated_setup(setup, angle):
+    """The lighting.Setup ``setup`` turned by ``angle`` degrees about +z under the maps' convention: a map rotated by a
+    gives E(w @ R(a)), so a light authored at direction d (position p, spot axis) ends up at R(a) d (column vector),
+    R = rotation_matrix(angle).  The product is taken in float64 from R's fp32 entries and rounded to fp32 once, by
+    lighting.light_table, with no renormalisation; angle 0 leaves every value as it is."""
+    m = rotation_matrix(angle).double().tolist()
+
+    def turn(v):
+        return tuple(m[i][0] * v[0] + m[i][1] * v[1] + m[i][2] * v[2] for i in range(3))
+
+    return dataclasses.replace(setup, lights=tuple(dataclasses.replace(l, direction=turn(l.direction),
+                                                                       position=turn(l.position))
+                                                   for l in setup.lights))
+
+
+def frame_rigs(rig, angles, aabb):
+    """The rig ``rig`` ({name: Setup}) turned by each frame's angle -> a list of {name: Setup}, one per frame.
+    ValueError naming the frame, the setup and the light when a turned point or spot light does not clear ``aabb``
+    (lighting.check_outside): a box that is not a cube can swallow a light that clears it unturned."""
+    out = []
+    for f, a in enumerate(angles):
+        turned = {name: rotated_setup(s, a) for name, s in rig.items()}
+        try:
+            check_outside(turned, aabb)
+        except ValueError as e:
+            raise ValueError(f"frame {f} (rotation {a:g} degrees): {e}") from None
+        out.append(turned)
+    return out
+
+
 # ---- the ground -----------------------------------------------------------------------------------------------------
 
 def ground_box(tensoIR):
@@ -207,6 +249,54 @@ def path_composite(envs, L, rays, acc, angle, ground_z, visibility, num_samples,
                                       R.vis_kind(vis_equation), int(num_samples), _lib.dptr(without_bg),
                                       _lib.dptr(with_bg), _lib.dptr(shadow, allow_none=True), int(with_bg.shape[1]),
                                       int(row0), _lib.stream_ptr()), "tir_path_composite")
+
+
+def rig_ground_box(tensoIR):
+    """ground_box clipped to the model's aabb: the box of tir_ground_lights_sample.  Every point or spot light lies
+    outside the aabb (lighting.check_outside), so a shadow ray that enters this box before the light also leaves it
+    before the light, which makes the distance cull exact (DESIGN §3.8)."""
+    lo, hi = ground_box(tensoIR)
+    a_lo, a_hi = tensoIR.aabb.detach().float().cpu().tolist()
+    return [max(x, y) for x, y in zip(lo, a_lo)], [min(x, y) for x, y in zip(hi, a_hi)]
+
+
+def ground_lights_visibility(tensoIR, setup, rays, ground_z, box, u, vis_equation, z_table):
+    """tir_ground_lights_sample for one lighting.Setup, the list in slot order, and its march.  Inputs are contiguous
+    device tensors (rays fp32 [n,6], u fp64 [n * slots_per_ray, 2]).  -> (g, pos, vis), what path_lights_composite
+    reads."""
+    lib = _lib.load()
+    dev = rays.device
+    n = int(rays.shape[0])
+    slots = n * slots_per_ray(setup)
+    if tuple(u.shape) != (slots, 2) or u.dtype != torch.float64:
+        raise ValueError(f"u must be float64 [{slots}, 2], got {u.dtype} {tuple(u.shape)}")
+    g = torch.empty(slots, device=dev)
+    pos = torch.empty(slots, dtype=torch.int32, device=dev)
+    list_o, list_d = R.append_list(
+        slots, dev, "ground visibility list", pos,
+        lambda *tail: _lib.check(lib.tir_ground_lights_sample(
+            light_table(setup), len(setup.lights), _lib.dptr(rays), n, float(ground_z), _c3(box[0]), _c3(box[1]),
+            _lib.dptr(u, torch.float64), _lib.dptr(g), _lib.dptr(pos, torch.int32), *tail, _lib.stream_ptr()),
+            "tir_ground_lights_sample"))
+    return g, pos, R.march_list(tensoIR, list_o, list_d, vis_equation, z_table)
+
+
+def path_lights_composite(setup, rays, acc, ground_z, visibility, vis_equation, out, row0, shadow=None):
+    """tir_path_lights_composite of the chunk's rows into out = (with_bg, without_bg) [R, 3] at rows row0..
+    (without_bg already shaded by lighting.rig_shade) over the setup's background colour, which the shadow darkens in
+    linear light (light_fit.srgb_to_linear, float64).  ``ground_z`` None: no ground (``visibility`` unused); else
+    ``visibility`` = ground_lights_visibility's result.  ``shadow`` [R, 3] or None gets the shadow ratio."""
+    lib = _lib.load()
+    with_bg, without_bg = out
+    assert with_bg.is_contiguous() and without_bg.is_contiguous()
+    gz = float("nan") if ground_z is None else float(ground_z)
+    g, pos, vis = visibility if ground_z is not None else (None, None, None)
+    _lib.check(lib.tir_path_lights_composite(
+        light_table(setup), len(setup.lights), _lib.dptr(rays), _lib.dptr(acc), int(rays.shape[0]), gz,
+        _c3(setup.background), _c3(srgb_to_linear(list(setup.background)).tolist()), _lib.dptr(g, allow_none=True),
+        _lib.dptr(pos, torch.int32, allow_none=True), _lib.dptr(vis, allow_none=True), R.vis_kind(vis_equation),
+        _lib.dptr(without_bg), _lib.dptr(with_bg), _lib.dptr(shadow, allow_none=True), int(with_bg.shape[0]),
+        int(row0), _lib.stream_ptr()), "tir_path_lights_composite")
 
 
 def check_estimator(args):
@@ -318,6 +408,53 @@ def render_frame(tensoIR, env, names, rays_f, angle, rescale, batch_size, genera
     return with_map, without_map, shadow_map
 
 
+@torch.no_grad()
+def render_rig_frame(tensoIR, rig, rays_f, rescale, batch_size, generator, seed, ground_z=None, box=None,
+                     acc_mask_threshold=0.5, vis_equation="nerv", shadow_table_z=None, shadow=False, timer=None):
+    """One frame of every setup of ``rig`` ({name: lighting.Setup}, already turned for the frame: frame_rigs) from
+    the rays ``rays_f`` [n,6], as render_frame is for maps.  ``generator`` is re-seeded with ``seed`` first; per chunk
+    and setup the object's uniforms [n * slots, 2] are drawn, then, with a ground, the ground's.  ``box``:
+    rig_ground_box (default the model's).  ``shadow_table_z``: the object's shadow march (lighting.shadow_table,
+    default out to the aabb diagonal).  ``timer(phase)`` as render_frame's.  -> (with_bg, without_bg, shadow ratio or
+    None) [setups, n, 3]."""
+    dev = rays_f.device
+    names = list(rig)
+    n_pix = int(rays_f.shape[0])
+    tick = timer or (lambda phase: None)
+    z_obj = shadow_table(default_shadow_far(tensoIR), dev) if shadow_table_z is None else shadow_table_z
+    if ground_z is not None:
+        box = rig_ground_box(tensoIR) if box is None else box
+        z_ground = ground_table(box, dev)
+    generator.manual_seed(int(seed))
+    with_map = torch.empty(len(names), n_pix, 3, device=dev)
+    without_map = torch.empty(len(names), n_pix, 3, device=dev)
+    shadow_map = torch.empty(len(names), n_pix, 3, device=dev) if shadow else None
+    for s, e, (_, depth, normal, albedo, rough, fresnel, acc, *_) in R._primary_chunks(tensoIR, rays_f, batch_size):
+        rays, (depth, normal, albedo, rough, fresnel, acc) = R.chunk_inputs(rays_f[s:e],
+                                                                            (depth, normal, albedo, rough, fresnel,
+                                                                             acc))
+        tick("primary")
+        for k, name in enumerate(names):
+            setup = rig[name]
+            slots = (e - s) * slots_per_ray(setup)
+            u = rig_uniforms(slots, dev, generator)
+            ug = rig_uniforms(slots, dev, generator) if ground_z is not None else None
+            vis = rig_visibility(tensoIR, setup, rays, depth, normal, acc, u, acc_mask_threshold, vis_equation, z_obj,
+                                 ordered=True)
+            tick("object_visibility")
+            rig_shade(setup, rays, normal, albedo, rough, fresnel, acc, acc_mask_threshold, rescale, vis,
+                      vis_equation, (with_map[k], without_map[k], None), s)
+            tick("object_shade")
+            gvis = None
+            if ground_z is not None:
+                gvis = ground_lights_visibility(tensoIR, setup, rays, ground_z, box, ug, vis_equation, z_ground)
+                tick("ground")
+            path_lights_composite(setup, rays, acc, ground_z, gvis, vis_equation, (with_map[k], without_map[k]), s,
+                                  None if shadow_map is None else shadow_map[k])
+            tick("composite")
+    return with_map, without_map, shadow_map
+
+
 def _write_frame(out, names, f, H, W, with_map, without_map):
     """{out}/{map}/with_bg/{f:04d}.png and without_bg/{f:04d}.png of [L, H*W, 3] maps (relighting._write_pairs'
     encoding)."""
@@ -330,26 +467,43 @@ def _write_frame(out, names, f, H, W, with_map, without_map):
 
 
 @torch.no_grad()
-def render_path(dataset, args, poses, angles, tensoIR=None, ground_z=None):
+def render_path(dataset, args, poses, angles, tensoIR=None, ground_z=None, rig=None):
     """Render the cameras ``poses`` [F,4,4] (OpenCV c2w) with the maps rotated by ``angles`` [F] degrees.
-    ``dataset`` gives img_wh and the focal length (dataset_focal) and, for the maps of args.hdrdir, what
+    ``dataset`` gives img_wh and the focal length (dataset_focal) and, for the maps of args.hdrdir or a rig, what
     compute_rescale_ratio reads; ``args`` needs ckpt (when ``tensoIR`` is None), out and batch_size, and may carry
     hdrdir, light ('learned'), seed (lighting.SEED), acc_mask_threshold, vis_equation and render_video.  ``ground_z``: the height of the
     shadow-catching ground plane, True for the bottom of the occupied-cell box, None for no ground.
     Writes {out}/{map}/with_bg/{f:04d}.png and without_bg/{f:04d}.png per frame and, with imageio, {out}/{map}.mp4 of
-    with_bg.  ValueError for MIS, indirect light, or learned lights of a general multi-light model."""
+    with_bg.  ``rig`` (whatever lighting.load_rig takes): light the frames with its setups instead, turned by
+    ``angles`` (frame_rigs), over each setup's background colour, the albedo scaled by compute_rescale_ratio and the
+    object's shadow rays marched to args.shadow_far (default the aabb diagonal); images go to {out}/{setup}/... and
+    {out}/{setup}.mp4 and hdrdir is not read.  ValueError for MIS, indirect light, learned lights of a general
+    multi-light model, a rig with light 'learned', or a turned light inside the aabb."""
     check_estimator(args)
     poses = torch.as_tensor(poses, dtype=torch.float32).reshape(-1, 4, 4)
     angles = [float(a) for a in angles]
     if len(angles) != poses.shape[0]:
         raise ValueError(f"{poses.shape[0]} poses but {len(angles)} angles")
+    if rig is not None:
+        if getattr(args, "light", None) is not None:
+            raise ValueError(f"a rig lights the frames itself: light must be unset, got {args.light!r}")
+        rig = load_rig(rig)
     tensoIR, device = R._model(args, tensoIR)
     if tensoIR is None:
         return
     thr = float(getattr(args, "acc_mask_threshold", R.SCRIPT_DEFAULTS["acc_mask_threshold"]))
     vis_eq = getattr(args, "vis_equation", R.SCRIPT_DEFAULTS["vis_equation"])
     R.vis_kind(vis_eq)
-    env, names, rescale = path_maps(args, tensoIR, dataset)
+    if rig is None:
+        env, names, rescale = path_maps(args, tensoIR, dataset)
+    else:
+        from .evaluation import compute_rescale_ratio
+        rigs = frame_rigs(rig, angles, tensoIR.aabb)
+        names = list(rig)
+        far = getattr(args, "shadow_far", None)
+        z_obj = shadow_table(default_shadow_far(tensoIR) if far is None else far, device)
+        _, rescale = compute_rescale_ratio(tensoIR, dataset)
+        rescale = torch.as_tensor(rescale, dtype=torch.float32).to(device)
     if ground_z is True:
         ground_z = default_ground_z(tensoIR)
     seed = getattr(args, "seed", None)
@@ -358,11 +512,19 @@ def render_path(dataset, args, poses, angles, tensoIR=None, ground_z=None):
     W, H = dataset.img_wh
     focal = dataset_focal(dataset)
     out = args.out
-    box = ground_box(tensoIR) if ground_z is not None else None
+    box = None
+    if ground_z is not None:
+        box = ground_box(tensoIR) if rig is None else rig_ground_box(tensoIR)
     for f in range(poses.shape[0]):
         rays_f = frame_rays(poses[f], W, H, focal, device)
-        with_map, without_map, _ = render_frame(tensoIR, env, names, rays_f, angles[f], rescale, args.batch_size, gen,
-                                                seed, ground_z, box, acc_mask_threshold=thr, vis_equation=vis_eq)
+        if rig is None:
+            with_map, without_map, _ = render_frame(tensoIR, env, names, rays_f, angles[f], rescale, args.batch_size,
+                                                    gen, seed, ground_z, box, acc_mask_threshold=thr,
+                                                    vis_equation=vis_eq)
+        else:
+            with_map, without_map, _ = render_rig_frame(tensoIR, rigs[f], rays_f, rescale, args.batch_size, gen, seed,
+                                                        ground_z, box, acc_mask_threshold=thr, vis_equation=vis_eq,
+                                                        shadow_table_z=z_obj)
         _write_frame(out, names, f, H, W, with_map, without_map)
     if getattr(args, "render_video", True):
         for name in names:

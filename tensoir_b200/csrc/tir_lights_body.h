@@ -58,8 +58,10 @@ RL_HD void lt_on_disc(const float c[3], const float w[3], float r, float x, floa
 }
 
 // The sample of light l seen from the surface point p: unit direction L and falloff (see the header).  u is read only
-// when the light has an extent and more than one sample.
-RL_HD void lt_sample(const TirLight& l, const float p[3], const double* u, float L[3], float& falloff) {
+// when the light has an extent and more than one sample.  dist2, when given, gets the squared distance from p to the
+// sample of a point or spot light; it is left alone for a directional light.
+RL_HD void lt_sample(const TirLight& l, const float p[3], const double* u, float L[3], float& falloff,
+                     float* dist2 = nullptr) {
   float x = 0.f, y = 0.f;
   const bool centre = lt_centre_only(l);
   if (!centre) lt_disc(u[0], u[1], x, y);
@@ -84,6 +86,7 @@ RL_HD void lt_sample(const TirLight& l, const float p[3], const double* u, float
   }
   for (int e = 0; e < 3; ++e) w[e] = ev_sub(q[e], p[e]);
   const float d2 = lt_dot(w, w);
+  if (dist2) *dist2 = d2;
   ev_normalize(w, L);
   float cone = 1.f;
   if (l.type == TIR_LIGHT_SPOT) {

@@ -2,8 +2,9 @@
 // rotated environment map (semantics in include/tensoir_b200.h, "camera-path frames").  Shared by the CUDA kernels
 // (tir_path.cu) and by a host build (tests/host_path.cpp) that the CPU tests drive and the GPU tests compare with.  The
 // inverse-CDF bin, the background lookup, the visibility read and the tone map are the environment-map pass's
-// (tir_relight_body.h).
+// (tir_relight_body.h).  The ground under analytic lights takes its light samples from tir_lights_body.h.
 #pragma once
+#include "tir_lights_body.h"
 #include "tir_relight_body.h"
 
 // The ground point of a primary ray (o, d): p = o + t d on the plane z = ground_z, when d.z < 0 and t > 0.  A NaN
@@ -96,8 +97,83 @@ RL_HD void pt_composite(const TirEnvMap& e, const float* ray, const float* rot, 
     with_bg[c] = ev_add(ev_mul(acc_t, wo[c]), ev_mul(ev_sub(1.f, acc_t), tir::tone(ev_mul(bg[c], r[c]), 1)));
 }
 
+// ---- the ground under analytic lights ----
+
+// One ground slot of light l: from the ground point p, the light sample's direction L, its weight g = falloff * L.z
+// and, for a point or spot light, the squared distance d2 from p to the sample.  -> -1 when L.z <= 1e-6 or g <= 0
+// (counts nowhere), -2 when the shadow ray p + t L misses the box or, for a point or spot light, enters it at or beyond
+// the light sample (unoccluded, not marched), 0 when it is marched from o, as pt_ground_slot.
+RL_HD int pt_light_slot(const TirLight& l, const float p[3], const float L[3], float g, float d2, const float lo[3],
+                        const float hi[3], float o[3]) {
+  if (!(L[2] > 1e-6f) || !(g > 0.f)) return -1;
+  float te;
+  if (!pt_slab(p, L, lo, hi, te)) return -2;
+  if (l.type != TIR_LIGHT_DIRECTIONAL && te >= sqrtf(d2)) return -2;
+  const float s = fmaxf(ev_sub(te, TIR_PATH_SHADOW_NEAR), 0.f);
+  for (int c = 0; c < 3; ++c) o[c] = ev_add(p[c], ev_mul(s, L[c]));
+  return 0;
+}
+
+// The ground's per-slot sums of one (light, ground point) over its K slots: lane `lane` of `lanes` adds slots lane,
+// lane + lanes, ... with pos != -1 to num += g V and den += g, V = 1 for pos -2 and the march's visibility for rows.
+// Reduced as pt_shadow_lane's sums are.
+RL_HD void pt_light_lane(const float* g, const int32_t* pos, const float* vis_list, int vis_kind, int K, int lane,
+                         int lanes, float& num, float& den) {
+  for (int s = lane; s < K; s += lanes) {
+    const int q = pos[s];
+    if (q == -1) continue;
+    const float v = q >= 0 ? rl_vis(vis_list, vis_kind, q) : 1.f;
+    num = ev_add(num, ev_mul(g[s], v));
+    den = ev_add(den, g[s]);
+  }
+}
+
+// One light's reduced sums added to the ratio's per-channel sums: power_c times the mean over its K slots, the same
+// expression for both, so that num == den when every V is 1
+RL_HD void pt_light_add(const TirLight& l, int K, float sn, float sd, float num[3], float den[3]) {
+  for (int c = 0; c < 3; ++c) {
+    num[c] = ev_add(num[c], ev_mul(l.power[c], ev_div(sn, (float)K)));
+    den[c] = ev_add(den[c], ev_mul(l.power[c], ev_div(sd, (float)K)));
+  }
+}
+
+// One output row under a setup of lights: the setup's display background where the ratio is 1, else the linear
+// background times r, tone-mapped; composited under the object with lt_finish's expression
+RL_HD void pt_lights_composite(const float* background, const float* background_linear, float acc, const float wo[3],
+                               const float r[3], float with_bg[3]) {
+  const float acc_t = acc <= 0.9f ? 0.f : acc;
+  for (int c = 0; c < 3; ++c) {
+    const float bg = r[c] == 1.f ? background[c] : tir::tone(ev_mul(background_linear[c], r[c]), 1);
+    with_bg[c] = ev_add(ev_mul(acc_t, wo[c]), ev_mul(ev_sub(1.f, acc_t), bg));
+  }
+}
+
 // The whole argument check of each entry, run by tir_path.cu and its host build before their launch / loop:
-// 1 run, 0 nothing to do, < 0 TirStatus
+// 1 run, 0 nothing to do, < 0 TirStatus.  The lights' checks also fill the table.
+inline int pt_lights_sample_check(const TirLight* lights, int32_t n_lights, const float* rays, int64_t n,
+                                  const float* box_lo, const float* box_hi, const double* u, const float* g,
+                                  const int32_t* pos, const float* list_o, const float* list_d, int64_t capacity,
+                                  const int64_t* count, LightTable& t) {
+  const int rc = lt_validate(lights, n_lights, n, t);
+  if (rc <= 0) return rc;
+  if (!rays || !box_lo || !box_hi || !u || !g || !pos || !count) return TIR_ERR_NULL;
+  const int lrc = rl_check_list(capacity, list_o, list_d);
+  return lrc ? lrc : 1;
+}
+
+inline int pt_lights_composite_check(const TirLight* lights, int32_t n_lights, const float* rays, const float* acc,
+                                     int64_t n, float ground_z, const float* background,
+                                     const float* background_linear, const float* g, const int32_t* pos,
+                                     const float* vis_list, int32_t vis_kind, const float* without_bg,
+                                     const float* with_bg, int64_t out_rows, int64_t row0, LightTable& t) {
+  const int rc = lt_validate(lights, n_lights, n, t);
+  if (rc <= 0) return rc;
+  if (!rays || !acc || !background || !background_linear || !without_bg || !with_bg) return TIR_ERR_NULL;
+  if (!isnan(ground_z) && (!g || !pos || !vis_list)) return TIR_ERR_NULL;
+  const int wrc = rl_check_window(1, vis_kind, n, out_rows, row0);
+  return wrc ? wrc : 1;
+}
+
 inline int pt_sample_check(const TirEnvMap* envs, int32_t n_lights, const float* rays, int64_t n,
                            const float* box_lo, const float* box_hi, int32_t n_samples, const double* u,
                            const int32_t* bin, const int32_t* pos, const float* list_o, const float* list_d,

@@ -229,9 +229,10 @@ def _uniforms(slots, device, generator=None):
     return torch.rand(slots, 2, device=device, dtype=torch.float64, generator=generator)
 
 
-def rig_sample(setup, rays, depth, normal, acc, u, acc_mask_threshold):
+def rig_sample(setup, rays, depth, normal, acc, u, acc_mask_threshold, ordered=False):
     """tir_lights_sample on contiguous fp32 device tensors (u fp64 [slots, 2]) -> (L, falloff, pos, list_o, list_d)
-    with the list cut to its length, which is the one host read of the chunk."""
+    with the list cut to its length, which is the one host read of the chunk.  ``ordered``: the list in slot order
+    (relighting.slot_order)."""
     lib = _lib.load()
     dev = rays.device
     n = int(rays.shape[0])
@@ -243,7 +244,7 @@ def rig_sample(setup, rays, depth, normal, acc, u, acc_mask_threshold):
     falloff = torch.empty(slots, device=dev)
     pos = torch.empty(slots, dtype=torch.int32, device=dev)
     list_o, list_d = R.append_list(
-        slots, dev, "shadow-ray list", None,
+        slots, dev, "shadow-ray list", pos if ordered else None,
         lambda *tail: _lib.check(lib.tir_lights_sample(
             light_table(setup), len(setup.lights), _lib.dptr(rays), _lib.dptr(depth), _lib.dptr(normal),
             _lib.dptr(acc), n, float(acc_mask_threshold), _lib.dptr(u, torch.float64), _lib.dptr(L),
@@ -251,9 +252,11 @@ def rig_sample(setup, rays, depth, normal, acc, u, acc_mask_threshold):
     return L, falloff, pos, list_o, list_d
 
 
-def rig_visibility(tensoIR, setup, rays, depth, normal, acc, u, acc_mask_threshold, vis_equation, z_table):
-    """The material-independent half of relight_chunk_rig -> (L, falloff, pos, vis), what rig_shade reads."""
-    L, falloff, pos, list_o, list_d = rig_sample(setup, rays, depth, normal, acc, u, acc_mask_threshold)
+def rig_visibility(tensoIR, setup, rays, depth, normal, acc, u, acc_mask_threshold, vis_equation, z_table,
+                   ordered=False):
+    """The material-independent half of relight_chunk_rig -> (L, falloff, pos, vis), what rig_shade reads.
+    ``ordered``: march the list in slot order (relighting.slot_order)."""
+    L, falloff, pos, list_o, list_d = rig_sample(setup, rays, depth, normal, acc, u, acc_mask_threshold, ordered)
     return L, falloff, pos, R.march_list(tensoIR, list_o, list_d, vis_equation, z_table)
 
 

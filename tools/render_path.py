@@ -1,8 +1,9 @@
 """Render a relit camera-path video of a checkpoint with the command line of tools/relight_importance.py
 (opt.config_parser, the same seed and dataset), calling tensoir_b200.camera_path.render_path: every frame is rendered
-once per environment map of --hdrdir (or per learned light with --light learned), from cameras that need not be dataset
-views, with the maps rotated per frame and, with --ground, a ground plane that catches the object's shadow.  Run it with
-a TensoIR checkout on PYTHONPATH (for opt and dataLoader):
+once per environment map of --hdrdir (or per learned light with --light learned, or per setup of an analytic light rig
+with --rig), from cameras that need not be dataset views, with the maps or lights rotated per frame and, with --ground,
+a ground plane that catches the object's shadow.  Run it with a TensoIR checkout on PYTHONPATH (for opt and
+dataLoader):
 
     PYTHONPATH=<TensoIR checkout>:. python tools/render_path.py --config <config> --ckpt <ckpt> \\
         --hdrdir <dir of .hdr maps> --geo_buffer_path <dir> --out <dir> --path orbit --frames 120 \\
@@ -17,10 +18,14 @@ Options (besides relight_importance.py's):
   --ground [z]                    a shadow-catching ground plane at height z (default: the bottom of the model's
                                   occupied box)
   --light learned                 the model's own learned lights instead of --hdrdir
-  --out <dir>                     {out}/{map}/with_bg/{frame:04d}.png, without_bg/..., {out}/{map}.mp4
+  --rig <rig.json>                the setups of an analytic light rig (README, "Analytic lights") instead of maps,
+                                  each over its background colour; --env_rotation turns the lights about +z as it
+                                  turns a map; not with --light
+  --shadow_far <d>                with --rig: how far the object's shadow rays are marched (default: the aabb diagonal)
+  --out <dir>                     {out}/{map or setup}/with_bg/{frame:04d}.png, without_bg/..., {out}/{map or setup}.mp4
 
---path orbit --env_rotation 0:360 turns the camera and the map together, so the background stands still while the
-object turns: a turntable.
+--path orbit --env_rotation 0:360 turns the camera and the map (or the rig) together, so the background and the
+lighting stand still while the object turns: a turntable.
 """
 import os
 import sys
@@ -35,7 +40,8 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from relight_lights import pop_option  # noqa: E402
 
 USAGE = ("usage: render_path.py <relight_importance.py options> --out <dir> [--path orbit|test|<poses.json>] "
-         "[--frames N (orbit only)] [--env_rotation a0:a1] [--ground [z]] [--light learned]")
+         "[--frames N (orbit only)] [--env_rotation a0:a1] [--ground [z]] "
+         "[--light learned | --rig <rig.json> [--shadow_far d]]")
 
 
 def path_options(argv):
@@ -76,6 +82,24 @@ def path_options(argv):
                 out=out)
 
 
+def rig_options(argv):
+    """Remove --rig and --shadow_far from argv -> dict(rig=None | path, shadow_far=None | d).  Run before
+    path_options, which removes --light.  SystemExit with the usage for a rig file that does not exist, --rig with
+    --light, --shadow_far without --rig, or a shadow_far that is not a finite number above the shadow march's near."""
+    from tensoir_b200.lighting import SHADOW_NEAR
+    rig = pop_option(argv, "--rig")
+    far = pop_option(argv, "--shadow_far", float)
+    if rig is not None and not os.path.isfile(rig):
+        raise SystemExit(f"--rig: no such file {rig!r}\n{USAGE}")
+    if rig is not None and "--light" in argv:
+        raise SystemExit(f"--rig lights the frames itself: it does not take --light\n{USAGE}")
+    if far is not None and rig is None:
+        raise SystemExit(f"--shadow_far sets the march of a rig's shadow rays: it needs --rig\n{USAGE}")
+    if far is not None and not (np.isfinite(far) and far > SHADOW_NEAR):
+        raise SystemExit(f"--shadow_far must be a finite distance above {SHADOW_NEAR}, got {far}\n{USAGE}")
+    return dict(rig=rig, shadow_far=far)
+
+
 def path_poses(opts, dataset, tensoIR):
     """The cameras of opts['path'] -> float32 [F,4,4]."""
     from tensoir_b200 import camera_path as P
@@ -91,6 +115,7 @@ def path_poses(opts, dataset, tensoIR):
 
 
 if __name__ == "__main__":
+    rig_opts = rig_options(sys.argv)
     opts = path_options(sys.argv)
     if not torch.cuda.is_available():
         raise SystemExit("render_path.py needs a CUDA device: tensoir_b200 has no CPU fallback")
@@ -118,6 +143,7 @@ if __name__ == "__main__":
     args.seed = SEED
     args.out = opts["out"]
     args.light = opts["light"]
+    args.shadow_far = rig_opts["shadow_far"]
 
     dataset = dataset_dict[args.dataset_name]
     # the relighting test set needs the names of ground-truth images to load; its cameras, rays and albedo are used
@@ -130,6 +156,6 @@ if __name__ == "__main__":
         raise SystemExit(1)
     poses = path_poses(opts, test_dataset, model)
     angles = P.frame_angles(poses.shape[0], opts["rotation"])
-    print(f"{poses.shape[0]} frames, map rotation {opts['rotation'][0]} -> {opts['rotation'][1]} degrees, ground "
-          f"{'off' if opts['ground'] is None else opts['ground']}")
-    P.render_path(test_dataset, args, poses, angles, tensoIR=model, ground_z=opts["ground"])
+    print(f"{poses.shape[0]} frames, {'rig' if rig_opts['rig'] else 'map'} rotation {opts['rotation'][0]} -> "
+          f"{opts['rotation'][1]} degrees, ground {'off' if opts['ground'] is None else opts['ground']}")
+    P.render_path(test_dataset, args, poses, angles, tensoIR=model, ground_z=opts["ground"], rig=rig_opts["rig"])
