@@ -30,16 +30,23 @@ def _grid(model):
     return list(ops.device_field(model).refresh(model).grid)
 
 
-def _d64(factors, lo, n):
-    """sum_k sum_c plane_k[c] * line_k[c] at the vertices of the box, in float64 -> (D, sum_k sum_c |plane*line|),
-    both [n_z, n_y, n_x]."""
-    xs, ys, zs = (torch.arange(lo[a], lo[a] + n[a]) for a in range(3))
-    P = [p.double().cpu()[0] for p in factors[0]]              # [C, G[m1], G[m0]]
-    L = [l.double().cpu()[0, :, :, 0] for l in factors[1]]     # [C, G[v]]
-    terms = (torch.einsum("cyx,cz->czyx", P[0][:, ys][:, :, xs], L[0][:, zs]),
-             torch.einsum("czx,cy->czyx", P[1][:, zs][:, :, xs], L[1][:, ys]),
-             torch.einsum("czy,cx->czyx", P[2][:, zs][:, :, ys], L[2][:, xs]))
-    return sum(t.sum(0) for t in terms), sum(t.abs().sum(0) for t in terms)
+def _d64(factors, lo, n, slab=16):
+    """sum_k sum_c plane_k[c] * line_k[c] at the vertices of the box, in float64 on the factors' device, ``slab`` z
+    planes at a time -> (D, sum_k sum_c |plane*line|), both [n_z, n_y, n_x] on the CPU."""
+    dev = factors[0][0].device
+    P = [p.double()[0] for p in factors[0]]                    # [C, G[m1], G[m0]]
+    L = [l.double()[0, :, :, 0] for l in factors[1]]           # [C, G[v]]
+    xs, ys = (torch.arange(lo[a], lo[a] + n[a], device=dev) for a in range(2))
+    D = torch.empty(n[2], n[1], n[0], dtype=torch.float64, device=dev)
+    mag = torch.empty_like(D)
+    for z0 in range(0, n[2], slab):
+        zs = torch.arange(lo[2] + z0, lo[2] + min(n[2], z0 + slab), device=dev)
+        terms = (torch.einsum("cyx,cz->czyx", P[0][:, ys][:, :, xs], L[0][:, zs]),
+                 torch.einsum("czx,cy->czyx", P[1][:, zs][:, :, xs], L[1][:, ys]),
+                 torch.einsum("czy,cx->czyx", P[2][:, zs][:, :, ys], L[2][:, xs]))
+        D[z0:z0 + zs.numel()] = sum(t.sum(0) for t in terms)
+        mag[z0:z0 + zs.numel()] = sum(t.abs().sum(0) for t in terms)
+    return D.cpu(), mag.cpu()
 
 
 def _built(model):
@@ -54,6 +61,7 @@ def _built(model):
 
 
 def _check_against_f64(factors, lo, n, got):
+    """-> the largest err / bound"""
     want, mag = _d64(factors, lo, n)
     # recursive fp32 summation of 3 x 16 products (each rounded): |err| <= (16 + 2) * u * sum|terms|, u = eps32 / 2;
     # c = 18 with eps32 leaves a factor 2 of slack and does not depend on the summation order
@@ -61,6 +69,7 @@ def _check_against_f64(factors, lo, n, got):
     err = (got.double() - want).abs()
     assert bool((err <= bound).all()), float((err - bound).max())
     assert float(want.abs().max()) > 0
+    return float((err / bound.clamp_min(1e-300)).max())
 
 
 @pytest.fixture(scope="module", params=("A", "B"))
@@ -147,9 +156,13 @@ def _compare(a, b, w_rtol):
     assert d_ind <= 1e-4
 
 
-def _lego_inputs(grid=128, n_rays=1024):
+def _lego_inputs(grid=128, n_rays=1024, m=None):
+    """A lego model (``m``, or make_lego_model(grid)) and the surface points, normals and light ids its own forward
+    gives on a training batch, with the step's 512 stratified directions."""
     from tensoir_b200.synthetic import make_lego_model, hemisphere_poses, training_batch, n_samples_for
-    m = make_lego_model(grid, DEV)
+    if m is None:
+        m = make_lego_model(grid, DEV)
+    grid = int(m.gridSize[0])
     rays, li = (t.to(DEV) for t in training_batch(hemisphere_poses(100), n_rays, 3))
     with torch.no_grad():
         out = m(rays, li, is_train=False, is_relight=True, N_samples=n_samples_for(grid))
@@ -172,13 +185,16 @@ def _shrunk_inputs(fx, m):
     return pts.to(DEV), nrm.to(DEV), li.to(DEV), dirs.to(DEV).contiguous()
 
 
-def test_volume_path_matches_factor_path_on_the_bench_scene():
-    m, surf, nrm, li, dirs = _lego_inputs()
+def volume_path_matches_factor_path(m, surf, nrm, li, dirs):
     assert dirs.shape[0] == 512 and surf.shape[0] > 50
     fac = _march(m, surf, nrm, li, dirs, 96, use_vol=False)
     vol = _march(m, surf, nrm, li, dirs, 96)
     assert fac["cnt"]["density"] > 10000 and fac["cnt"]["app"] > 1000
     _compare(vol, fac, W_RTOL)
+
+
+def test_volume_path_matches_factor_path_on_lego_128():
+    volume_path_matches_factor_path(*_lego_inputs())
 
 
 def test_volume_path_matches_factor_path_on_shrunk_states(shrunk):
@@ -220,9 +236,14 @@ def test_sub_box_holds_every_vertex_a_valid_sample_reads(scene):
         fx = load_shrunk_state(scene)
         m = model_from_fixture(fx, DEV)
         pts, nrm, li, dirs = _shrunk_inputs(fx, m)
+    sub_box_holds_every_vertex_a_valid_sample_reads(m, pts, nrm, li, dirs, proper=scene == "lego")
+
+
+def sub_box_holds_every_vertex_a_valid_sample_reads(m, pts, nrm, li, dirs, proper):
+    """``proper``: the extent must be smaller than the grid"""
     lo, n, _ = _built(m)
     assert all(n[a] >= 1 for a in range(3))
-    if scene == "lego":
+    if proper:
         assert n != _grid(m)                                    # the box really is a sub-box here
     sub = _march(m, pts, nrm, li, dirs, 96)
     v_full, buf_full = _whole_grid_volume(m)

@@ -132,13 +132,15 @@ def _random_model(opaque):
 _SCENES = {}
 
 
-def scene(name):
-    """-> (Scene, surface points, normals, light indices) with at least 3x the largest dense grid of points."""
-    if name not in _SCENES:
+def scene(name, lego=None):
+    """-> (Scene, surface points, normals, light indices) with at least 3x the largest dense grid of points.  ``lego``:
+    the lego model of the "lego" scene (default: make_lego_model(128)); its surface points come from its own forward."""
+    key = name if lego is None else (name, id(lego))
+    if key not in _SCENES:
         from gpu_helpers import load_shrunk_state, model_from_fixture
         n = 3 * dense_grid(True) + 64
         if name == "lego":
-            m, surf, nrm, li, _ = _lego_inputs(n_rays=4096)
+            m, surf, nrm, li, _ = _lego_inputs(n_rays=4096, m=lego)
             reps = -(-n // surf.shape[0])
             pts, nrm, li = surf.repeat(reps, 1)[:n], nrm.repeat(reps, 1)[:n], li.repeat(reps)[:n]
         else:
@@ -154,8 +156,8 @@ def scene(name):
             nrm[a:b] = 0.0
         pts[7:12] = m.aabb[1].float() * 1.3
         pts[12] = m.aabb[0].float() * 1.1
-        _SCENES[name] = (Scene(m, name), pts.contiguous(), nrm.contiguous(), li.reshape(-1).to(torch.int32).contiguous())
-    return _SCENES[name]
+        _SCENES[key] = (Scene(m, name), pts.contiguous(), nrm.contiguous(), li.reshape(-1).to(torch.int32).contiguous())
+    return _SCENES[key]
 
 
 def stratified_dirs(sc, n_dirs):

@@ -34,13 +34,19 @@ VEC = O.VEC_MODE
 
 class Field:
     """Random VM factors in the reference's NCHW layout plus the channel-last copies and the TirField the kernels
-    read."""
+    read.  ``model``: take the factors of that TensorVMSplit (and its grid) instead."""
 
-    def __init__(self, seed=0):
+    def __init__(self, seed=0, model=None):
         from tensoir_b200 import _lib
         g = torch.Generator().manual_seed(seed)
         self.dplane, self.dline, self.aplane, self.aline = [], [], [], []
+        self.grid = GRID if model is None else tuple(int(x) for x in model.gridSize)
         for k in range(3):
+            if model is not None:
+                for name, src in (("dplane", model.density_plane), ("dline", model.density_line),
+                                  ("aplane", model.app_plane), ("aline", model.app_line)):
+                    getattr(self, name).append(src[k].detach().float().cpu())
+                continue
             W, H, D = GRID[MAT[k][0]], GRID[MAT[k][1]], GRID[VEC[k]]
             self.dplane.append(torch.randn(1, 16, H, W, generator=g))
             self.dline.append(torch.randn(1, 16, D, 1, generator=g))
@@ -52,7 +58,7 @@ class Field:
         for k in range(3):
             s.dplane[k], s.dline[k] = self.cl["dplane"][k].data_ptr(), self.cl["dline"][k].data_ptr()
             s.aplane[k], s.aline[k] = self.cl["aplane"][k].data_ptr(), self.cl["aline"][k].data_ptr()
-            s.grid[k] = GRID[k]
+            s.grid[k] = self.grid[k]
         s.dC, s.aC = 16, 48
         self.struct = s
 
@@ -60,7 +66,7 @@ class Field:
         """OracleField of the same factors (|factors| when ``absolute``) on the GPU in ``dtype``."""
         def cp(ts):
             return [(t.abs() if absolute else t).clone() for t in ts]
-        f = O.OracleField(aabb=torch.tensor([[-1.0] * 3, [1.0] * 3]), grid_size=list(GRID),
+        f = O.OracleField(aabb=torch.tensor([[-1.0] * 3, [1.0] * 3]), grid_size=list(self.grid),
                           density_plane=cp(self.dplane), density_line=cp(self.dline), app_plane=cp(self.aplane),
                           app_line=cp(self.aline), basis_w=None, mlp_rgb=None)
         return f.to(DEV, dtype)
@@ -159,6 +165,7 @@ def bound(mag, unit, n_add=None, grid=GRID):
 
 
 def check(got, want, bnd, what):
+    """-> the largest err / bound"""
     got, want = got.detach().double().reshape(want.shape), want.detach().double()
     err = (got - want).abs()
     ratio = err / bnd.reshape(want.shape).clamp_min(1e-30)
@@ -166,11 +173,14 @@ def check(got, want, bnd, what):
     worst = int(ratio.reshape(-1).argmax())
     assert float(ratio.max()) <= 1.0, (what, float(ratio.max()), float(err.reshape(-1)[worst]),
                                        float(want.reshape(-1)[worst]), float(bnd.reshape(-1)[worst]))
+    return float(ratio.max())
 
 
 def check_scatter(gp_got, gl_got, want_p, want_l, mags, units, what, grid=GRID):
-    """Parameter gradients (channel-last [H,W,C] / [D,1,C] from the kernel) against the float64 NCHW gradients."""
+    """Parameter gradients (channel-last [H,W,C] / [D,1,C] from the kernel) against the float64 NCHW gradients.
+    -> the largest err / bound"""
     gp_n, gl_n = as_param_layout(gp_got, gl_got)
+    worst = 0.0
     for k in range(3):
         mp, ml, cp, cl = mags[k]
         up, ul = units[k][0], units[k][1]
@@ -179,8 +189,9 @@ def check_scatter(gp_got, gl_got, want_p, want_l, mags, units, what, grid=GRID):
         D = want_l[k].shape[2]
         bp = bound(mp, up, cp[:, None], grid).t().reshape(1, C_, H, W)
         bl = bound(ml, ul, cl[:, None], grid).t().reshape(1, C_, D, 1)
-        check(gp_n[k], want_p[k], bp, f"{what} plane {k}")
-        check(gl_n[k], want_l[k], bl, f"{what} line {k}")
+        worst = max(worst, check(gp_n[k], want_p[k], bp, f"{what} plane {k}"),
+                    check(gl_n[k], want_l[k], bl, f"{what} line {k}"))
+    return worst
 
 
 # ------------------------------------------------------------------------------------------------------------------

@@ -17,6 +17,7 @@ pytestmark = pytest.mark.gpu
 
 DEV = V.DEV
 RUNS = [1, 2, 31, 32, 33, 64, 65]
+CHUNK = 1 << 16
 
 
 def _cell(g, lo=0.15, hi=0.85):
@@ -65,14 +66,16 @@ def zero_weight_runs(seed):
     return torch.cat(rows)
 
 
-def lego_valid_list():
-    """the valid-sample list of 256 rays of the bench's lego field at 128^3, in ray order"""
+def lego_valid_list(m=None, n_rays=256):
+    """the valid-sample list of ``n_rays`` rays of a training batch on the lego field ``m`` (default: the bench's lego
+    field at 128^3), in ray order"""
     from tensoir_b200 import vm_autograd as vm
     from tensoir_b200.synthetic import hemisphere_poses, make_lego_model, n_samples_for, training_batch
-    m = make_lego_model(128, torch.device(DEV))
-    rays, _ = training_batch(hemisphere_poses(100), 256, 0)
+    if m is None:
+        m = make_lego_model(128, torch.device(DEV))
+    rays, _ = training_batch(hemisphere_poses(100), n_rays, 0)
     rays = rays.to(DEV).float()
-    ref = vm.valid_samples(m, rays[:, :3], rays[:, 3:6], n_samples=n_samples_for(128))
+    ref = vm.valid_samples(m, rays[:, :3], rays[:, 3:6], n_samples=n_samples_for(int(m.gridSize[0])))
     return ref["xn"].float().cpu()
 
 
@@ -108,11 +111,56 @@ def field():
     return V.Field(0)
 
 
-@pytest.mark.parametrize("case", CASES)
-def test_density_bwd_runs(field, case):
+def scatter_reference(field, kind, x, g, gp, gl, what):
+    """The density ("density": g [n]) or appearance-products ("app": g [n, 144]) scatter the kernel wrote into gp / gl
+    against float64 autograd of the gather, with test_vm_kernels_fp64's bound; the reference runs in chunks of CHUNK
+    rows, so lists of a training step fit.  -> the largest err / bound"""
+    planes_of = (lambda f: (f.density_plane, f.density_line)) if kind == "density" else \
+        (lambda f: (f.app_plane, f.app_line))
+    C_ = 16 if kind == "density" else 48
+    with V.f64():
+        f = field.oracle(torch.float64)
+        planes, lines = planes_of(f)
+        for p in planes + lines:
+            p.requires_grad_(True)
+        mags = units = None
+        for a in range(0, x.shape[0], CHUNK):
+            xs = x[a:a + CHUNK].to(DEV, torch.float64)
+            gc = g[a:a + CHUNK].to(DEV).double()
+            if kind == "density":
+                (O.density_feature(f, xs) * gc).sum().backward()
+                ga = gc.abs()[:, None]
+
+                def coef_p(k, t, j):
+                    return ga * t["ptaps"][j][1][:, None] * t["AL"]
+
+                def coef_l(k, t, j):
+                    return ga * t["ltaps"][j][1][:, None] * t["AP"]
+            else:
+                ps, ls = O._app_products(f, xs)
+                (ps * ls).t().backward(gc)
+                ga = gc.abs().view(-1, 3, 48)
+
+                def coef_p(k, t, j):
+                    return ga[:, k] * t["ptaps"][j][1][:, None] * t["AL"]
+
+                def coef_l(k, t, j):
+                    return ga[:, k] * t["ltaps"][j][1][:, None] * t["AP"]
+            with torch.no_grad():
+                m = V.scatter(V.tap_sums(planes, lines, xs, False, False, field.grid), coef_p, coef_l, C_)
+                u = V.scatter(V.tap_sums(planes, lines, xs, False, True, field.grid), coef_p, coef_l, C_)
+            mags = m if mags is None else [tuple(p + q for p, q in zip(A, B)) for A, B in zip(mags, m)]
+            units = u if units is None else [tuple(p + q for p, q in zip(A, B)) for A, B in zip(units, u)]
+        return V.check_scatter(gp, gl, [p.grad for p in planes], [l_.grad for l_ in lines], mags, units, what,
+                               field.grid)
+
+
+def density_bwd(field, x, what):
+    """tir_vm_density_bwd on the rows x (every 7th upstream gradient 0: skipped rows inside runs) against float64
+    -> the largest err / bound"""
     from tensoir_b200 import _lib
     lib = _lib.load()
-    x = points(case).float()
+    x = x.float()
     xd = x.to(DEV).contiguous()
     n = x.shape[0]
     g = torch.randn(n, generator=torch.Generator().manual_seed(n + 1))
@@ -122,28 +170,14 @@ def test_density_bwd_runs(field, case):
     _lib.check(lib.tir_vm_density_bwd(C.byref(field.struct), _lib.dptr(xd), n, _lib.dptr(gd), ap, al,
                                       _lib.stream_ptr()), "density bwd")
     torch.cuda.synchronize()
-    with V.f64():
-        f = field.oracle(torch.float64)
-        for p in f.density_plane + f.density_line:
-            p.requires_grad_(True)
-        xs = x.to(DEV, torch.float64)
-        (O.density_feature(f, xs) * gd.double()).sum().backward()
-        ts = V.tap_sums(f.density_plane, f.density_line, xs, False, False)
-        tu = V.tap_sums(f.density_plane, f.density_line, xs, False, True)
-        ga = gd.double().abs()[:, None]
-        m = V.scatter(ts, lambda k, t, j: ga * t["ptaps"][j][1][:, None] * t["AL"],
-                      lambda k, t, j: ga * t["ltaps"][j][1][:, None] * t["AP"], 16)
-        u = V.scatter(tu, lambda k, t, j: ga * t["ptaps"][j][1][:, None] * t["AL"],
-                      lambda k, t, j: ga * t["ltaps"][j][1][:, None] * t["AP"], 16)
-        V.check_scatter(gp, gl, [p.grad for p in f.density_plane], [l.grad for l in f.density_line], m, u,
-                        f"density bwd {case}")
+    return scatter_reference(field, "density", x, gd, gp, gl, f"density bwd {what}")
 
 
-@pytest.mark.parametrize("case", CASES)
-def test_app_products_bwd_runs(field, case):
+def app_products_bwd(field, x, what):
+    """tir_vm_app_products_bwd on the rows x against float64 -> the largest err / bound"""
     from tensoir_b200 import _lib
     lib = _lib.load()
-    x = points(case).float()
+    x = x.float()
     xd = x.to(DEV).contiguous()
     n = x.shape[0]
     gout = torch.randn(n, 144, generator=torch.Generator().manual_seed(n)).to(DEV)
@@ -151,22 +185,17 @@ def test_app_products_bwd_runs(field, case):
     _lib.check(lib.tir_vm_app_products_bwd(C.byref(field.struct), _lib.dptr(xd), n, _lib.dptr(gout), ap, al,
                                            _lib.stream_ptr()), "app products bwd")
     torch.cuda.synchronize()
-    with V.f64():
-        f = field.oracle(torch.float64)
-        for p in f.app_plane + f.app_line:
-            p.requires_grad_(True)
-        xs = x.to(DEV, torch.float64)
-        ps, ls = O._app_products(f, xs)
-        (ps * ls).t().backward(gout.double())
-        ts = V.tap_sums(f.app_plane, f.app_line, xs, False, False)
-        tu = V.tap_sums(f.app_plane, f.app_line, xs, False, True)
-        ga = gout.double().abs().view(n, 3, 48)
-        m = V.scatter(ts, lambda k, t, j: ga[:, k] * t["ptaps"][j][1][:, None] * t["AL"],
-                      lambda k, t, j: ga[:, k] * t["ltaps"][j][1][:, None] * t["AP"], 48)
-        u = V.scatter(tu, lambda k, t, j: ga[:, k] * t["ptaps"][j][1][:, None] * t["AL"],
-                      lambda k, t, j: ga[:, k] * t["ltaps"][j][1][:, None] * t["AP"], 48)
-        V.check_scatter(gp, gl, [p.grad for p in f.app_plane], [l.grad for l in f.app_line], m, u,
-                        f"app products bwd {case}")
+    return scatter_reference(field, "app", x, gout, gp, gl, f"app products bwd {what}")
+
+
+@pytest.mark.parametrize("case", CASES)
+def test_density_bwd_runs(field, case):
+    density_bwd(field, points(case), case)
+
+
+@pytest.mark.parametrize("case", CASES)
+def test_app_products_bwd_runs(field, case):
+    app_products_bwd(field, points(case), case)
 
 
 @pytest.mark.parametrize("case", [c for c in CASES if c != "zero-weight"])
